@@ -1,16 +1,20 @@
-"""Pre-build the reference's three JIT CUDA plugins (bias_act, upfirdn2d, filtered_lrelu) for sm_100 in the build container,
-into the directory layout `torch_utils/custom_ops.get_plugin` (custom_ops.py:61-157) will look for on the GPU box:
-TORCH_EXTENSIONS_DIR/<plugin>/<md5 of sources>-nvidia-b200/.  Same sources (copied verbatim by install_ref.sh), same flags
-(`--use_fast_math`, the only flag the reference passes).  If ninja decides on the box that something is stale it simply
-rebuilds (~40 s per plugin) - this only saves GPU-box minutes.
+"""Pre-build the reference's three JIT CUDA plugins (bias_act, upfirdn2d, filtered_lrelu) for an H100 on a machine without a
+GPU, into the directory layout `torch_utils/custom_ops.get_plugin` (custom_ops.py:61-157) looks for:
+TORCH_EXTENSIONS_DIR/<plugin>/<md5 of sources>-<mangled GPU name>/.  Same sources (copied verbatim by install_ref.sh), same
+flags (`--use_fast_math`, the only flag the reference passes) and the arch list get_plugin ends up with on a single H100:
+it clears TORCH_CUDA_ARCH_LIST, so torch derives '9.0+PTX' from the device.  If ninja decides on the GPU machine that
+something is stale it simply rebuilds (~40 s per plugin) - this only saves GPU minutes.
 
-    python baseline/prebuild_ref_plugins.py baseline/_ref baseline/_ref/_torch_ext
+    python baseline/prebuild_ref_plugins.py baseline/_ref baseline/_ref/_torch_ext [mangled GPU name]
+
+The GPU name defaults to custom_ops._get_mangled_gpu_name() of "NVIDIA H100 80GB HBM3"; pass the name of another card.
 """
 import os, sys, time, hashlib, shutil
-os.environ['TORCH_CUDA_ARCH_LIST'] = '10.0'
+os.environ['TORCH_CUDA_ARCH_LIST'] = '9.0+PTX'
 import torch, torch.utils.cpp_extension as ce
 REF = sys.argv[1]
 OUT = sys.argv[2]
+GPU = sys.argv[3] if len(sys.argv) > 3 else 'nvidia-h100-80gb-hbm3'
 os.environ['TORCH_EXTENSIONS_DIR'] = OUT
 src_dir = os.path.join(REF, '_train/eg3dc/src/torch_utils/ops')
 plugins = {
@@ -25,7 +29,7 @@ for name, (srcs, hdrs, flags) in plugins.items():
     for f in allf:
         h.update(open(f, 'rb').read())
     top = ce._get_build_directory(name, verbose=False)
-    bdir = os.path.join(top, f'{h.hexdigest()}-nvidia-b200')
+    bdir = os.path.join(top, f'{h.hexdigest()}-{GPU}')
     os.makedirs(bdir, exist_ok=True)
     for f in allf:
         shutil.copyfile(f, os.path.join(bdir, os.path.basename(f)))

@@ -9,7 +9,7 @@ texels) + ray generation + ImportanceRenderer.forward.  Synthetic data, random-i
     python bench.py [--gpus N] [--steps K] [--warmup W]           our arm (CUDA, one rank per GPU)
     python bench.py --impl reference [...]                        the reference's CPU algorithm (oracle port)
 
-Prints ONE JSON line (rank 0).  See DESIGN.md section "Measurement" for how every field is derived.
+Prints ONE JSON line (rank 0); DESIGN.md section "Measurement" says how each field is derived.  --dump-outputs DIR also saves the last timed step's outputs as DIR/<name>.npy.
 """
 from __future__ import annotations
 
@@ -31,9 +31,6 @@ UNIT = 'views/s'
 R, S, SF, P, C, VIEWS = 128, 96, 96, 512, 32, 8
 FLOP_PER_SAMPLE = 2 * 32 * 64 + 2 * 64 * 33            # 8,320 tensor-eligible FLOP (SURVEY 8d)
 BYTES_PER_VIEW = 3 * C * P * P * 4 + R * R * 37 * 4    # tri-plane read once + 37 floats/ray out
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the default fused kernel on this workload, from the committed
-# `ncu --set full` capture of the default bench command (profiles/r2_final_ws3_raw.csv: 632.8 MB read + 22.6 MB written)
-FUSED_TRAFFIC = 655.4e6
 
 
 # rendering_options of BASELINE configs[1] (train_eclustrousC.py:409-440 + eg3dc_v0.py:30-31,55-56)
@@ -45,7 +42,7 @@ def workload_config(n_gpus, mlp_mode='tc_3xbf16', planes='fp32'):
     return {'workload': f'{VIEWS} views/GPU x {R}x{R} rays x ({S}+{SF}) samples, {VIEWS} distinct 3x{C}x{P}x{P} fp32 tri-planes/GPU',
             'views_per_gpu': VIEWS, 'rays': R * R, 'samples_coarse': S, 'samples_importance': SF, 'plane': P,
             'decoder': '32-64-33 softplus', 'mlp_mode': mlp_mode, 'plane_storage': planes, 'parallelism': f'views sharded x{n_gpus}',
-            'l2': 'inputs (805 MB of tri-planes re-laid out every step) exceed the 126 MB L2; no explicit flush'}
+            'l2': 'inputs (805 MB of tri-planes re-laid out every step) exceed the 50 MB L2; no explicit flush'}
 
 
 def read_peaks():
@@ -54,11 +51,11 @@ def read_peaks():
             pk = json.load(f)
         return pk['hbm_gbs'], pk.get('bf16_tflops_sustained', pk['bf16_tflops']), 'measured (MEASURED_PEAKS.json, sustained)'
     except Exception:
-        return 6650.0, 1400.0, 'fallback (B200_PROFILING.md)'
+        return 3350.0, 989.0, 'H100 SXM data sheet (HBM3, dense BF16), not measured'
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = 'index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,' \
         'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
 
@@ -260,11 +257,14 @@ def run_ours(args):
     peer = pviews.PeerGather((VIEWS, R * R, 32), torch.float32, dev, dst=0) if gather_mode == 'p2p' else None
     step_no = [0]
 
+    last = {}
+
     def step():
         c2w, K = labels_dev[:, :16].view(-1, 4, 4), labels_dev[:, 16:25].view(-1, 3, 3)
         ro, rd = sampler(c2w, K, R)
         renderer._planes.key = None                                           # distinct tri-planes every step: redo the layout pass
         rgb, depth, wsum, xyz = renderer(planes, decoder, ro, rd, opts)
+        last.update(rgb=rgb, depth=depth, weights_sum=wsum, xyz=xyz)
         if gather_mode == 'nccl':
             dist.all_gather_into_tensor(gather_buf, rgb)
         elif gather_mode == 'p2p':
@@ -295,6 +295,8 @@ def run_ours(args):
         barrier()
         ms = e0.elapsed_time(e1)
         launches = _lib.launch_count() - n0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last)
     with torch.no_grad():
         # ---- per-kernel device time for the roofline (separate short run with event brackets enabled)
         L.p3d_profile_enable(1)
@@ -472,11 +474,8 @@ def run_ours(args):
             roof = {'bound': 'tensor', 'achieved': flops / (kern_ms * 1e-3) / 1e12, 'peak': tc_tf, 'unit': 'TFLOP/s'}
         else:
             roof = {'bound': 'hbm', 'achieved': byts / (kern_ms * 1e-3) / 1e9, 'peak': hbm_gbs, 'unit': 'GB/s'}
-        # dram__bytes_read.sum + dram__bytes_write.sum of one launch, from the committed `ncu --set full` capture of this
-        # command (profiles/r1_final_ws_raw.csv: 630.5 MB + 22.3 MB); only valid for the default kernel / workload
-        traffic = FUSED_TRAFFIC if (fused and args.planes == 'fp32' and os.environ.get('P3D_FUSED_IMPL', 'v5') == 'v5') else None
-        roof.update({'frac': roof['achieved'] / roof['peak'], 'traffic': traffic,
-                     'kernel': ('k_render_ws3' if os.environ.get('P3D_FUSED_IMPL', 'v5') == 'v5' else 'k_render_ws') if fused else 'k_sample_decode',
+        roof.update({'frac': roof['achieved'] / roof['peak'],
+                     'kernel': 'k_render_ws3' if fused else 'k_sample_decode',
                      'kernel_ms_per_launch': kern_ms,
                      'launches_timed': int(slot_n[slot]), 'peak_source': peak_src,
                      'step_breakdown_ms': {'sample_decode': slot_ms[0] / 3, 'importance': slot_ms[1] / 3, 'composite': slot_ms[2] / 3,
@@ -504,6 +503,15 @@ def run_ours(args):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, tensors):
+    """What the timed path returned in its last step, one float32 .npy per output (rgb feature image, depth, weights_sum,
+    xyz: about 19 MB for the default workload)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in tensors.items():
+        np.save(os.path.join(out_dir, f'{name}.npy'), t.detach().float().cpu().numpy())
 
 
 def run_e2e(L, _lib, planes, decoder, labels, opts, mlp_mode, args, barrier):
@@ -556,6 +564,7 @@ def main():
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--no-variants', action='store_true', help='skip the 48+48 / bf16 / fp32_simt context measurements')
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s outputs to DIR/<name>.npy (float32)')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference(args)

@@ -97,7 +97,7 @@ def main():
     cond = {}
     gain, r1_gamma = 1.0, 1.0
     # training mode 'Agrad': paste_params with grad_sample=True (loss_orthocondA.py:131-150); the thresholds of that mode select nothing
-    # on a random-weight generator (cf. profiles/r2_configs/c3p_compare.json), so the harness opens them up: mask = (weights > 0.5)
+    # on a random-weight generator, so the harness opens them up: mask = (weights > 0.5)
     paste_params = ({'mode': 'default', 'thresh_weight': 0.5, 'thresh_edges': 0.5, 'thresh_occ': 2.0, 'offset_occ': 0.01, 'thresh_dxyz': 10.0,
                      'grad_sample': True} if args.paste else None)
     lin = torch.linspace(0, 1, res)

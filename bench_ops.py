@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench_ops.py - HBM-roofline measurement of the three StyleGAN ops on the shapes panic3d's path hits
 (SURVEY.md section 8a12-a14).  Not the driver's bench (that is bench.py); this produces the per-op numbers quoted in
-DESIGN.md / profiles/.  One JSON line per case:
+One JSON line per case:
 
     {"op": ..., "case": ..., "dtype": ..., "ms": ..., "algorithmic_bytes": ..., "gbs": ..., "frac_of_hbm_peak": ...}
 
@@ -25,7 +25,7 @@ def hbm_peak():
     try:
         return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'], 'measured'
     except Exception:
-        return 6650.0, 'fallback'
+        return 3350.0, 'H100 SXM data sheet'
 
 
 def timeit(fn, flush_buf, iters=20, warm=5):
@@ -66,7 +66,7 @@ def main():
         from panic3d_b200.torch_utils.ops import bias_act, upfirdn2d, filtered_lrelu
     dev = torch.device('cuda:0')
     peak, src = hbm_peak()
-    flush = torch.zeros(192 * 1024 * 1024 // 4, device=dev)          # 192 MB > 126 MB L2
+    flush = torch.zeros(192 * 1024 * 1024 // 4, device=dev)          # 192 MB > 50 MB L2
     f4 = upfirdn2d.setup_filter([1, 3, 3, 1], device=dev)
     f12 = upfirdn2d.setup_filter(torch.hann_window(14)[1:-1].numpy(), device=dev)   # 12 taps, separable
     out = []

@@ -91,7 +91,7 @@ def main():
     try:
         peak, peak_src = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs'], 'measured'
     except Exception:
-        peak, peak_src = 6650.0, 'fallback'
+        peak, peak_src = 3350.0, 'H100 SXM data sheet'
     nbytes = N * S * S * 72 + N * R * R * 4 * (3 + 1 + 1 + 3 + 3)
     line = {'op': 'paste_front', 'impl': args.impl, 'views': N, 'render': R, 'image': S, 'algorithmic_bytes': nbytes, 'hbm_peak_gbs': peak,
             'hbm_peak_source': peak_src}

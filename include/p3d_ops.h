@@ -1,5 +1,5 @@
 /*
- * p3d_ops.h - C ABI of the B200-native StyleGAN custom ops (bias_act, upfirdn2d, filtered_lrelu).
+ * p3d_ops.h - C ABI of the H100-native StyleGAN custom ops (bias_act, upfirdn2d, filtered_lrelu).
  *
  * Each entry point replaces one pybind11 function of the reference's JIT plugins
  * (/root/reference/_train/eg3dc/src/torch_utils/ops/): same argument meaning, but plain device

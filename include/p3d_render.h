@@ -1,5 +1,5 @@
 /*
- * p3d_render.h - C ABI of the B200-native tri-plane volumetric renderer.
+ * p3d_render.h - C ABI of the H100-native tri-plane volumetric renderer.
  *
  * Drop-in boundary for the hot path of panic3d's EG3D-derived ray-marcher.  The
  * reference has NO native code on this path (it is ~60 eager PyTorch ops per
@@ -44,8 +44,8 @@ extern "C" {
 
 /* decoder arithmetic */
 #define P3D_MLP_FP32_SIMT   0  /* scalar FFMA, bit-for-bit-class fp32 (parity reference kernel) */
-#define P3D_MLP_TC_3XBF16   1  /* tcgen05 bf16 tensor cores, 3-pass split operands (fp32-class accuracy) */
-#define P3D_MLP_TC_BF16     2  /* tcgen05 bf16 single pass (fast mode; ~1e-2 abs) */
+#define P3D_MLP_TC_3XBF16   1  /* wgmma bf16 tensor cores, 3-pass split operands (fp32-class accuracy) */
+#define P3D_MLP_TC_BF16     2  /* wgmma bf16 single pass (fast mode; ~1e-2 abs) */
 
 typedef struct p3d_render_params {
     /* problem size */
@@ -110,7 +110,7 @@ int p3d_raygen_ortho(const float* rot, const float* dist, int32_t n_views, int32
 /* Scratch needed by p3d_render_forward for these params (bytes). */
 size_t p3d_render_workspace_bytes(const p3d_render_params* p);
 
-/* 1 when the fused tcgen05 renderer (mlp_mode P3D_MLP_TC_*) has a kernel for these params
+/* 1 when the fused tensor-core renderer (mlp_mode P3D_MLP_TC_*) has a kernel for these params
    (depth_resolution == depth_resolution_importance in {48, 96}, C=32, hidden 64, out 33, rays per view a multiple of
    384/S, 32-bit tap offsets), else 0: such configurations run on the fp32 SIMT kernels (P3D_MLP_FP32_SIMT).  The host
    mirror (ImportanceRenderer.mlp_mode = 'auto') uses this to pick the tensor-core path whenever it exists; an
@@ -168,7 +168,7 @@ int p3d_decode_points(const p3d_render_params* p, const void* planes,
                       float* out_rgb, float* out_sigma, void* stream);
 
 /* 1 when p3d_decode_points / p3d_volume_query have a tensor-core kernel for these params (mlp_mode P3D_MLP_TC_*: the
-   renderer's gather -> tcgen05 decoder pipeline streamed over the points; any point count), else 0 (fp32 SIMT kernels).
+   renderer's gather -> wgmma decoder pipeline streamed over the points; any point count), else 0 (fp32 SIMT kernels).
    The host mirror's mlp_mode = 'auto' uses it like p3d_render_fused_supported. */
 int p3d_decode_tc_supported(const p3d_render_params* p, int64_t n_points_total);
 

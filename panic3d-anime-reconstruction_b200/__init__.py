@@ -1,4 +1,4 @@
-"""panic3d_b200 - B200-native (sm_100a) implementation of panic3d's tri-plane volumetric
+"""panic3d_b200 - H100-native (sm_90a) implementation of panic3d's tri-plane volumetric
 rendering hot path behind the reference's own Python call surface.
 
 Layout (mirrors the reference tree under /root/reference/_train/eg3dc/src):

@@ -1,4 +1,4 @@
-"""Build recipe for lib/libp3d.so: plain nvcc, sm_100a only, in-tree output (so it travels to the GPU box)."""
+"""Build recipe for lib/libp3d.so: plain nvcc, sm_90a (H100), in-tree output next to the package."""
 from __future__ import annotations
 
 import glob
@@ -10,7 +10,8 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB = os.path.join(PKG, 'lib', 'libp3d.so')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+NVCC_FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
 
@@ -43,7 +44,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     nvcc = shutil.which('nvcc') or '/usr/local/cuda/bin/nvcc'
     if not os.path.exists(nvcc):
         raise RuntimeError('nvcc not found: cannot build libp3d.so')
-    objdir = os.path.join(PKG, '..', 'gpurun_out', '.obj')        # scratch: neither tracked nor shipped to the GPU box
+    objdir = os.path.join(PKG, 'lib', 'obj')                      # per-source objects (git-ignored build products)
     os.makedirs(objdir, exist_ok=True)
     headers = glob.glob(os.path.join(CSRC, '*.cuh')) + glob.glob(os.path.join(PKG, '..', 'include', '*.h')) + [os.path.abspath(__file__)]
     t_hdr = max(os.path.getmtime(h) for h in headers)
@@ -61,9 +62,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError('nvcc failed on %s' % os.path.basename(src))
         if verbose:
             print(out)
-    os.makedirs(os.path.dirname(LIB), exist_ok=True)       # lib/ holds only ignored artefacts: a fresh clone has no such directory
     tmp = LIB + '.tmp.%d' % os.getpid()
-    r = subprocess.run([nvcc, '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', tmp] + objs + ['-lz'],     # zlib: deflate + crc32 of the PNG writer (csrc/image_io.cu)
+    r = subprocess.run([nvcc] + ARCH + ['-shared', '-o', tmp] + objs + ['-lz'],     # zlib: deflate + crc32 of the PNG writer (csrc/image_io.cu)
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

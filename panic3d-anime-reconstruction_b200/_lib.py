@@ -9,7 +9,7 @@ import os
 import threading
 
 PKG = os.path.dirname(os.path.abspath(__file__))
-# P3D_LIBP3D: load another build of the library (A/B experiments: profiles/experiments/build_variants.py); default in-tree
+# P3D_LIBP3D: load another build of the library (A/B experiments); default in-tree
 LIB_PATH = os.environ.get('P3D_LIBP3D') or os.path.join(PKG, 'lib', 'libp3d.so')
 
 P3D_PLANES_EG3D, P3D_PLANES_PANIC3D = 0, 1

@@ -291,7 +291,7 @@ using namespace p3d;
 
 extern "C" {
 
-const char* p3d_version(void) { return "p3d-render-b200 0.1 (sm_100a)"; }
+const char* p3d_version(void) { return "p3d-render-b200 0.1 (sm_90a)"; }
 const char* p3d_last_error(void) { return g_err; }
 uint64_t p3d_launch_count(void) { return g_launches.load(); }
 
@@ -372,7 +372,7 @@ size_t p3d_render_workspace_bytes(const p3d_render_params* p) {
 int p3d_render_fused_supported(const p3d_render_params* p) {
     Geom g;
     if (!p || make_geom(p, &g)) return 0;
-    return (fused_ws3_supported(g) || fused_ws_supported(g)) ? 1 : 0;
+    return fused_ws3_supported(g) ? 1 : 0;
 }
 
 int p3d_decode_tc_supported(const p3d_render_params* p, int64_t n_points_total) {
@@ -403,16 +403,8 @@ int p3d_render_forward(const p3d_render_params* p, const void* planes, const flo
         return render_forward_v1(g, p, planes, w1, b1, w2, b2, ray_origins, ray_dirs, u_coarse, u_fine, ws, out_rgb,
                                  out_depth, out_wsum, out_xyz, (cudaStream_t)stream);
     if (p->mlp_mode == P3D_MLP_TC_3XBF16 || p->mlp_mode == P3D_MLP_TC_BF16) {
-        // P3D_FUSED_IMPL selects among the fused kernels for A/B runs (read once per process):
-        //   (default) "v5"  render_fused_ws3.cu  warp-specialised, pipeline depth 3, dedicated ray warps
-        //             "v3"  render_fused_ws.cu   warp-specialised, two ray groups in flight (round-1 design + the round-2 gather)
-        static const char* impl = getenv("P3D_FUSED_IMPL");
-        const char which = (impl && impl[0] == 'v') ? impl[1] : '5';
-        if (which == '5' && fused_ws3_supported(g))
-            return render_forward_fused_ws3(g, p, planes, w1, b1, w2, b2, ray_origins, ray_dirs, u_coarse, u_fine, ws, out_rgb,
-                                            out_depth, out_wsum, out_xyz, (cudaStream_t)stream);
-        return render_forward_fused_ws(g, p, planes, w1, b1, w2, b2, ray_origins, ray_dirs, u_coarse, u_fine, ws, out_rgb,
-                                       out_depth, out_wsum, out_xyz, (cudaStream_t)stream);     // P3D_EUNSUPPORTED when it has no kernel either
+        return render_forward_fused_ws3(g, p, planes, w1, b1, w2, b2, ray_origins, ray_dirs, u_coarse, u_fine, ws, out_rgb,
+                                        out_depth, out_wsum, out_xyz, (cudaStream_t)stream);     // P3D_EUNSUPPORTED without a kernel
     }
     set_error("mlp_mode %d has no kernel in this build", p->mlp_mode);
     return P3D_EUNSUPPORTED;

@@ -1,16 +1,15 @@
 // Streaming tensor-core decode of tri-plane points: p3d_decode_points (ImportanceRenderer.run_model, renderer.py:266-280) and
 // p3d_volume_query (get_eg3d_volume, _util/eg3d_metrics3d.py:94-183) when mlp_mode is P3D_MLP_TC_*.
 //
-// The renderer's gather -> tcgen05 decoder pipeline without any per-ray phase, so nothing ever waits on a dependency chain:
+// The renderer's gather -> tensor-core decoder pipeline without any per-ray phase, so nothing ever waits on a dependency chain:
 //
 //   warps  0-11  GATHER    three teams of four warps; team j takes tiles j, j+3, ... ; a warp owns 32 points of its tile:
 //                          position (given coordinates, or the reference's sheared voxel lattice generated in-kernel) -> tap
-//                          table -> 12 x 128-bit loads per lane -> packed-FMA lerp -> bf16 hi/lo A1 tile (4-stage ring)
-//   warps 12-19  EPILOGUE  tile t: tcgen05.ld D1 -> softplus2 -> A2 tile (double-buffered); tile t-1: tcgen05.ld D2 ->
-//                          sigma / sigmoid colours -> global (and, for the volume query, density with the crop / cull
-//                          overwrites and the lattice coordinates, written where the reference's reshape + flip puts them)
-//   warp  20     MMA       one thread: layer 1 (N = 64) and layer 2 (N = 48: 32 colour logits, sigma, 15 zero rows) as
-//                          3-pass split-bf16 tcgen05.mma; D1 single, D2 double-buffered in TMEM (160 columns)
+//                          table -> 12 x 128-bit loads per lane -> FMA lerp -> bf16 hi/lo A1 tile (4-stage ring)
+//   warps 12-19  DECODER   two warpgroups, one per 64-row half of every tile: layer 1 (wgmma, A1 and W1 from shared memory)
+//                          -> softplus2 in registers -> layer 2 (wgmma, N = 48: 32 colour logits, sigma, 15 zero rows; A from
+//                          the registers) -> sigma / sigmoid colours -> global (and, for the volume query, density with the crop
+//                          / cull overwrites and the lattice coordinates, written where the reference's reshape + flip puts them)
 //
 // A tile is 128 consecutive points; CTA b of the persistent grid takes tiles b, b + grid, ...
 #include <stdlib.h>
@@ -24,22 +23,18 @@ using namespace dev;
 using namespace fused;
 
 constexpr int kGW = 12, kEW = 8, kTeams = 3;
-constexpr int kWarpsD = kGW + kEW + 1;
-constexpr int kThreadsD = kWarpsD * 32;          // 672
+constexpr int kWarpsD = kGW + kEW;
+constexpr int kThreadsD = kWarpsD * 32;          // 640
 constexpr int kNA = 4;                           // A1 ring depth
-constexpr int kTmemColsD = 256;
-constexpr int kColD1 = 0, kColD2 = 64, kD2Cols = 48;   // D2[b] = 64 + 48 b
-constexpr int kLBO_A = 2048, kLBO_A1 = 2080, kLBO_W1 = 1024, kLBO_W2 = 768;
+constexpr int kD2Cols = 48;
+constexpr int kLBO_A1 = 2080, kLBO_W1 = 1024, kLBO_W2 = 768;
 
 struct __align__(1024) DecSmem {
     unsigned char a1[kNA][2][4 * kLBO_A1];
-    unsigned char a2[2][2][16384];
     unsigned char w1[2][4096], w2[2][6144];
     float b1[kHidden], b2c[kRgb], b2s, pad0[3];
     uint4 tab[kGW][32][4];
-    unsigned long long a1_full[kNA], a1_empty[kNA], a2_full[2], a2_empty[2];
-    unsigned long long d1_full, d1_empty, d2_full[2], d2_empty[2];
-    unsigned int tmem_base, pad1;
+    unsigned long long a1_full[kNA], a1_empty[kNA];
 };
 
 struct DecArgs {
@@ -83,17 +78,8 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const int n_my = (a.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles of this CTA
 
-    if (warp == kWarpsD - 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "r"(kTmemColsD) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (tid == 0) {
-        for (int i = 0; i < kNA; ++i) { mbar_init(&sm.a1_full[i], 4); mbar_init(&sm.a1_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&sm.a2_full[i], kEW); mbar_init(&sm.a2_empty[i], 1);
-            mbar_init(&sm.d2_full[i], 1); mbar_init(&sm.d2_empty[i], kEW);
-        }
-        mbar_init(&sm.d1_full, 1); mbar_init(&sm.d1_empty, kEW);
+        for (int i = 0; i < kNA; ++i) { mbar_init(&sm.a1_full[i], 4); mbar_init(&sm.a1_empty[i], kEW); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = tid; i < kHidden * kC; i += kThreadsD) {             // W1' = W1 * gain * log2(e) / 3   (64 x 32)
@@ -117,10 +103,7 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
     if (tid < kRgb) sm.b2c[tid] = -__fmul_rn(a.b2[tid + 1], g.b2_gain) * kLog2e;
     if (tid == 0) sm.b2s = __fmul_rn(a.b2[0], g.b2_gain);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm.tmem_base;
 
     if (warp < kGW) {
         // =========================================================================== GATHER
@@ -187,17 +170,13 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
                 const float4 w0 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 1));
                 const float4 w1 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 2));
                 const float4 w2 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 3));
-                unsigned long long acc[2] = {0ull, 0ull};
+                float acc[4] = {0.f, 0.f, 0.f, 0.f};
                 fma4(acc, v4[0], w0.x); fma4(acc, v4[1], w0.y); fma4(acc, v4[2], w0.z); fma4(acc, v4[3], w0.w);
                 fma4(acc, v4[4], w1.x); fma4(acc, v4[5], w1.y); fma4(acc, v4[6], w1.z); fma4(acc, v4[7], w1.w);
                 fma4(acc, v4[8], w2.x); fma4(acc, v4[9], w2.y); fma4(acc, v4[10], w2.z); fma4(acc, v4[11], w2.w);
                 uint32_t h[2], l[2];
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    float e0, e1;
-                    upk2(acc[j], e0, e1);
-                    split2(e0, e1, h[j], l[j]);
-                }
+                split2(acc[0], acc[1], h[0], l[0]);
+                split2(acc[2], acc[3], h[1], l[1]);
                 const int trow = wt * 32 + lrow;
                 const int off = (trow >> 3) * kSBO + (qd >> 1) * kLBO_A1 + (trow & 7) * 16 + (qd & 1) * 8;
                 *reinterpret_cast<uint2*>(a1h + off) = make_uint2(h[0], h[1]);
@@ -207,152 +186,70 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
             __syncwarp();
             if (lane == 0) mbar_arrive(&sm.a1_full[stage]);
         }
-    } else if (warp < kGW + kEW) {
-        // =========================================================================== EPILOGUE
-        const int e = warp - kGW, quarter = e & 3, chunk = e >> 2;
-        const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-        // layer-2 result of tile it2 -> outputs.  chunk 0: colours [0,16) + sigma (+ density); chunk 1: colours [16,32) (+ coordinates)
-        auto epilogue2 = [&](int it2) {
-            const int db = it2 & 1;
-            mbar_wait(&sm.d2_full[db], (it2 >> 1) & 1);
-            tc_fence_after();
-            float v[16];
-            tmem_ld16(tmem + kColD2 + db * kD2Cols + 16 * chunk + lane_base, v);
-            float sg = 0.f;
-            if (chunk == 0) sg = tmem_ld1(tmem + kColD2 + db * kD2Cols + kRgb + lane_base) + sm.b2s;
-            tc_fence_before();
+    } else {
+        // =========================================================================== DECODER (two warpgroups)
+        const int e = warp - kGW, half = e >> 2, w = e & 3;
+        const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]), w2h = smem_u32(sm.w2[0]), w2l = smem_u32(sm.w2[1]);
+        for (int it = 0; it < n_my; ++it) {
+            const int stage = it % kNA;
+            mbar_wait(&sm.a1_full[stage], (it / kNA) & 1);
+            float d1[32];
+            decoder_layer1(d1, smem_u32(sm.a1[stage][0]), smem_u32(sm.a1[stage][1]), kLBO_A1, w1h, w1l, kLBO_W1, half, a.single_pass);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.d2_empty[db]);
-            const long long tile = (long long)blockIdx.x + (long long)it2 * gridDim.x;
-            const long long gidx = tile * 128 + quarter * 32 + lane;
-            if (gidx >= a.total) return;
-            long long dest = gidx, n = 0;
-            if (VOLUME) {
-                const long long view = gidx / a.per_view;
-                n = gidx - view * a.per_view;
-                dest = view * a.per_view + volume_dest(n, a.vol_res);
-            }
-            if (a.out_rgb) {
-                float4* dst = reinterpret_cast<float4*>(a.out_rgb + dest * kRgb + 16 * chunk);
+            if (lane == 0) mbar_arrive(&sm.a1_empty[stage]);
+            uint32_t ah[16], al[16];
+            decoder_hidden(d1, sm.b1, lane, ah, al);
+            float d2[kD2Cols / 2];
+            decoder_layer2_issue<kD2Cols>(d2, ah, al, w2h, w2l, kLBO_W2, a.single_pass);
+            wgmma_commit();
+            wgmma_wait_all();
+            fence_operands(d2);
+            // this thread's two rows (fragment elements 2 rs, 2 rs + 1 of each 8-column block): colours [0, 32) in column
+            // pairs, sigma = column 32 (lanes with l % 4 == 0), the volume lattice coordinates from the l % 4 == 1 lanes
+            const long long tile = (long long)blockIdx.x + (long long)it * gridDim.x;
 #pragma unroll
-                for (int c4 = 0; c4 < 4; ++c4) {
-                    float o[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float s = rcp_approx(1.f + ex2_approx(v[4 * c4 + j] + sm.b2c[16 * chunk + 4 * c4 + j]));
-                        o[j] = g.force_sigmoid ? s : __fsub_rn(__fmul_rn(s, 1.002f), 0.001f);
-                    }
-                    dst[c4] = make_float4(o[0], o[1], o[2], o[3]);
+            for (int rs = 0; rs < 2; ++rs) {
+                const long long gidx = tile * 128 + 64 * half + frag_row(2 * rs, lane, w);
+                if (gidx >= a.total) continue;
+                long long dest = gidx, n = 0;
+                if (VOLUME) {
+                    const long long view = gidx / a.per_view;
+                    n = gidx - view * a.per_view;
+                    dest = view * a.per_view + volume_dest(n, a.vol_res);
                 }
-            }
-            if (chunk == 0) {
-                a.out_sigma[dest] = sg;
-                if (VOLUME && a.out_density) {
-                    // sigma2density, then the crop / cull overwrites; the reference applies cull_clouds_mask to the DENSITIES
-                    // (eg3d_metrics3d.py:155-162 -> renderer.py:150-153): the threshold acts on the twice-transformed value
+                if (a.out_rgb) {
+#pragma unroll
+                    for (int blk = 0; blk < 4; ++blk) {
+                        const int i = 4 * blk + 2 * rs, c = frag_col(i, lane);
+                        float o[2];
+#pragma unroll
+                        for (int j = 0; j < 2; ++j) {
+                            const float s = rcp_approx(1.f + ex2_approx(d2[i + j] + sm.b2c[c + j]));
+                            o[j] = g.force_sigmoid ? s : __fsub_rn(__fmul_rn(s, 1.002f), 0.001f);
+                        }
+                        *reinterpret_cast<float2*>(a.out_rgb + dest * kRgb + c) = make_float2(o[0], o[1]);
+                    }
+                }
+                if ((lane & 3) == 0) {
+                    const float sg = d2[16 + 2 * rs] + sm.b2s;
+                    a.out_sigma[dest] = sg;
+                    if (VOLUME && a.out_density) {
+                        // sigma2density, then the crop / cull overwrites; the reference applies cull_clouds_mask to the DENSITIES
+                        // (eg3d_metrics3d.py:155-162 -> renderer.py:150-153): the threshold acts on the twice-transformed value
+                        float x, y, z;
+                        volume_point(n, a.vol_res, a.vol_size, a.vol_origin, x, y, z);
+                        float dens = 1.f - expf(-softplus_t(__fsub_rn(sg, 1.f)));
+                        if (a.vol_crop_on && !((fabsf(x) <= a.vol_crop) && (fabsf(z) <= a.vol_crop))) dens = -1e3f;
+                        if (a.vol_cull_on && (1.f - expf(-softplus_t(__fsub_rn(dens, 1.f)))) < a.vol_cull) dens = -1e3f;
+                        a.out_density[dest] = dens;
+                    }
+                } else if (VOLUME && a.out_coords && (lane & 3) == 1) {
                     float x, y, z;
                     volume_point(n, a.vol_res, a.vol_size, a.vol_origin, x, y, z);
-                    float dens = 1.f - expf(-softplus_t(__fsub_rn(sg, 1.f)));
-                    if (a.vol_crop_on && !((fabsf(x) <= a.vol_crop) && (fabsf(z) <= a.vol_crop))) dens = -1e3f;
-                    if (a.vol_cull_on && (1.f - expf(-softplus_t(__fsub_rn(dens, 1.f)))) < a.vol_cull) dens = -1e3f;
-                    a.out_density[dest] = dens;
-                }
-            } else if (VOLUME && a.out_coords) {
-                float x, y, z;
-                volume_point(n, a.vol_res, a.vol_size, a.vol_origin, x, y, z);
-                a.out_coords[dest * 3 + 0] = x; a.out_coords[dest * 3 + 1] = y; a.out_coords[dest * 3 + 2] = z;
-            }
-        };
-        for (int it = 0; it < n_my; ++it) {
-            mbar_wait(&sm.d1_full, it & 1);
-            tc_fence_after();
-            float v[32];
-            tmem_ld32(tmem + kColD1 + lane_base + 32 * chunk, v);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.d1_empty);
-            const int buf = it & 1;
-            mbar_wait(&sm.a2_empty[buf], ((it >> 1) & 1) ^ 1);
-            {
-                const int trow = quarter * 32 + lane;
-                unsigned char* a2h = sm.a2[buf][0];
-                unsigned char* a2l = sm.a2[buf][1];
-#pragma unroll
-                for (int c8 = 0; c8 < 4; ++c8) {
-                    uint32_t ph[4], pl[4];
-#pragma unroll
-                    for (int x = 0; x < 4; ++x) {
-                        const int j = c8 * 8 + 2 * x;
-                        const unsigned long long x2 = add2(pk2(v[j], v[j + 1]), *reinterpret_cast<const unsigned long long*>(&sm.b1[32 * chunk + j]));
-                        float x0, x1;
-                        upk2(x2, x0, x1);
-                        const unsigned long long u2 = add2(pk2(ex2_approx(-fabsf(x0)), ex2_approx(-fabsf(x1))), pk2(1.f, 1.f));
-                        float u0, u1;
-                        upk2(u2, u0, u1);
-                        split2p(add2(pk2(fmaxf(x0, 0.f), fmaxf(x1, 0.f)), pk2(lg2_approx(u0), lg2_approx(u1))), ph[x], pl[x]);
-                    }
-                    const int off = tile_off(trow, 32 * chunk + 8 * c8, kLBO_A);
-                    *reinterpret_cast<uint4*>(a2h + off) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-                    *reinterpret_cast<uint4*>(a2l + off) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+                    a.out_coords[dest * 3 + 0] = x; a.out_coords[dest * 3 + 1] = y; a.out_coords[dest * 3 + 2] = z;
                 }
             }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.a2_full[buf]);
-            if (it > 0) epilogue2(it - 1);
         }
-        if (n_my > 0) epilogue2(n_my - 1);
-    } else {
-        // =========================================================================== MMA issuer (one thread)
-        if (lane == 0) {
-            const uint32_t idesc1 = umma_idesc(128, kHidden), idesc2 = umma_idesc(128, kD2Cols);
-            const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]), w2h = smem_u32(sm.w2[0]), w2l = smem_u32(sm.w2[1]);
-            auto layer2 = [&](int it2) {
-                const int buf = it2 & 1, db = it2 & 1;
-                mbar_wait(&sm.a2_full[buf], (it2 >> 1) & 1);
-                mbar_wait(&sm.d2_empty[db], ((it2 >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t a2h = smem_u32(sm.a2[buf][0]), a2l = smem_u32(sm.a2[buf][1]);
-                const uint32_t d2 = tmem + kColD2 + db * kD2Cols;
-#pragma unroll
-                for (int ks = 0; ks < kHidden / 16; ++ks) {
-                    const uint32_t ao = ks * 2 * kLBO_A, bo = ks * 2 * kLBO_W2;
-                    umma_bf16(d2, umma_desc(a2h + ao, kLBO_A, kSBO), umma_desc(w2h + bo, kLBO_W2, kSBO), idesc2, ks > 0);
-                    if (!a.single_pass) {
-                        umma_bf16(d2, umma_desc(a2h + ao, kLBO_A, kSBO), umma_desc(w2l + bo, kLBO_W2, kSBO), idesc2, 1);
-                        umma_bf16(d2, umma_desc(a2l + ao, kLBO_A, kSBO), umma_desc(w2h + bo, kLBO_W2, kSBO), idesc2, 1);
-                    }
-                }
-                umma_commit(&sm.d2_full[db]);
-                umma_commit(&sm.a2_empty[buf]);
-            };
-            for (int it = 0; it < n_my; ++it) {
-                const int stage = it % kNA;
-                mbar_wait(&sm.a1_full[stage], (it / kNA) & 1);
-                mbar_wait(&sm.d1_empty, (it & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t a1h = smem_u32(sm.a1[stage][0]), a1l = smem_u32(sm.a1[stage][1]);
-#pragma unroll
-                for (int ks = 0; ks < kC / 16; ++ks) {
-                    const uint32_t ao = ks * 2 * kLBO_A1, bo = ks * 2 * kLBO_W1;
-                    umma_bf16(tmem + kColD1, umma_desc(a1h + ao, kLBO_A1, kSBO), umma_desc(w1h + bo, kLBO_W1, kSBO), idesc1, ks > 0);
-                    if (!a.single_pass) {
-                        umma_bf16(tmem + kColD1, umma_desc(a1h + ao, kLBO_A1, kSBO), umma_desc(w1l + bo, kLBO_W1, kSBO), idesc1, 1);
-                        umma_bf16(tmem + kColD1, umma_desc(a1l + ao, kLBO_A1, kSBO), umma_desc(w1h + bo, kLBO_W1, kSBO), idesc1, 1);
-                    }
-                }
-                umma_commit(&sm.d1_full);
-                umma_commit(&sm.a1_empty[stage]);
-                if (it > 0) layer2(it - 1);
-            }
-            if (n_my > 0) layer2(n_my - 1);
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kWarpsD - 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemColsD) : "memory");
     }
 }
 

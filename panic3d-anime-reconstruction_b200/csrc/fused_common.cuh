@@ -1,5 +1,5 @@
-// PTX wrappers (mbarrier, tcgen05 MMA / TMEM, packed f32x2 arithmetic) and the tri-plane gather helpers shared by the fused
-// tensor-core kernels: render_fused_ws3.cu (the renderer) and decode_tc.cu (point / volume decode).
+// PTX wrappers (mbarrier, Hopper wgmma) and the tri-plane gather / decoder helpers shared by the fused tensor-core
+// kernels: render_fused_ws3.cu (the renderer) and decode_tc.cu (point / volume decode).
 #pragma once
 #include "render_device.cuh"
 
@@ -8,11 +8,8 @@ namespace fused {
 
 using namespace dev;
 
-constexpr int kSBO = 128;                        // byte distance between 8-row groups of a K-major no-swizzle UMMA tile
+constexpr int kSBO = 128;                        // byte distance between 8-row groups of a K-major no-swizzle wgmma operand tile
 constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
-#ifndef P3D_W3_WAIT
-#define P3D_W3_WAIT 0          // 0: try_wait with a suspend-time hint, bounded (traps on a protocol bug); 2: plain try_wait, bounded (measured slower)
-#endif
 
 // ------------------------------------------------------------------------------------------ PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -24,16 +21,6 @@ __device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
 }
 __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
-#if P3D_W3_WAIT == 2
-#pragma unroll 1
-    for (int it = 0; it < (1 << 24); ++it) {             // plain try_wait: the hardware's own suspend window per try; still bounded
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    asm volatile("trap;");
-#endif
     // (not unrolled: ptxas otherwise replicates the body 16x at each of the ~50 call sites - half of the kernel's code size)
 #pragma unroll 1
     for (int it = 0; it < (1 << 17); ++it) {             // ~20 us per try: the cap turns a protocol bug into a trap after ~2 s
@@ -47,55 +34,52 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t pari
     asm volatile("trap;");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// ---- warpgroup MMA (sm_90a).  Operands in shared memory use the K-major, no-swizzle canonical layout of tile_off():
+// 8-row x 16-byte core matrices, kSBO bytes between 8-row groups, `lbo` bytes between 8-column (16-byte) groups along K.
+// A warpgroup's accumulator fragment of m64nN: element i of thread (warp w, lane l) is row 16 w + l / 4 + 8 ((i / 2) & 1),
+// column 8 (i / 4) + 2 (l & 3) + (i & 1) - frag_row / frag_col below.  Columns [16 j, 16 j + 16) of it are, packed in pairs,
+// the register A operand of k-step j of the next layer (the accumulator layout equals the A-fragment layout).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
     uint64_t d = (uint64_t)((saddr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;
-    return d;
+    return d;                                          // base offset 0, layout type 0 (no swizzle)
 }
-__device__ __forceinline__ constexpr uint32_t umma_idesc(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ int frag_row(int i, int lane, int w) { return 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a_desc), "l"(b_desc), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void wgmma_rs_n8(float (&d)[4], const uint32_t* a, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %9, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0,%1,%2,%3}, {%4,%5,%6,%7}, %8, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t* a, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
 }
-__device__ __forceinline__ float tmem_ld1(uint32_t taddr) {
-    uint32_t r;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];\n\ttcgen05.wait::ld.sync.aligned;" : "=r"(r) : "r"(taddr) : "memory");
-    return __uint_as_float(r);
+__device__ __forceinline__ void wgmma_rs_n48(float (&d)[24], const uint32_t* a, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, {%24,%25,%26,%27}, %28, p, 1, 1, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
 }
+
 __device__ __forceinline__ uint32_t pack_bf16x2(float e0, float e1) {
     uint32_t d;
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(e1), "f"(e0));
@@ -140,35 +124,6 @@ __device__ __forceinline__ bool plane_taps_rec(const Geom& g, int srow, int scol
     w = make_float4(wl * wt, wr * wt, wl * wb, wr * wb);
     return ((unsigned)(dx + 1) < 3u) && ((unsigned)(dy + 1) < 3u);
 }
-// packed f32x2 arithmetic (one instruction for two lanes of data)
-__device__ __forceinline__ unsigned long long pk2(float a, float b) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(unsigned long long v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ unsigned long long add2(unsigned long long a, unsigned long long b) { unsigned long long r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) { unsigned long long r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) { unsigned long long r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) { unsigned long long r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-// lg2(1 + t) for t in [0, 1] on the FMA pipe, two values per instruction: t * q(t), q = degree-6 near-minimax fit of
-// lg2(1 + t) / t (max abs error 1.4e-6 in fp32 Horner form, exact 0 at t = 0).  Takes the second MUFU of every softplus off the
-// MUFU / MIO queue, which is what throttles the tile epilogue (ncu: mio_throttle on the softplus lines).
-__device__ __forceinline__ unsigned long long lg2_1p_poly2(unsigned long long t) {
-    unsigned long long q = fma2(t, pk2(0.020490340888500214f, 0.020490340888500214f), pk2(-0.09606623649597168f, -0.09606623649597168f));
-    q = fma2(t, q, pk2(0.2155885100364685f, 0.2155885100364685f));
-    q = fma2(t, q, pk2(-0.33924776315689087f, -0.33924776315689087f));
-    q = fma2(t, q, pk2(0.4777059257030487f, 0.4777059257030487f));
-    q = fma2(t, q, pk2(-0.721162736415863f, -0.721162736415863f));
-    q = fma2(t, q, pk2(1.4426932334899902f, 1.4426932334899902f));
-    return mul2(t, q);
-}
-// (h0, h1) -> bf16x2 hi word and bf16x2 lo word of the residuals, 4 instructions + the pack
-__device__ __forceinline__ void split2p(unsigned long long h2, uint32_t& hi, uint32_t& lo) {
-    float h0, h1;
-    upk2(h2, h0, h1);
-    hi = pack_bf16x2(h0, h1);
-    const unsigned long long r2 = sub2(h2, pk2(__uint_as_float(hi << 16), __uint_as_float(hi & 0xffff0000u)));
-    float r0, r1;
-    upk2(r2, r0, r1);
-    lo = pack_bf16x2(r0, r1);
-}
 // four consecutive channels of one texel (16 B fp32 / 8 B bf16) at addr + IMM bytes, predicated; v keeps its old value when !pred
 template <bool BF16, int IMM>
 __device__ __forceinline__ void load_quad_p(float (&v)[4], const char* addr, bool pred) {
@@ -182,14 +137,66 @@ __device__ __forceinline__ void load_quad_p(float (&v)[4], const char* addr, boo
                      : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]) : "l"(addr), "r"((int)pred), "n"(IMM));
     }
 }
-__device__ __forceinline__ void fma4(unsigned long long (&acc)[2], const float (&v)[4], float w) {
-    unsigned long long ww;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(ww) : "f"(w));
+__device__ __forceinline__ void fma4(float (&acc)[4], const float (&v)[4], float w) {
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        unsigned long long vv;
-        asm("mov.b64 %0, {%1, %2};" : "=l"(vv) : "f"(v[2 * j]), "f"(v[2 * j + 1]));
-        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[j]) : "l"(vv), "l"(ww));
+    for (int j = 0; j < 4; ++j) acc[j] = fmaf(v[j], w, acc[j]);
+}
+
+// ------------------------------------------------------------------------------------------ decoder (one warpgroup, 64 rows)
+// Layer 1 of rows [64 half, 64 half + 64) of a 128-row A1 tile (bf16 hi / lo planes, K = 32, `lbo_a` bytes between K groups):
+// D1 = A1 W1'^T as 3-pass split bf16 (hi hi + hi lo + lo hi), or hi hi alone when single_pass.
+__device__ __forceinline__ void decoder_layer1(float (&d1)[32], uint32_t a1h, uint32_t a1l, int lbo_a, uint32_t w1h, uint32_t w1l,
+                                               int lbo_w1, int half, bool single_pass) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d1[i] = 0.f;
+    const uint32_t ra = (uint32_t)half * 8 * kSBO;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+        const uint32_t ao = ra + ks * 2 * lbo_a, bo = ks * 2 * lbo_w1;
+        wgmma_ss_n64(d1, wgmma_desc(a1h + ao, lbo_a, kSBO), wgmma_desc(w1h + bo, lbo_w1, kSBO));
+        if (!single_pass) {
+            wgmma_ss_n64(d1, wgmma_desc(a1h + ao, lbo_a, kSBO), wgmma_desc(w1l + bo, lbo_w1, kSBO));
+            wgmma_ss_n64(d1, wgmma_desc(a1l + ao, lbo_a, kSBO), wgmma_desc(w1h + bo, lbo_w1, kSBO));
+        }
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(d1);
+}
+// softplus2(D1 + b1') -> the bf16 hi / lo register A operands of layer 2 (k-step j = registers [4 j, 4 j + 4)).
+// softplus2(x) = max(x, 0) + lg2(1 + 2^-|x|): no overflow for any x, so no threshold select.
+__device__ __forceinline__ void decoder_hidden(const float (&d1)[32], const float* b1, int lane, uint32_t (&ah)[16], uint32_t (&al)[16]) {
+#pragma unroll
+    for (int m = 0; m < 16; ++m) {
+        const int c = frag_col(2 * m, lane);
+        const float x0 = d1[2 * m] + b1[c], x1 = d1[2 * m + 1] + b1[c + 1];
+        const float h0 = fmaxf(x0, 0.f) + lg2_approx(1.f + ex2_approx(-fabsf(x0)));
+        const float h1 = fmaxf(x1, 0.f) + lg2_approx(1.f + ex2_approx(-fabsf(x1)));
+        split2(h0, h1, ah[m], al[m]);
+    }
+}
+// Layer 2 against an N-row K-major weight tile (hi / lo planes, `lbo_w` bytes between K groups, K = 64).
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t* a, uint64_t b_desc) {
+    if constexpr (N == 8) wgmma_rs_n8(d, a, b_desc);
+    else if constexpr (N == 32) wgmma_rs_n32(d, a, b_desc);
+    else wgmma_rs_n48(d, a, b_desc);
+}
+template <int N>
+__device__ __forceinline__ void decoder_layer2_issue(float (&d)[N / 2], const uint32_t (&ah)[16], const uint32_t (&al)[16], uint32_t wh,
+                                                     uint32_t wl, int lbo_w, bool single_pass) {
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+        const uint32_t bo = ks * 2 * lbo_w;
+        wgmma_rs<N>(d, ah + 4 * ks, wgmma_desc(wh + bo, lbo_w, kSBO));
+        if (!single_pass) {
+            wgmma_rs<N>(d, ah + 4 * ks, wgmma_desc(wl + bo, lbo_w, kSBO));
+            wgmma_rs<N>(d, al + 4 * ks, wgmma_desc(wh + bo, lbo_w, kSBO));
+        }
     }
 }
 

@@ -1,8 +1,8 @@
-// bias_act for sm_100a: y = clamp(gain * act(x + b)), and its first / second derivatives.
+// bias_act for sm_90a: y = clamp(gain * act(x + b)), and its first / second derivatives.
 //
 // Semantics follow the reference plugin kernel (ops/bias_act.cu:27-151) exactly - same activation
 // table, same G=0/1/2 formulas expressed through the saved xref / yref, same clamp rule - but the
-// kernel is rebuilt for B200's memory system: it is a pure HBM-streaming op (1 read + 1 write per
+// kernel is rebuilt for H100's memory system: it is a pure HBM-streaming op (1 read + 1 write per
 // element forward, up to 4 reads in the gradient modes), so
 //   * every tensor moves as 128-bit vectors (4 fp32 / 8 fp16|bf16 per access);
 //   * the bias index costs one 64-bit div+mod per VECTOR (NCHW: all lanes of a vector share one

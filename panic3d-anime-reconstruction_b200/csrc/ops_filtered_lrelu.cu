@@ -1,4 +1,4 @@
-// filtered_lrelu for sm_100a: bias -> up-FIR -> gain*lrelu/clamp (with the 2-bit sign tensor) -> down-FIR,
+// filtered_lrelu for sm_90a: bias -> up-FIR -> gain*lrelu/clamp (with the 2-bit sign tensor) -> down-FIR,
 // one CTA per 32x16 output tile of one (n,c) image, everything between the input read and the output write
 // lives in shared memory.  Semantics follow the reference plugin (ops/filtered_lrelu.cu:143-1103, host side
 // ops/filtered_lrelu.cpp:20-214) and its Python composition (ops/filtered_lrelu.py:123-155):
@@ -7,7 +7,7 @@
 //     y = upfirdn2d(v, fd, down)
 // The reference ships 31 hand-specialised tile/filter configurations and returns -1 ("no kernel") for the rest;
 // here ONE runtime-generic kernel covers every (up, down, filter shape, separable or full) combination:
-// shared memory on B200 (227 KB/CTA) holds the up-sampled tile for every practical filter, and the op is
+// shared memory on H100 (227 KB/CTA) holds the up-sampled tile for every practical filter, and the op is
 // far from compute bound, so per-shape template specialisation buys nothing.
 //   A) input footprint -> smem (bias added on real pixels, zeros outside);
 //   B) each thread produces a 4-wide strip of the up-sampled tile (polyphase taps only), applies the
@@ -324,7 +324,14 @@ extern "C" int p3d_filtered_lrelu_act(void* x, uint8_t* s, int32_t dtype, int32_
     for (int i = 0; i < 4; ++i) p.xs[i] = x_stride[i];
     p.sH = sign_mode ? s_h : 0; p.sW = sign_mode ? s_w : 0; p.sx = sx; p.sy = sy; p.gain = gain; p.slope = slope; p.clamp = clamp; p.sign_mode = sign_mode;
     const long long total = (long long)n * c * (sign_mode == 1 ? (h > s_h ? h : s_h) : h) * (((sign_mode == 1 ? (w > s_w ? w : s_w) : w) + 3) / 4);
-    const int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    static int n_sm = 0;
+    if (!n_sm) {
+        int dev = 0;
+        P3D_CUDA_TRY(cudaGetDevice(&dev));
+        P3D_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    }
+    const long long cap = (long long)n_sm * 16;                               // 16 CTAs of 256 threads per SM, grid-stride beyond
+    const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
     cudaStream_t st = (cudaStream_t)stream;
     switch (dtype) {
         case P3D_F32: k_filtered_lrelu_act<float><<<grid, 256, 0, st>>>(p); break;

@@ -1,10 +1,10 @@
-// upfirdn2d for sm_100a: zero-insert upsample -> pad/crop -> 2-D FIR -> decimate, x gain.
+// upfirdn2d for sm_90a: zero-insert upsample -> pad/crop -> 2-D FIR -> decimate, x gain.
 //
 //   y[n,c,oy,ox] = gain * sum_{ky,kx} P[oy*downy + ky, ox*downx + kx] * w[ky][kx]
 //   P[py,px]     = x[(py-pady0)/upy, (px-padx0)/upx] where both divisions are exact and in range, else 0
 //   w[ky][kx]    = flip ? f[ky][kx] : f[fH-1-ky][fW-1-kx]          (reference semantics: ops/upfirdn2d.py:169-213,
 //                                                                    kernels ops/upfirdn2d.cu:33-204)
-// The op is HBM-bound (read x once, write y once, a handful of FMAs per output), so the B200 kernel is built
+// The op is HBM-bound (read x once, write y once, a handful of FMAs per output), so the kernel is built
 // around memory behaviour rather than per-(up,down,filter) template specialisations (the reference has ~100):
 //   * tiled path (input rows contiguous along W): a CTA produces a 64x16 output tile of one (n,c) image; the
 //     input footprint is staged ONCE in shared memory with coalesced row reads, zero-filled outside the image,
@@ -18,6 +18,9 @@
 
 namespace p3d {
 namespace {
+
+// a * b + c per component, each rounded once (fma.rn)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 template <typename T> struct Px;
 template <> struct Px<float> { using acc = float; static __device__ float ld(float v) { return v; } static __device__ float st(float v) { return v; } };
@@ -288,11 +291,11 @@ __global__ void __launch_bounds__(kThreads) k_upfirdn2d_fast(const UpfirdnParams
 #pragma unroll
                     for (int j = 0; j < NT; ++j) {
                         if (UP == 1) {                                       // same tap j, two blocks
-                            acc[r][q] = __ffma2_rn(make_float2(v[(2 * q) % NB][j], v[(2 * q + 1) % NB][j]), w2[ky][j], acc[r][q]);
+                            acc[r][q] = ffma2(make_float2(v[(2 * q) % NB][j], v[(2 * q + 1) % NB][j]), w2[ky][j], acc[r][q]);
                         } else {                                             // even column: tap 2j, input j; odd: tap KX_ODD+2j
                             constexpr int dummy = 0; (void)dummy;
                             const int sco = (DOWN + Cfg::KX_ODD + j * UP) / UP;
-                            acc[r][q] = __ffma2_rn(make_float2(v[q % NB][j], v[q % NB][sco]), w2[ky][j], acc[r][q]);
+                            acc[r][q] = ffma2(make_float2(v[q % NB][j], v[q % NB][sco]), w2[ky][j], acc[r][q]);
                         }
                     }
                 }

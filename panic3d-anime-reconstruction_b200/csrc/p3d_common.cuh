@@ -1,4 +1,4 @@
-// Shared device/host helpers for the p3d CUDA library (sm_100a only).
+// Shared device/host helpers for the p3d CUDA library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

@@ -1,4 +1,4 @@
-// Device functions shared by the v1 (multi-kernel SIMT) and the fused tcgen05 renderer.
+// Device functions shared by the v1 (multi-kernel SIMT) and the fused tensor-core renderer.
 #pragma once
 #include "render_internal.cuh"
 

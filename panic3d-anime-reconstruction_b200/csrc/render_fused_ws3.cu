@@ -1,26 +1,26 @@
-// The default fused renderer (round 2): warp-specialised, pipeline depth 3 ("v5").  Same roles and arithmetic as
-// render_fused_ws.cu plus dedicated RAY warps, but the
-// colour logits are parked differently so that THREE ray groups are in flight instead of two:
+// The fused renderer: warp-specialised, pipeline depth 3 - THREE ray groups in flight.
 //
-//   TMEM   D1 [0,64) | sigma [64,80) | coarse areas CA[a] = [96 + 96a, +96), a = n % 3 | fine area FA = [384, 480)
 //   passes C(0) C(1) | F(0) C(2) | F(1) C(3) | ... | F(N-2) F(N-1)          (C = 3 coarse tiles, F = 3 importance tiles)
 //
-// Only the COARSE logits of a group have to wait for the compositing weights through a whole fine pass; the fine
-// logits are consumed right after the group's merge, so all groups share one fine area.  With F(n) followed by C(n+2):
+// A tile's colour sigmoids wait for the group's compositing weights (omega), which exist only after its fine pass.  They are
+// staged in global memory, in this CTA's own slice of the workspace colour buffers (see colour_area: coarse areas
+// CA[n % 3] and one fine area FA, 4 x 48 KB per CTA, ~25 MB on 132 SMs).  The areas are rewritten every few groups, so
+// their footprint fits the 50 MB L2, but they share it with the streamed tri-plane gather; how much of the round trip is
+// served by L2 rather than HBM has not been measured.  Only
+// the COARSE colours of a group have to wait through a whole fine pass; the fine ones are consumed right after the group's
+// merge, so all groups share one fine area.  With F(n) followed by C(n+2):
 //   * importance(n) has two passes of slack (F(n-1), C(n+1)) before the gather of F(n) needs its depths;
-//   * merge(n) + omega(n) run on the RAY warps while the epilogue converts the three tiles of C(n+2); colours(n) runs at
-//     the top of F(n+1)'s first tile - the last point before layer 2 of F(n+1) overwrites the fine area (C(n+3), which
-//     reuses CA[n % 3], comes later still);
+//   * merge(n) + omega(n) run on the RAY warps while the decoder handles the three tiles of C(n+2); colours(n) runs at the
+//     top of F(n+1)'s first tile - the last point before F(n+1) overwrites the fine area (C(n+3), which reuses
+//     CA[n % 3], comes later still);
 //   * the per-group state ring stays 4 deep (groups n .. n+3 alive), the omega slot 2 deep.
-// The round-1 cycle accounts put the gather role at ~30 k cycles/group, the epilogue at ~22 k without the per-ray
-// phases, the ray warps at ~15 k: with the dependency chain hidden this design should sit near the gather bound
-// (~1.5x the 49 k cycles/group of the default kernel).
 //
 //   warps  0-11  GATHER    three teams of four warps; team j takes tiles j, j+3, ... of the tile sequence
-//   warps 12-19  EPILOGUE  per tile: tcgen05.ld D1 -> softplus2 -> A2 tile; sigma read-back; colour reduction
+//   warps 12-19  DECODER   two warpgroups, one per 64-row half of every tile: layer 1 (wgmma, A1 and W1 from shared memory)
+//                          -> softplus2 in registers -> layer 2 (wgmma, A from the registers): colour sigmoids -> colour area,
+//                          sigma -> group state; colour reduction of a group once its omega is ready
 //   warps 20-23  RAY       a warp per ray: importance sampling after a group's coarse pass, merge / transmittance /
 //                          omega and the per-ray outputs after its fine pass
-//   warp  24     MMA       one thread: layer-1 and layer-2 tcgen05.mma, commits
 #include <stdlib.h>
 #include "fused_common.cuh"
 
@@ -31,24 +31,14 @@ namespace {
 using namespace dev;
 using namespace fused;
 
-constexpr int kGW = 12, kEW = 8, kRW = 4, kTeams = 3;   // 25 warps: 7 on one SM sub-partition -> 72 registers per thread
-constexpr int kWarpsWS = kGW + kEW + kRW + 1;
-constexpr int kThreadsWS = kWarpsWS * 32;        // 800
+constexpr int kGW = 12, kEW = 8, kRW = 4, kTeams = 3;   // 24 warps = 6 warpgroups -> 80 registers per thread
+constexpr int kWarpsWS = kGW + kEW + kRW;
+constexpr int kThreadsWS = kWarpsWS * 32;        // 768
 constexpr int kNA = 4;                           // A1 ring depth
 constexpr int kStates = 4;                       // per-group state ring
 constexpr int kRowsG = 384;                      // rows per pass per group
-constexpr int kTmemColsWS = 512;
-constexpr int kColD1 = 0, kColSig = 64, kColCA = 96, kColFA = 384;   // see the TMEM map above
-__device__ __forceinline__ uint32_t d2_col(int n, int pass, int k) { return (uint32_t)(pass == 0 ? kColCA + (n % 3) * 96 + k * 32 : kColFA + k * 32); }
 
-constexpr int kLBO_A = 2048, kLBO_A1 = 2080, kLBO_W1 = 1024, kLBO_W2C = 512, kLBO_W2S = 256;
-// build-time A/B switches (profiles/r2_kernel_log.md); the defaults are what ships
-#ifndef P3D_W3_LG2POLY
-#define P3D_W3_LG2POLY 0       // 1: the lg2(1 + t) half of the tile epilogue's softplus as a packed polynomial on the FMA pipe (needs P3D_W3_SOFTPLUS)
-#endif
-#ifndef P3D_W3_SOFTPLUS
-#define P3D_W3_SOFTPLUS 1      // 1: guard-free softplus max(x,0) + lg2(1 + 2^-|x|) with packed f32x2 adds and a packed hi/lo split
-#endif
+constexpr int kLBO_A1 = 2080, kLBO_W1 = 1024, kLBO_W2C = 512, kLBO_W2S = 256;
 
 
 struct GroupState {                               // written by G (t_c, crop), E (sg_*), R (t_f)
@@ -64,18 +54,15 @@ struct SlotState {                                // written by R (composite), r
 
 struct __align__(1024) WsSmem {
     unsigned char a1[kNA][2][4 * kLBO_A1];
-    unsigned char a2[2][2][16384];
     unsigned char w1[2][4096], w2c[2][4096], w2s[2][2048];
     float b1[kHidden], b2c[kRgb], b2s, pad0[3];
     uint4 tab[kGW][32][4];                        // tap table of a gather warp's 32 rows (see "gather" below)
     GroupState st[kStates];
     SlotState slot[2];
     float rscratch[kRW][768];                      // private scratch of each ray warp (importance / merge)
-    unsigned long long a1_full[kNA], a1_empty[kNA], a2_full[2], a2_empty[2];
-    unsigned long long d1_full, d1_empty, d2_full, dsig_empty;
+    unsigned long long a1_full[kNA], a1_empty[kNA];
     unsigned long long fine_ready[kStates], state_free[kStates];
     unsigned long long sigc_ready[kStates], sigf_ready[kStates], omega_ready[2];   // E -> R (sigma in smem), R -> E (omega)
-    unsigned int tmem_base, pad1;
 };
 
 static_assert(sizeof(WsSmem) + 1024 <= 232448, "WsSmem + alignment slack exceeds the 227 KB a CTA can opt into");
@@ -88,6 +75,7 @@ struct WsArgs {
     const float *ray_t0, *ray_t1;
     unsigned int* bounds;
     float *out_rgb, *out_depth, *out_wsum, *out_xyz;
+    float *col_c, *col_f;            // workspace colour buffers: this kernel's colour areas (colour_area)
     long long R;
     int n_groups, single_pass;
     int srow, scol, splane;
@@ -134,17 +122,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
     const int T = 6 * n_my;
 
     // ---------------- setup
-    if (warp == kWarpsWS - 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "r"(kTmemColsWS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (tid == 0) {
-        for (int i = 0; i < kNA; ++i) { mbar_init(&sm.a1_full[i], 4); mbar_init(&sm.a1_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&sm.a2_full[i], kEW); mbar_init(&sm.a2_empty[i], 1); }
-        mbar_init(&sm.d1_full, 1); mbar_init(&sm.d1_empty, kEW); mbar_init(&sm.d2_full, 1); mbar_init(&sm.dsig_empty, 4);
+        for (int i = 0; i < kNA; ++i) { mbar_init(&sm.a1_full[i], 4); mbar_init(&sm.a1_empty[i], kEW); }
         for (int i = 0; i < kStates; ++i) {
             mbar_init(&sm.fine_ready[i], kRW); mbar_init(&sm.state_free[i], 1);
-            mbar_init(&sm.sigc_ready[i], 4); mbar_init(&sm.sigf_ready[i], 4);      // the four chunk-0 epilogue warps
+            mbar_init(&sm.sigc_ready[i], kEW); mbar_init(&sm.sigf_ready[i], kEW);
         }
         mbar_init(&sm.omega_ready[0], kRW); mbar_init(&sm.omega_ready[1], kRW);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -177,17 +159,13 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
     if (tid < kRgb) sm.b2c[tid] = -__fmul_rn(a.b2[tid + 1], g.b2_gain) * kLog2e;
     if (tid == 0) sm.b2s = __fmul_rn(a.b2[0], g.b2_gain);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm.tmem_base;
 
     if (warp < kGW) {
         // =========================================================================== GATHER
         const int gw = warp, team = gw >> 2, wt = gw & 3;
         Tick tk_(a.timing, blockIdx.x == 0 && gw == 0 && lane == 0);
         constexpr int kEsz = BF16 ? 2 : 4;
-        constexpr int kImmX = SCOL * kEsz;                                  // byte offset of the x+1 texel when the column stride is static
         const long long scolB = (long long)a.scol * kEsz, srowB = (long long)a.srow * kEsz;
         unsigned char* tab = reinterpret_cast<unsigned char*>(sm.tab[gw]);
         float v[6][8];
@@ -288,17 +266,13 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                     const float4 w0 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 1));
                     const float4 w1 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 2));
                     const float4 w2 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 3));
-                    unsigned long long acc[2] = {0ull, 0ull};
+                    float acc[4] = {0.f, 0.f, 0.f, 0.f};
                     fma4(acc, v4[0], w0.x); fma4(acc, v4[1], w0.y); fma4(acc, v4[2], w0.z); fma4(acc, v4[3], w0.w);
                     fma4(acc, v4[4], w1.x); fma4(acc, v4[5], w1.y); fma4(acc, v4[6], w1.z); fma4(acc, v4[7], w1.w);
                     fma4(acc, v4[8], w2.x); fma4(acc, v4[9], w2.y); fma4(acc, v4[10], w2.z); fma4(acc, v4[11], w2.w);
                     uint32_t h[2], l[2];
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) {
-                        float e0, e1;
-                        asm("mov.b64 {%0, %1}, %2;" : "=f"(e0), "=f"(e1) : "l"(acc[j]));
-                        split2(e0, e1, h[j], l[j]);
-                    }
+                    split2(acc[0], acc[1], h[0], l[0]);
+                    split2(acc[2], acc[3], h[1], l[1]);
                     const int trow = wt * 32 + lrow;
                     const int off = (trow >> 3) * kSBO + (qd >> 1) * kLBO_A1 + (trow & 7) * 16 + (qd & 1) * 8;
                     *reinterpret_cast<uint2*>(a1h + off) = make_uint2(h[0], h[1]);
@@ -311,44 +285,27 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             tk_.lap(3);                                                   // [3] gather of one tile (32 rows)
         }
     } else if (warp < kGW + kEW) {
-        // =========================================================================== EPILOGUE
-        const int e = warp - kGW, quarter = e & 3, chunk = e >> 2;
-        const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-        const int etid = tid - kGW * 32;                                  // 0..255 inside the epilogue group
-
-        auto sigma_read = [&](int it_prev, const TileDesc& tp) {          // column 0 of the sigma accumulator -> state
-            if (chunk != 0) return;
-            mbar_wait(&sm.d2_full, it_prev & 1);
-            tc_fence_after();
-            float sg = tmem_ld1(tmem + kColSig + lane_base) + sm.b2s;
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.dsig_empty);
-            GroupState& st = sm.st[tp.n & 3];
-            const int trow = quarter * 32 + lane;
-            const int rl = trow / RPT, s = tp.k * RPT + (trow - rl * RPT);
-            const int srow = rl * S + s;
-            if (st.crop[tp.pass][srow]) sg = -1e3f;
-            if (g.binarize_on) sg = sg < a.sigma_cull ? -1e3f : 1e3f;
-            else if (g.cull_on && sg < a.sigma_cull) sg = -1e3f;
-            (tp.pass == 0 ? st.sg_c : st.sg_f)[srow] = sg;
-            if (tp.k == 2) {                                              // the group's pass is complete: hand it to the ray warps
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tp.pass == 0 ? &sm.sigc_ready[tp.n & 3] : &sm.sigf_ready[tp.n & 3]);
-            }
+        // =========================================================================== DECODER
+        const int e = warp - kGW, quarter = e & 3, chunk = e >> 2;      // chunk = warpgroup = 64-row half of a tile
+        const int etid = tid - kGW * 32;                                  // 0..255 inside the decoder group
+        // this CTA's colour area of (group n, pass): 384 rows x 32 sigmoids, row = 128 k + row of tile k.  Areas are slices of
+        // the workspace colour buffers that belong to this CTA's own first two groups (coarse and fine buffer each), so they
+        // exist whenever they are used: CA[0..2] = slices 0..2, FA = slice 3 (slice 1 when the CTA has a single group)
+        auto colour_area = [&](int n, int pass) -> float* {
+            const int j = pass == 0 ? n % 3 : (n_my >= 2 ? 3 : 1);
+            return ((j & 1) ? a.col_f : a.col_c) + ((long long)blockIdx.x + (long long)(j >> 1) * gridDim.x) * (kRowsG * kRgb);
         };
-        auto ebar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };   // the eight epilogue warps
-        auto colours = [&](int n) {                                        // sum_j omega_j * rgb_j for group n, from TMEM
+        auto ebar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };   // the eight decoder warps
+        auto colours = [&](int n) {                                        // sum_j omega_j * rgb_j for group n
             const int slot_i = n & 1;
             SlotState& sl = sm.slot[slot_i];
             mbar_wait(&sm.omega_ready[slot_i], (n >> 1) & 1);              // omega / pos / back of group n (ray warps)
-            tc_fence_after();
             const int grp = (int)blockIdx.x + n * (int)gridDim.x;
             const long long ray0 = (long long)grp * GR;
-            // A warp's 32 TMEM rows are the same ray(s) in each of its three tiles, so the per-tile column sums are
-            // first added up in a register and published once: every (ray, channel) cell of sl.acc then receives
-            // exactly two shared-memory adds (one per chunk), whose order cannot change the rounded sum - the kernel
-            // is bit-reproducible run to run and independent of how the rays are batched.
+            // A warp's 32 rows are the same ray(s) in each of its three tiles, so the per-tile column sums are first added
+            // up in a register and published once: every (ray, channel) cell of sl.acc then receives exactly two
+            // shared-memory adds (one per chunk), whose order cannot change the rounded sum - the kernel is
+            // bit-reproducible run to run and independent of how the rays are batched.
             float part[2] = {0.f, 0.f};
             const int rl_first = (quarter * 32) / RPT;
             for (int i = 0; i < 3; ++i) {
@@ -360,9 +317,14 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 const float om = live ? sl.om[rl * L + sl.pos[pass * kRowsG + rl * S + s]] : 0.f;
                 const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
                 float v[32];
-                tmem_ld32(tmem + d2_col(n, pass, k) + lane_base, v);
+                const float4* src = reinterpret_cast<const float4*>(colour_area(n, pass) + (k * 128 + trow) * kRgb);
 #pragma unroll
-                for (int c = 0; c < kRgb; ++c) v[c] = fmaf(rcp_approx(1.f + ex2_approx(v[c] + sm.b2c[c])), ca, cb);
+                for (int c4 = 0; c4 < 8; ++c4) {
+                    const float4 q4 = src[c4];
+                    v[4 * c4] = q4.x; v[4 * c4 + 1] = q4.y; v[4 * c4 + 2] = q4.z; v[4 * c4 + 3] = q4.w;
+                }
+#pragma unroll
+                for (int c = 0; c < kRgb; ++c) v[c] = fmaf(v[c], ca, cb);
 #pragma unroll
                 for (int t2 = 0; t2 < 32 / RPT; ++t2) {
                     const int target = rl_first + t2;
@@ -384,88 +346,71 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             }
 #pragma unroll
             for (int t2 = 0; t2 < 32 / RPT; ++t2) atomicAdd(&sl.acc[rl_first + t2][lane], part[t2]);
-            tc_fence_before();
-            asm volatile("bar.sync 1, 256;" ::: "memory");                 // all eight epilogue warps
+            ebar();                                                        // all eight decoder warps (also: the areas are read)
             if (etid < GR * kRgb) {
                 const int rl = etid >> 5, c = etid & 31;
                 const long long ray = ray0 + rl;
                 if (ray < a.R) a.out_rgb[ray * kRgb + c] = __fsub_rn(__fmul_rn(__fadd_rn(sl.acc[rl][c], sl.back[rl]), 2.f), 1.f);
             }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            ebar();
             if (etid == 0) mbar_arrive(&sm.state_free[n & 3]);
         };
 
         // colours(n) needs omega from the ray warps; it runs at the top of the first tile of F(n+1) - three tiles (C(n+2))
-        // after the group's last sigma - which is also the last point before layer 2 of F(n+1) overwrites the fine area.
+        // after the group's last sigma - which is also the last point before F(n+1) overwrites the fine area.
+        const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]);
+        const uint32_t w2ch = smem_u32(sm.w2c[0]), w2cl = smem_u32(sm.w2c[1]), w2sh = smem_u32(sm.w2s[0]), w2sl = smem_u32(sm.w2s[1]);
         Tick tk_(a.timing, blockIdx.x == 0 && e == 0 && lane == 0);
-        auto after_sigma_t = [&](const TileDesc&) {};
-        int it = 0;
-        TileDesc prev{0, 0, 0};
-        bool have_prev = false;
-        for (int q = 0; q < T; ++q) {
-            const TileDesc td = tile_at(q, n_my);
-            // ---- epilogue 1: D1 -> softplus2 -> A2[buf]
+        for (int it = 0; it < T; ++it) {
+            const TileDesc td = tile_at(it, n_my);
             tk_.lap(4);
             if (td.pass == 1 && td.k == 0 && td.n >= 1) { colours(td.n - 1); tk_.lap(11); }   // [11] colours (incl. wait for omega)
-            mbar_wait(&sm.d1_full, it & 1);
-            tk_.lap(5);                                                   // [5] wait d1_full
-            tc_fence_after();
-            float v[32];
-            tmem_ld32(tmem + kColD1 + lane_base + 32 * chunk, v);
-            tc_fence_before();
+            const int stage = it % kNA;
+            mbar_wait(&sm.a1_full[stage], (it / kNA) & 1);
+            tk_.lap(5);                                                   // [5] wait a1_full
+            float d1[32];
+            decoder_layer1(d1, smem_u32(sm.a1[stage][0]), smem_u32(sm.a1[stage][1]), kLBO_A1, w1h, w1l, kLBO_W1, chunk, a.single_pass);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.d1_empty);
-            const int buf = it & 1;
-            tk_.lap(6);                                                   // [6] tcgen05.ld D1
-            mbar_wait(&sm.a2_empty[buf], ((it >> 1) & 1) ^ 1);
-            tk_.lap(7);                                                   // [7] wait a2_empty
-            {
-                const int trow = quarter * 32 + lane;
-                unsigned char* a2h = sm.a2[buf][0];
-                unsigned char* a2l = sm.a2[buf][1];
+            if (lane == 0) mbar_arrive(&sm.a1_empty[stage]);
+            uint32_t ah[16], al[16];
+            decoder_hidden(d1, sm.b1, lane, ah, al);
+            float dc[16], ds[4];
+            decoder_layer2_issue<kRgb>(dc, ah, al, w2ch, w2cl, kLBO_W2C, a.single_pass);
+            decoder_layer2_issue<8>(ds, ah, al, w2sh, w2sl, kLBO_W2S, a.single_pass);
+            wgmma_commit();
+            wgmma_wait_all();
+            fence_operands(dc);
+            fence_operands(ds);
+            tk_.lap(6);                                                   // [6] both layers
+            // this thread's two rows of the tile (fragment elements 2 rs, 2 rs + 1 of each 8-column block)
+            float* area = colour_area(td.n, td.pass) + td.k * 128 * kRgb;
+            GroupState& st = sm.st[td.n & 3];
 #pragma unroll
-                for (int c8 = 0; c8 < 4; ++c8) {
-                    uint32_t ph[4], pl[4];
+            for (int rs = 0; rs < 2; ++rs) {
+                const int trow = 64 * chunk + frag_row(2 * rs, lane, quarter);
 #pragma unroll
-                    for (int x = 0; x < 4; ++x) {
-                        const int j = c8 * 8 + 2 * x;
-#if P3D_W3_SOFTPLUS
-                        // softplus2(x) = max(x, 0) + lg2(1 + 2^-|x|): no overflow for any x, so no threshold select; the two adds
-                        // of a column pair are packed
-                        const unsigned long long x2 = add2(pk2(v[j], v[j + 1]), *reinterpret_cast<const unsigned long long*>(&sm.b1[32 * chunk + j]));
-                        float x0, x1;
-                        upk2(x2, x0, x1);
-#if P3D_W3_LG2POLY
-                        split2p(add2(pk2(fmaxf(x0, 0.f), fmaxf(x1, 0.f)), lg2_1p_poly2(pk2(ex2_approx(-fabsf(x0)), ex2_approx(-fabsf(x1))))), ph[x], pl[x]);
-#else
-                        const unsigned long long u2 = add2(pk2(ex2_approx(-fabsf(x0)), ex2_approx(-fabsf(x1))), pk2(1.f, 1.f));
-                        float u0, u1;
-                        upk2(u2, u0, u1);
-                        split2p(add2(pk2(fmaxf(x0, 0.f), fmaxf(x1, 0.f)), pk2(lg2_approx(u0), lg2_approx(u1))), ph[x], pl[x]);
-#endif
-#else
-                        split2(softplus2(v[j] + sm.b1[32 * chunk + j]), softplus2(v[j + 1] + sm.b1[32 * chunk + j + 1]), ph[x], pl[x]);
-#endif
-                    }
-                    const int off = tile_off(trow, 32 * chunk + 8 * c8, kLBO_A);
-                    *reinterpret_cast<uint4*>(a2h + off) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-                    *reinterpret_cast<uint4*>(a2l + off) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+                for (int blk = 0; blk < 4; ++blk) {
+                    const int i = 4 * blk + 2 * rs, c = frag_col(i, lane);
+                    *reinterpret_cast<float2*>(area + trow * kRgb + c) =
+                        make_float2(rcp_approx(1.f + ex2_approx(dc[i] + sm.b2c[c])), rcp_approx(1.f + ex2_approx(dc[i + 1] + sm.b2c[c + 1])));
+                }
+                if ((lane & 3) == 0) {                                    // column 0 of the sigma accumulator
+                    float sg = ds[2 * rs] + sm.b2s;
+                    const int rl = trow / RPT, s = td.k * RPT + (trow - rl * RPT);
+                    const int srow = rl * S + s;
+                    if (st.crop[td.pass][srow]) sg = -1e3f;
+                    if (g.binarize_on) sg = sg < a.sigma_cull ? -1e3f : 1e3f;
+                    else if (g.cull_on && sg < a.sigma_cull) sg = -1e3f;
+                    (td.pass == 0 ? st.sg_c : st.sg_f)[srow] = sg;
                 }
             }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm.a2_full[buf]);
-            tk_.lap(8);                                                   // [8] softplus / split / A2 stores
-            // ---- sigma of the PREVIOUS tile (its layer 2 has had a whole epilogue to finish), then its group's per-ray phase
-            if (have_prev) { sigma_read(it - 1, prev); tk_.lap(12); after_sigma_t(prev); }   // [12] sigma read-back (incl. wait d2_full)
-            prev = td; have_prev = true;
-            ++it;
-            // last tile of a pass: its sigma completes the group's hand-off to the ray warps (and, at the tail, the next tile
-            // depends on it), so it is read at once.  (Deferring it behind the next tile's conversion like the other tiles'
-            // was measured: 3.66 ms vs 3.60 ms per launch - the ray warps lose the slack the epilogue gains.)
-            if (td.k == 2) { sigma_read(it - 1, prev); tk_.lap(12); after_sigma_t(prev); have_prev = false; }
+            if (td.k == 2) {                                              // the group's pass is complete: hand it to the ray warps
+                __threadfence_block();                                    // (its colour-area stores included)
+                __syncwarp();
+                if (lane == 0) mbar_arrive(td.pass == 0 ? &sm.sigc_ready[td.n & 3] : &sm.sigf_ready[td.n & 3]);
+            }
+            tk_.lap(8);                                                   // [8] colour / sigma stores
         }
-        if (have_prev) { sigma_read(it - 1, prev); after_sigma_t(prev); }
         colours(n_my - 1);
     } else if (warp < kGW + kEW + kRW) {
         // =========================================================================== RAY (one warp per ray)
@@ -697,68 +642,6 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 tr_.lap(10);                                                  // [10] merge / weights
             }
         }
-    } else {
-        // =========================================================================== MMA issuer (one thread)
-        if (lane == 0) {
-            const uint32_t idesc1 = umma_idesc(128, kHidden), idesc2c = umma_idesc(128, kRgb), idesc2s = umma_idesc(128, 16);
-            const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]);
-            const uint32_t w2ch = smem_u32(sm.w2c[0]), w2cl = smem_u32(sm.w2c[1]), w2sh = smem_u32(sm.w2s[0]), w2sl = smem_u32(sm.w2s[1]);
-            auto layer2 = [&](int it2, const TileDesc& tp) {
-                const int buf = it2 & 1;
-                mbar_wait(&sm.a2_full[buf], (it2 >> 1) & 1);
-                mbar_wait(&sm.dsig_empty, (it2 & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t a2h = smem_u32(sm.a2[buf][0]), a2l = smem_u32(sm.a2[buf][1]);
-                const uint32_t dc = tmem + d2_col(tp.n, tp.pass, tp.k), ds = tmem + kColSig;
-#pragma unroll
-                for (int ks = 0; ks < kHidden / 16; ++ks) {
-                    const uint32_t ao = ks * 2 * kLBO_A;
-                    umma_bf16(dc, umma_desc(a2h + ao, kLBO_A, kSBO), umma_desc(w2ch + ks * 2 * kLBO_W2C, kLBO_W2C, kSBO), idesc2c, ks > 0);
-                    umma_bf16(ds, umma_desc(a2h + ao, kLBO_A, kSBO), umma_desc(w2sh + ks * 2 * kLBO_W2S, kLBO_W2S, kSBO), idesc2s, ks > 0);
-                    if (!a.single_pass) {
-                        umma_bf16(dc, umma_desc(a2h + ao, kLBO_A, kSBO), umma_desc(w2cl + ks * 2 * kLBO_W2C, kLBO_W2C, kSBO), idesc2c, 1);
-                        umma_bf16(dc, umma_desc(a2l + ao, kLBO_A, kSBO), umma_desc(w2ch + ks * 2 * kLBO_W2C, kLBO_W2C, kSBO), idesc2c, 1);
-                        umma_bf16(ds, umma_desc(a2h + ao, kLBO_A, kSBO), umma_desc(w2sl + ks * 2 * kLBO_W2S, kLBO_W2S, kSBO), idesc2s, 1);
-                        umma_bf16(ds, umma_desc(a2l + ao, kLBO_A, kSBO), umma_desc(w2sh + ks * 2 * kLBO_W2S, kLBO_W2S, kSBO), idesc2s, 1);
-                    }
-                }
-                umma_commit(&sm.d2_full);
-                umma_commit(&sm.a2_empty[buf]);
-            };
-            int it = 0;
-            TileDesc prev{0, 0, 0};
-            bool have_prev = false;
-            for (int q = 0; q < T; ++q) {
-                const TileDesc td = tile_at(q, n_my);
-                    const int stage = it % kNA;
-                mbar_wait(&sm.a1_full[stage], (it / kNA) & 1);
-                mbar_wait(&sm.d1_empty, (it & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t a1h = smem_u32(sm.a1[stage][0]), a1l = smem_u32(sm.a1[stage][1]);
-#pragma unroll
-                for (int ks = 0; ks < kC / 16; ++ks) {
-                    const uint32_t ao = ks * 2 * kLBO_A1, bo = ks * 2 * kLBO_W1;
-                    umma_bf16(tmem + kColD1, umma_desc(a1h + ao, kLBO_A1, kSBO), umma_desc(w1h + bo, kLBO_W1, kSBO), idesc1, ks > 0);
-                    if (!a.single_pass) {
-                        umma_bf16(tmem + kColD1, umma_desc(a1h + ao, kLBO_A1, kSBO), umma_desc(w1l + bo, kLBO_W1, kSBO), idesc1, 1);
-                        umma_bf16(tmem + kColD1, umma_desc(a1l + ao, kLBO_A1, kSBO), umma_desc(w1h + bo, kLBO_W1, kSBO), idesc1, 1);
-                    }
-                }
-                umma_commit(&sm.d1_full);
-                umma_commit(&sm.a1_empty[stage]);
-                if (have_prev) layer2(it - 1, prev);
-                prev = td; have_prev = true;
-                ++it;
-                if (td.k == 2) { layer2(it - 1, prev); have_prev = false; }   // see EPILOGUE
-            }
-            if (have_prev) layer2(it - 1, prev);
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kWarpsWS - 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemColsWS) : "memory");
     }
 }
 
@@ -793,6 +676,7 @@ int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const vo
     a.g = g; a.planes = planes; a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2; a.ro = ro; a.rd = rd; a.u_c = u_c; a.u_f = u_f;
     a.ray_t0 = ws.ray_t0; a.ray_t1 = ws.ray_t1; a.bounds = ws.bounds;
     a.out_rgb = out_rgb; a.out_depth = out_depth; a.out_wsum = out_wsum; a.out_xyz = out_xyz;
+    a.col_c = ws.rgb_c; a.col_f = ws.rgb_f;
     const int GR = 384 / g.S;
     a.R = R; a.n_groups = (int)((R + GR - 1) / GR);
     a.single_pass = p->mlp_mode == P3D_MLP_TC_BF16;
@@ -836,12 +720,11 @@ int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const vo
         P3D_CUDA_TRY(cudaStreamSynchronize(stream));
         const int groups_cta0 = (a.n_groups + grid - 1) / grid;
         fprintf(stderr, "[p3d ws timing, CTA0, cycles/group over %d groups] G(warp0: 1/3 of tiles): wait_dep %.0f wait_ring %.0f gather %.0f | "
-                        "E(warp0): wait_d1 %.0f ld_d1 %.0f wait_a2 %.0f epi1 %.0f sigma %.0f colours(+omega wait) %.0f other %.0f | "
+                        "D(warp0): wait_a1 %.0f layers %.0f stores %.0f colours(+omega wait) %.0f other %.0f | "
                         "R(warp0): wait_sigc %.0f importance %.0f wait_sigf %.0f merge %.0f\n",
                 groups_cta0, (double)h[1] / groups_cta0, (double)h[2] / groups_cta0, (double)h[3] / groups_cta0, (double)h[5] / groups_cta0,
-                (double)h[6] / groups_cta0, (double)h[7] / groups_cta0, (double)h[8] / groups_cta0, (double)h[12] / groups_cta0,
-                (double)h[11] / groups_cta0, (double)(h[0] + h[4]) / groups_cta0, (double)h[13] / groups_cta0, (double)h[9] / groups_cta0,
-                (double)h[14] / groups_cta0, (double)h[10] / groups_cta0);
+                (double)h[6] / groups_cta0, (double)h[8] / groups_cta0, (double)h[11] / groups_cta0, (double)h[4] / groups_cta0,
+                (double)h[13] / groups_cta0, (double)h[9] / groups_cta0, (double)h[14] / groups_cta0, (double)h[10] / groups_cta0);
     }
     if (p->defer_depth_clamp) return P3D_OK;
     return launch_depth_finalize(out_depth, R, ws.bounds, stream);

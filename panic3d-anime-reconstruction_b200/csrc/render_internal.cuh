@@ -57,22 +57,16 @@ int render_backward_v1(const Geom& g, const p3d_render_params* p, const void* pl
                        float* d_w2, float* d_b2, cudaStream_t stream);
 int launch_bounds_to_float(const unsigned int* bounds, float* out2, cudaStream_t stream);
 int launch_depth_finalize_f(float* depth, long long R, const float* bounds2, cudaStream_t stream);
-// warp-specialised fused renderer (v3): 1 CTA/SM, gather / epilogue / ray / MMA roles, two ray groups in flight.
-// pipeline-depth-3 variant with dedicated ray warps (render_fused_ws3.cu): the default fused kernel (P3D_FUSED_IMPL=v3 selects the one above)
+// warp-specialised fused renderer (render_fused_ws3.cu): gather / wgmma decoder / ray roles, three ray groups in flight
 bool fused_ws3_supported(const Geom& g);
 int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
                              const float* w2, const float* b2, const float* ro, const float* rd, const float* u_c,
                              const float* u_f, const Workspace& ws, float* out_rgb, float* out_depth, float* out_wsum,
                              float* out_xyz, cudaStream_t stream);
-bool fused_ws_supported(const Geom& g);
-int render_forward_fused_ws(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
-                            const float* w2, const float* b2, const float* ro, const float* rd, const float* u_c,
-                            const float* u_f, const Workspace& ws, float* out_rgb, float* out_depth, float* out_wsum,
-                            float* out_xyz, cudaStream_t stream);
 int decode_points_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
                      const float* w2, const float* b2, const float* coords, long long n_pts, float* out_rgb,
                      float* out_sigma, cudaStream_t stream);
-// streaming tensor-core decode (decode_tc.cu): the gather -> tcgen05 decoder pipeline of the renderer without per-ray phases
+// streaming tensor-core decode (decode_tc.cu): the gather -> wgmma decoder pipeline of the renderer without per-ray phases
 bool decode_tc_supported(const Geom& g, long long total);
 int decode_points_tc(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
                      const float* w2, const float* b2, const float* coords, long long n_pts, float* out_rgb,

@@ -373,7 +373,7 @@ int launch_sample_decode(const SampleArgs& a, bool bf16, cudaStream_t stream) {
 
 }  // namespace
 
-// small launches shared with the fused renderers (render_fused_ws*.cu)
+// small launches shared with the fused renderer (render_fused_ws3.cu)
 int launch_bounds_init(unsigned int* bounds, cudaStream_t stream) {
     k_init_bounds<<<1, 32, 0, stream>>>(bounds);
     P3D_LAUNCH_CHECK();

@@ -1,4 +1,4 @@
-"""Plug the B200 hot path into an unmodified checkout of the reference.
+"""Plug the H100 hot path into an unmodified checkout of the reference.
 
 The reference instantiates the renderer by import name
 (`from training.volumetric_rendering.renderer import ImportanceRenderer`, triplane.py:14-15, and again when

@@ -1,10 +1,10 @@
 """CUDA-graph replay of the generator's launch-bound sub-networks (SURVEY.md 8f-1: the callers of the renderer).
 
-Measured on a B200 (``profiles/r2_configs/c3_kernels.json``): one view of the eval sweep through the unchanged ``G.f`` costs
-10.0 ms of wall clock but only 3.1 ms of device time - ~150 eager PyTorch launches per view, most of them a few microseconds long
-(per-layer modulation, demodulation, noise, bias/activation, layout conversions around cuDNN), issued by one Python thread.  The
-renderer is a single 0.48 ms launch; the StyleGAN2 backbone (``G.backbone.synthesis``) and the super-resolution head
-(``G.superresolution``) are where the launches are, and for a given input signature they are static launch sequences.  This module
+One view of the eval sweep through the unchanged ``G.f`` is ~150 eager PyTorch launches, most of them a few microseconds long
+(per-layer modulation, demodulation, noise, bias/activation, layout conversions around cuDNN), issued by one Python thread, so its
+wall clock is far above its device time.  The renderer is a single launch; the StyleGAN2 backbone (``G.backbone.synthesis``) and
+the super-resolution head (``G.superresolution``) are where the launches are, and for a given input signature they are static
+launch sequences.  This module
 captures each of them ONCE into a CUDA graph and replays it:
 
     ``GraphedCallable(fn)``        inference-only wrapper: the first call with a new signature (tensor shapes / dtypes, non-tensor

@@ -1,4 +1,4 @@
-"""Image output behind the renderer - the B200 replacement for ``I(tensor).save(fn)`` at the end of every view of the
+"""Image output behind the renderer - the H100 replacement for ``I(tensor).save(fn)`` at the end of every view of the
 reference's eval sweep (``_scripts/eval/generate.py:141-148``; ``_util/twodee_v1.py:36-91,174-185,732-760``; SURVEY.md 8f-4).
 
 The reference converts on the host: a blocking ``.cpu()`` of the fp32 image, ``to_pil_image(t.float().clamp(0,1))``

@@ -1,4 +1,4 @@
-"""Front-view paste - the B200 replacement for ``paste_front`` and its helpers
+"""Front-view paste - the H100 replacement for ``paste_front`` and its helpers
 (reference ``_train/eg3dc/src/training/triplane.py:555-691``; SURVEY.md section 8f-3).
 
 ``TriPlaneGenerator.f`` (triplane.py:498-502) calls ``paste_front(self, x, ret, **x['paste_params'])`` for every view

@@ -1,7 +1,7 @@
 """Drop-in for ``torch_utils/ops/bias_act.py`` (reference ops/bias_act.py:23-209).
 
 Same call surface - ``bias_act(x, b, dim, act, alpha, gain, clamp, impl)`` and the ``activation_funcs`` table -
-over the sm_100a kernel ``p3d_bias_act`` (include/p3d_ops.h).  First and second derivatives are the same fused
+over the sm_90a kernel ``p3d_bias_act`` (include/p3d_ops.h).  First and second derivatives are the same fused
 kernel in grad mode 1 / 2, wired through two autograd Functions exactly as the op's contract requires
 (what gets saved is dictated by which of x / y each activation's derivative is expressed in).
 No CPU path and no ``impl='ref'`` here: the PyTorch restatement lives in ``oracle/ops_oracle.py`` (tests only).

@@ -1,6 +1,6 @@
 """Drop-in for ``torch_utils/ops/filtered_lrelu.py`` (reference ops/filtered_lrelu.py:58-274).
 
-``filtered_lrelu(x, fu, fd, b, up, down, padding, gain, slope, clamp, flip_filter, impl)`` over the sm_100a
+``filtered_lrelu(x, fu, fd, b, up, down, padding, gain, slope, clamp, flip_filter, impl)`` over the sm_90a
 kernel ``p3d_filtered_lrelu`` (include/p3d_ops.h).  One runtime-generic kernel covers every filter/up/down
 combination, so the reference's "no optimised kernel -> generic fallback" branch does not exist here.  The
 forward pass records 2 bits per up-sampled pixel (negative / clamped) so the backward pass - the same op with

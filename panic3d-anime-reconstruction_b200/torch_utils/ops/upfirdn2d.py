@@ -8,7 +8,7 @@ formulation - is this repository's own.
 
 Same public names and argument meaning - ``setup_filter``, ``upfirdn2d``, ``filter2d``, ``upsample2d``,
 ``downsample2d`` (+ the ``_parse_*`` / ``_get_filter_size`` helpers other reference modules import) - over the
-sm_100a kernel ``p3d_upfirdn2d`` (include/p3d_ops.h).  upfirdn2d is linear, so its gradient of any order is
+sm_90a kernel ``p3d_upfirdn2d`` (include/p3d_ops.h).  upfirdn2d is linear, so its gradient of any order is
 another upfirdn2d with up/down swapped, the filter flipped and the adjoint padding; the autograd Function below
 re-enters itself for that, which is what makes R1's double-backward work.  No CPU path, no ``impl='ref'``.
 """

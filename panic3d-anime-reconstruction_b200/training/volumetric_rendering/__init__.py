@@ -1,1 +1,1 @@
-"""B200 renderer modules served under the reference import name ``training.volumetric_rendering``."""
+"""H100 renderer modules served under the reference import name ``training.volumetric_rendering``."""

@@ -193,7 +193,7 @@ class ImportanceRenderer(torch.nn.Module):
         self.ray_marcher = MipRayMarcher2()
         self.use_triplane = bool(use_triplane)
         self.plane_axes = generate_planes(use_triplane=use_triplane)
-        # decoder arithmetic (include/p3d_render.h).  'auto' (default): the fused tcgen05 kernel in its fp32-class 3-pass
+        # decoder arithmetic (include/p3d_render.h).  'auto' (default): the fused tensor-core kernel in its fp32-class 3-pass
         # mode wherever it exists (p3d_render_fused_supported: depth_resolution == depth_resolution_importance in
         # {48, 96} - the reference's training and eval settings), the fp32 SIMT kernels for every other sample count.
         # An explicit _lib.P3D_MLP_* value forces that mode and raises if it has no kernel.

@@ -1,4 +1,4 @@
-"""Dense sigma / colour volume for mesh extraction - the B200 replacement for ``get_eg3d_volume``
+"""Dense sigma / colour volume for mesh extraction - the H100 replacement for ``get_eg3d_volume``
 (reference ``_util/eg3d_metrics3d.py:94-183``; SURVEY.md section 8f-2).
 
 The reference evaluates resolution^3 = 16.8 M grid points as 168 host-side chunks of 100k: every chunk re-runs the

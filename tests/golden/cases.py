@@ -52,7 +52,7 @@ RENDER_CASES = {
     # eval sampling 96+96 (eg3dc_v0.py:30-31) on a small image
     'mid_eval96': dict(seed=24, N=1, R=24, P=128, opts=_opts(), cameras=[(0.0, 0.0, 1.0, 30.0)],
                        triplane_crop=0.1, cull_clouds=0.5, force_sigmoid=True, sigma_bias=2.0),
-    # ---- fused tcgen05 kernel coverage (it exists for S = Sf in {48, 96} only): the option matrix of the small_* cases at 48+48
+    # ---- fused tensor-core kernel coverage (it exists for S = Sf in {48, 96} only): the option matrix of the small_* cases at 48+48
     'fused48_ortho': _small(51, ortho=True, cameras=[(20.0, -135.0, 1.0, -1.0)], opts=dict(depth_resolution=48, depth_resolution_importance=48)),
     'fused48_auto_limits': _small(52, opts=dict(ray_start='auto', ray_end='auto', depth_resolution=48, depth_resolution_importance=48)),
     'fused48_disparity': _small(53, opts=dict(disparity_space_sampling=True, depth_resolution=48, depth_resolution_importance=48)),

@@ -40,7 +40,7 @@ def test_every_declared_symbol_is_exported(lib):
 
 def test_version_and_host_only_calls(lib):
     from panic3d_b200 import _lib
-    assert b'sm_100a' in lib.p3d_version()
+    assert b'sm_90a' in lib.p3d_version()
     p = _lib.RenderParams()
     p.n_views, p.n_rays, p.n_coarse, p.n_fine = 8, 128 * 128, 96, 96
     p.channels, p.hidden, p.out_dim, p.plane_h, p.plane_w = 32, 64, 33, 512, 512
