@@ -67,6 +67,11 @@ _PROTOS = {
     'p3d_copy_async': (C.c_int, [_VP, _VP, C.c_size_t, _VP]),
     'p3d_profile_enable': (None, [C.c_int]),
     'p3d_profile_read': (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int, C.c_int]),
+    # include/p3d_mesh.h (panic3d_b200.mesh)
+    'p3d_mc_workspace_bytes': (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
+    'p3d_mc_count': (C.c_int, [_VP, C.c_int64, C.c_int64, C.c_int64, C.c_float, _VP, C.c_size_t, _VP, _VP]),
+    'p3d_mc_emit': (C.c_int, [_VP, C.c_int64, C.c_int64, C.c_int64, C.c_float, _VP, C.c_size_t] + [_VP] * 6),
+    'p3d_mc_lattice_coords': (C.c_int, [_VP, C.c_int64, C.c_int32, C.c_double, _VP, _VP]),
 }
 
 

@@ -46,28 +46,11 @@ struct DecArgs {
     long long total, per_view;
     int single_pass, n_tiles;
     int srow, scol, splane;
-    // volume mode (see render_v1.cu: volume_point / volume_dest)
+    // volume mode (render_device.cuh: volume_point / volume_dest)
     int vol_res;
     float vol_size, vol_origin, vol_crop, vol_cull;
     int vol_crop_on, vol_cull_on;
 };
-
-// point n of the reference's create_samples lattice, bit for bit (eg3d_metrics3d.py:70-92: un-floored float y / x "indices")
-__device__ __forceinline__ void volume_point(long long n, int R, float vsize, float vorigin, float& x, float& y, float& z) {
-    const float nf = (float)n, Rf = (float)R;
-    const float iz = (float)(n % R);
-    const float q1 = __fdiv_rn(nf, Rf);
-    const float iy = fmodf(q1, Rf);
-    const float ix = fmodf(__fdiv_rn(q1, Rf), Rf);
-    x = __fadd_rn(__fmul_rn(ix, vsize), vorigin);
-    y = __fadd_rn(__fmul_rn(iy, vsize), vorigin);
-    z = __fadd_rn(__fmul_rn(iz, vsize), vorigin);
-}
-__device__ __forceinline__ long long volume_dest(long long n, int R) {
-    const long long rr = (long long)R * R;
-    const long long a = n / rr, rest = n - a * rr;
-    return ((long long)(R - 1) - a) * rr + rest;
-}
 
 template <bool BF16, bool VOLUME, int SCOL>
 __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {

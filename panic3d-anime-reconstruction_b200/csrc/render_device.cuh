@@ -30,6 +30,31 @@ __device__ __forceinline__ float coarse_depth(const Geom& g, int s, float u, flo
 }
 
 // -------------------------------------------------------------------------------------------
+// Grid point n of the reference's create_samples (eg3d_metrics3d.py:70-92), bit for bit: the z index is the integer
+// n % R, but the y and x "indices" come from FLOAT divisions that are never floored - (float(n)/R) % R and
+// ((float(n)/R)/R) % R - so the lattice is sheared by a fraction of a voxel.  Meshes downstream were extracted from
+// exactly these points, so the shear is part of the contract.  Used by the v1 and tensor-core volume queries and by
+// the mesh's colour lookup (marching_cubes.cu).
+// -------------------------------------------------------------------------------------------
+__device__ __forceinline__ void volume_point(long long n, int R, float vsize, float vorigin, float& x, float& y, float& z) {
+    const float nf = (float)n, Rf = (float)R;
+    const float iz = (float)(n % R);
+    const float q1 = __fdiv_rn(nf, Rf);
+    const float iy = fmodf(q1, Rf);
+    const float ix = fmodf(__fdiv_rn(q1, Rf), Rf);
+    x = __fadd_rn(__fmul_rn(ix, vsize), vorigin);
+    y = __fadd_rn(__fmul_rn(iy, vsize), vorigin);
+    z = __fadd_rn(__fmul_rn(iz, vsize), vorigin);
+}
+// where sample n of a view lands in the returned volume: reshape (R,R,R) by flat index, first axis flipped.  The map is
+// its own inverse, so it also gives the sample n of volume element (a, b, c).
+__device__ __forceinline__ long long volume_dest(long long n, int R) {
+    const long long rr = (long long)R * R;
+    const long long a = n / rr, rest = n - a * rr;
+    return ((long long)(R - 1) - a) * rr + rest;
+}
+
+// -------------------------------------------------------------------------------------------
 // Tri-plane bilinear gather for one sample, channels [4q, 4q+4).  renderer.py:52-81:
 //   grid = coord * (2/box_warp); texel = ((grid+1)*size - 1)/2  (align_corners=False);
 //   taps outside the plane contribute zero (padding_mode='zeros'); mean over the 3 planes.

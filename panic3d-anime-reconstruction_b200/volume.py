@@ -91,6 +91,15 @@ def get_eg3d_volume(G, xin, resolution=256, max_batch=100000):
     the reference's warm-up call), the backbone once more for the tri-planes (``triplane.py:283-291``), then ONE
     volume launch replaces the 168-chunk loop; ``max_batch`` is accepted and ignored."""
     del max_batch
+    planes = synthesize_planes(G, xin)
+    return query_volume(planes, G.decoder, G.rendering_kwargs, resolution=resolution,
+                        triplane_crop=xin['triplane_crop'] if 'triplane_crop' in xin else None,
+                        cull_clouds=xin['cull_clouds'] if 'cull_clouds' in xin else None,
+                        renderer=getattr(G, 'renderer', None))
+
+
+def synthesize_planes(G, xin):
+    """The tri-planes ``get_eg3d_volume`` queries: ``G.f`` once to resolve ``ws``, then the backbone once (no grad)."""
     dev = next(G.parameters()).device if hasattr(G, 'parameters') else torch.device('cuda')
     with torch.no_grad():
         xin_ = _AttrDict({**xin, 'elevations': torch.zeros(1, device=dev), 'azimuths': torch.zeros(1, device=dev)})
@@ -98,8 +107,4 @@ def get_eg3d_volume(G, xin, resolution=256, max_batch=100000):
         ws = xin_['ws']
         planes = G.backbone.synthesis(ws, xin['cond'], update_emas=False, noise_mode='const')
         width = G.triplane_width * G.rendering_kwargs.get('triplane_depth', 1)
-        planes = planes.view(len(planes), 3, width, planes.shape[-2], planes.shape[-1])
-    return query_volume(planes, G.decoder, G.rendering_kwargs, resolution=resolution,
-                        triplane_crop=xin['triplane_crop'] if 'triplane_crop' in xin else None,
-                        cull_clouds=xin['cull_clouds'] if 'cull_clouds' in xin else None,
-                        renderer=getattr(G, 'renderer', None))
+        return planes.view(len(planes), 3, width, planes.shape[-2], planes.shape[-1])
