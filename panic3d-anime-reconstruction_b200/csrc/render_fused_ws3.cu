@@ -664,7 +664,9 @@ int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const vo
                             const float* u_f, const Workspace& ws, float* out_rgb, float* out_depth, float* out_wsum,
                             float* out_xyz, cudaStream_t stream) {
     if (!fused_ws3_supported(g)) {
-        set_error("fused warp-specialised renderer supports depth_resolution == depth_resolution_importance in {48, 96} (got %d, %d)", g.S, g.Sf);
+        set_error("fused warp-specialised renderer supports depth_resolution == depth_resolution_importance in {48, 96}, rays per "
+                  "view a multiple of 384 / depth_resolution, planes of at least 2x2 texels and strides that are multiples of "
+                  "8 elements (got %d + %d samples, %d rays, stride_col %lld)", g.S, g.Sf, g.M, (long long)g.stride_col);
         return P3D_EUNSUPPORTED;
     }
     const long long R = (long long)g.N * g.M;

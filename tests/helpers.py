@@ -41,6 +41,24 @@ def oracle_render(case, gather='manual'):
                       cull_clouds=case.get('cull_clouds'), binarize_clouds=case.get('binarize_clouds'), gather=gather)
 
 
+def profiled(fn):
+    """fn() and the number of launches per library profile slot it made (slots: csrc/p3d_common.cuh).  Profiling is
+    switched off again even when fn raises."""
+    import ctypes as C
+    from panic3d_b200 import _lib
+    L = _lib.lib()
+    L.p3d_profile_enable(1)
+    L.p3d_profile_read(None, None, 0, 1)
+    try:
+        out = fn()
+        torch.cuda.synchronize()
+        ms, n = (C.c_double * 8)(), (C.c_uint64 * 8)()
+        L.p3d_profile_read(ms, n, 8, 1)
+    finally:
+        L.p3d_profile_enable(0)
+    return out, list(n)
+
+
 def input_checksum(case):
     planes, dec, c2w, K, u_c, u_f, opts = build_case_inputs(case)
     return float(planes.double().sum() + u_c.double().sum() + dec['w1'].double().sum())

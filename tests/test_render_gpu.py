@@ -489,13 +489,16 @@ def test_ragged_sample_counts_match_oracle(S, Sf, M):
         assert (o.cpu() - o_ref).abs().max().item() < TIGHT
 
 
-def test_fused_handles_ray_counts_that_leave_partial_groups():
-    """M = 12 rays (3 fused groups of 4 at S=96) and N = 3 views: odd number of groups per CTA, tail tiles."""
+def test_fused_takes_whole_groups_only_and_auto_falls_back_otherwise():
+    """M = 12 rays (3 fused groups of 4 at S=96) and N = 3 views: nine CTAs of one group each, equal to the SIMT kernels.
+    M = 10 would leave a partial group per view, which the fused kernel does not take (a group reads one view's planes):
+    'auto' renders it with the SIMT kernels and a forced fused mode raises."""
+    from tests.helpers import profiled
     from panic3d_b200.training.volumetric_rendering.renderer import ImportanceRenderer
     dev = _dev()
-    planes, dec_m, ro, rd = _tiny(dev, N=3, M=12, P=16, seed=5)
     opts = dict(orc.DEFAULT_OPTS)
     g = torch.Generator().manual_seed(2)
+    planes, dec_m, ro, rd = _tiny(dev, N=3, M=12, P=16, seed=5)
     u_c, u_f = torch.rand(3, 12, 96, 1, generator=g), torch.rand(36, 96, generator=g)
     outs = []
     for mode in (0, 1):
@@ -506,6 +509,16 @@ def test_fused_handles_ray_counts_that_leave_partial_groups():
             outs.append(r(planes.to(dev), dec_m.to(dev), ro.to(dev), rd.to(dev), opts))
     for a_, b_ in zip(*outs):
         assert (a_ - b_).abs().max().item() < 1e-4
+
+    planes, dec_m, ro, rd = _tiny(dev, N=3, M=10, P=16, seed=6)
+    r = ImportanceRenderer(use_triplane=True)
+    with torch.no_grad():
+        _, n = profiled(lambda: r(planes.to(dev), dec_m.to(dev), ro.to(dev), rd.to(dev), opts))
+    assert n[5] == 0 and n[0] >= 1, 'M % 4 != 0 at 96+96 must render with the SIMT kernels under mlp_mode auto'
+    r.mlp_mode = 1
+    with pytest.raises(RuntimeError, match='fused'):
+        with torch.no_grad():
+            r(planes.to(dev), dec_m.to(dev), ro.to(dev), rd.to(dev), opts)
 
 
 def test_bad_inputs_raise():
