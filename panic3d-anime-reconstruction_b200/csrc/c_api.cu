@@ -64,8 +64,8 @@ int make_geom(const p3d_render_params* p, Geom* g) {
     memset(g, 0, sizeof(*g));
     g->N = p->n_views; g->M = p->n_rays; g->S = p->n_coarse; g->Sf = p->n_fine; g->H = p->plane_h; g->W = p->plane_w;
     g->stride_view = p->stride_view; g->stride_plane = p->stride_plane; g->stride_row = p->stride_row; g->stride_col = p->stride_col;
-    const int align = p->planes_bf16 ? 4 : 4;   // quads of 4 channels: 16 B (fp32) / 8 B (bf16) vector loads
-    P3D_REQUIRE(p->stride_view % align == 0 && p->stride_plane % align == 0 && p->stride_row % align == 0 && p->stride_col % align == 0,
+    // quads of 4 channels: 16 B (fp32) / 8 B (bf16) vector loads
+    P3D_REQUIRE(p->stride_view % 4 == 0 && p->stride_plane % 4 == 0 && p->stride_row % 4 == 0 && p->stride_col % 4 == 0,
                 "plane strides must be multiples of 4 elements");
     g->coord_scale = (float)(2.0 / p->box_warp);
     g->half_box = (float)(p->box_warp / 2.0);
@@ -489,16 +489,21 @@ int p3d_volume_query(const p3d_render_params* p, const void* planes, const float
     P3D_REQUIRE(cube_length > 0, "cube_length must be > 0");
     if (g.N == 0) return P3D_OK;
     P3D_REQUIRE(planes && w1 && b1 && w2 && b2 && out_sigma, "null pointer");
+    VolumeSpec vol;
+    vol.res = resolution;
+    vol.size = (float)(cube_length / (double)(resolution - 1));          // python float -> fp32 scalar operand
+    vol.origin = (float)(0.0 - cube_length / 2.0);
+    vol.crop = triplane_crop >= 0 ? (float)(p->box_warp / 2.0 - triplane_crop) : -1.f;    // renderer.py:139-148
+    vol.cull = cull_clouds >= 0 ? (float)cull_clouds : -1.f;
+    vol.crop_on = triplane_crop >= 0; vol.cull_on = cull_clouds >= 0;
     if (p->mlp_mode == P3D_MLP_TC_3XBF16 || p->mlp_mode == P3D_MLP_TC_BF16) {
         if (!decode_tc_supported(g, (long long)g.N * resolution * resolution * resolution)) {
             set_error("tensor-core volume query needs planes of at least 2x2 texels with non-negative strides below 2^31 elements per view");
             return P3D_EUNSUPPORTED;
         }
-        return volume_query_tc(g, p, planes, w1, b1, w2, b2, resolution, cube_length, triplane_crop, cull_clouds, out_sigma, out_rgb,
-                               out_density, out_coords, (cudaStream_t)stream);
+        return volume_query_tc(g, p, planes, w1, b1, w2, b2, vol, out_sigma, out_rgb, out_density, out_coords, (cudaStream_t)stream);
     }
-    return volume_query_v1(g, p, planes, w1, b1, w2, b2, resolution, cube_length, triplane_crop, cull_clouds, out_sigma,
-                           out_rgb, out_density, out_coords, (cudaStream_t)stream);
+    return volume_query_v1(g, p, planes, w1, b1, w2, b2, vol, out_sigma, out_rgb, out_density, out_coords, (cudaStream_t)stream);
 }
 
 int p3d_render_forward_host(const p3d_render_params* p_in, const float* planes_nchw, const float* w1, const float* b1,

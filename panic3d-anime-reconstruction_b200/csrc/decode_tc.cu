@@ -12,7 +12,6 @@
 //                          / cull overwrites and the lattice coordinates, written where the reference's reshape + flip puts them)
 //
 // A tile is 128 consecutive points; CTA b of the persistent grid takes tiles b, b + grid, ...
-#include <stdlib.h>
 #include "fused_common.cuh"
 
 namespace p3d {
@@ -27,7 +26,7 @@ constexpr int kWarpsD = kGW + kEW;
 constexpr int kThreadsD = kWarpsD * 32;          // 640
 constexpr int kNA = 4;                           // A1 ring depth
 constexpr int kD2Cols = 48;
-constexpr int kLBO_A1 = 2080, kLBO_W1 = 1024, kLBO_W2 = 768;
+constexpr int kLBO_W2 = 768;
 
 struct __align__(1024) DecSmem {
     unsigned char a1[kNA][2][4 * kLBO_A1];
@@ -46,10 +45,7 @@ struct DecArgs {
     long long total, per_view;
     int single_pass, n_tiles;
     int srow, scol, splane;
-    // volume mode (render_device.cuh: volume_point / volume_dest)
-    int vol_res;
-    float vol_size, vol_origin, vol_crop, vol_cull;
-    int vol_crop_on, vol_cull_on;
+    VolumeSpec vol;               // volume mode
 };
 
 template <bool BF16, bool VOLUME, int SCOL>
@@ -65,26 +61,9 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
         for (int i = 0; i < kNA; ++i) { mbar_init(&sm.a1_full[i], 4); mbar_init(&sm.a1_empty[i], kEW); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int i = tid; i < kHidden * kC; i += kThreadsD) {             // W1' = W1 * gain * log2(e) / 3   (64 x 32)
-        const int n = i / kC, k = i % kC;
-        unsigned short hi, lo;
-        split1(__fmul_rn(a.w1[i], g.w1_gain) * (kLog2e / 3.f), hi, lo);
-        const int off = tile_off(n, k, kLBO_W1);
-        *reinterpret_cast<unsigned short*>(sm.w1[0] + off) = hi;
-        *reinterpret_cast<unsigned short*>(sm.w1[1] + off) = lo;
-    }
-    for (int i = tid; i < kD2Cols * kHidden; i += kThreadsD) {        // rows 0..31: -W2 colour rows; row 32: W2 sigma row * ln2; 33..47: 0
-        const int n = i / kHidden, k = i % kHidden;
-        unsigned short hi = 0, lo = 0;
-        if (n < kRgb) split1(-__fmul_rn(a.w2[(n + 1) * kHidden + k], g.w2_gain), hi, lo);
-        else if (n == kRgb) split1(__fmul_rn(a.w2[k], g.w2_gain) * kLn2, hi, lo);
-        const int off = tile_off(n, k, kLBO_W2);
-        *reinterpret_cast<unsigned short*>(sm.w2[0] + off) = hi;
-        *reinterpret_cast<unsigned short*>(sm.w2[1] + off) = lo;
-    }
-    if (tid < kHidden) sm.b1[tid] = __fmul_rn(a.b1[tid], g.b1_gain) * kLog2e;
-    if (tid < kRgb) sm.b2c[tid] = -__fmul_rn(a.b2[tid + 1], g.b2_gain) * kLog2e;
-    if (tid == 0) sm.b2s = __fmul_rn(a.b2[0], g.b2_gain);
+    stage_w1_biases(g, a.w1, a.b1, a.b2, sm.w1, sm.b1, sm.b2c, sm.b2s, tid, kThreadsD);
+    // tile rows 0..31: the colour rows; row 32: the sigma row; 33..47: zeros
+    stage_w2(g, a.w2, sm.w2, kD2Cols, kLBO_W2, [](int n) { return n < kRgb ? n + 1 : (n == kRgb ? 0 : -1); }, tid, kThreadsD);
     fence_proxy_async();
     __syncthreads();
 
@@ -94,77 +73,30 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
         constexpr int kEsz = BF16 ? 2 : 4;
         const long long scolB = (long long)a.scol * kEsz, srowB = (long long)a.srow * kEsz;
         unsigned char* tab = reinterpret_cast<unsigned char*>(sm.tab[gw]);
-        float v4[12][4];
+        float v[12][4];
 #pragma unroll
         for (int k = 0; k < 12; ++k)
 #pragma unroll
-            for (int c = 0; c < 4; ++c) v4[k][c] = 0.f;
-        const int sub = lane >> 3, qd = lane & 7;
-        constexpr int kImmX4 = SCOL * kEsz;
+            for (int c = 0; c < 4; ++c) v[k][c] = 0.f;
         for (int it = team; it < n_my; it += kTeams) {
             const long long tile = (long long)blockIdx.x + (long long)it * gridDim.x;
             // ---- tap table of this warp's 32 points: lane = point
-            long long view_w = 0;
             {
                 const long long gidx = tile * 128 + wt * 32 + lane;
                 float px = 1e30f, py = 1e30f, pz = 1e30f;
+                long long view = 0;
                 if (gidx < a.total) {
-                    const long long view = gidx / a.per_view;
-                    if (VOLUME) volume_point(gidx - view * a.per_view, a.vol_res, a.vol_size, a.vol_origin, px, py, pz);
+                    view = gidx / a.per_view;
+                    if (VOLUME) volume_point(gidx - view * a.per_view, a.vol.res, a.vol.size, a.vol.origin, px, py, pz);
                     else { px = a.coords[gidx * 3]; py = a.coords[gidx * 3 + 1]; pz = a.coords[gidx * 3 + 2]; }
-                    view_w = view;
                 }
-                const bool pm = g.plane_mode == P3D_PLANES_PANIC3D;
-                uint32_t o0, o1, o2;
-                float4 w0, w1, w2;
-                const bool f0 = plane_taps_rec(g, a.srow, a.scol, 0, px, py, o0, w0);
-                const bool f1 = plane_taps_rec(g, a.srow, a.scol, a.splane, px, pz, o1, w1);
-                const bool f2 = plane_taps_rec(g, a.srow, a.scol, 2 * a.splane, pm ? py : pz, pm ? pz : px, o2, w2);
-                // a tile may straddle two views: the view index travels with the row (bits 8.. of the flags word)
-                *reinterpret_cast<uint4*>(tab + tab_off(lane, 0)) = make_uint4(o0, o1, o2, (f0 ? 1u : 0u) | (f1 ? 2u : 0u) | (f2 ? 4u : 0u) | ((uint32_t)view_w << 8));
-                *reinterpret_cast<float4*>(tab + tab_off(lane, 1)) = w0;
-                *reinterpret_cast<float4*>(tab + tab_off(lane, 2)) = w1;
-                *reinterpret_cast<float4*>(tab + tab_off(lane, 3)) = w2;
+                write_tap_row(tab, lane, g, a.srow, a.scol, a.splane, px, py, pz, (uint32_t)view);   // a tile may straddle two views
             }
             __syncwarp();
             const int stage = it % kNA;
             mbar_wait(&sm.a1_empty[stage], ((it / kNA) & 1) ^ 1);
-            unsigned char* a1h = sm.a1[stage][0];
-            unsigned char* a1l = sm.a1[stage][1];
-            const char* pq = reinterpret_cast<const char*>(a.planes) + (long long)(4 * qd) * kEsz;
-#pragma unroll 1
-            for (int round = 0; round < 8; ++round) {
-                const int lrow = round * 4 + sub;
-                const uint4 c0 = *reinterpret_cast<const uint4*>(tab + tab_off(lrow, 0));
-                const bool p0 = c0.w & 1u, p1 = c0.w & 2u, p2 = c0.w & 4u;
-                const char* vq4 = pq + (long long)(c0.w >> 8) * g.stride_view * kEsz;
-                const char* b0 = vq4 + (unsigned long long)c0.x * kEsz;
-                const char* b1 = vq4 + (unsigned long long)c0.y * kEsz;
-                const char* b2 = vq4 + (unsigned long long)c0.z * kEsz;
-#define P3D_LD4(k, base, pr)                                                                                         \
-                load_quad_p<BF16, 0>(v4[k], base, pr);                                                                \
-                if (SCOL) load_quad_p<BF16, kImmX4>(v4[k + 1], base, pr); else load_quad_p<BF16, 0>(v4[k + 1], base + scolB, pr); \
-                load_quad_p<BF16, 0>(v4[k + 2], base + srowB, pr);                                                    \
-                if (SCOL) load_quad_p<BF16, kImmX4>(v4[k + 3], base + srowB, pr); else load_quad_p<BF16, 0>(v4[k + 3], base + srowB + scolB, pr);
-                P3D_LD4(0, b0, p0)
-                P3D_LD4(4, b1, p1)
-                P3D_LD4(8, b2, p2)
-#undef P3D_LD4
-                const float4 w0 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 1));
-                const float4 w1 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 2));
-                const float4 w2 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 3));
-                float acc[4] = {0.f, 0.f, 0.f, 0.f};
-                fma4(acc, v4[0], w0.x); fma4(acc, v4[1], w0.y); fma4(acc, v4[2], w0.z); fma4(acc, v4[3], w0.w);
-                fma4(acc, v4[4], w1.x); fma4(acc, v4[5], w1.y); fma4(acc, v4[6], w1.z); fma4(acc, v4[7], w1.w);
-                fma4(acc, v4[8], w2.x); fma4(acc, v4[9], w2.y); fma4(acc, v4[10], w2.z); fma4(acc, v4[11], w2.w);
-                uint32_t h[2], l[2];
-                split2(acc[0], acc[1], h[0], l[0]);
-                split2(acc[2], acc[3], h[1], l[1]);
-                const int trow = wt * 32 + lrow;
-                const int off = (trow >> 3) * kSBO + (qd >> 1) * kLBO_A1 + (trow & 7) * 16 + (qd & 1) * 8;
-                *reinterpret_cast<uint2*>(a1h + off) = make_uint2(h[0], h[1]);
-                *reinterpret_cast<uint2*>(a1l + off) = make_uint2(l[0], l[1]);
-            }
+            gather_a1<BF16, SCOL>(tab, reinterpret_cast<const char*>(a.planes), g.stride_view * kEsz, srowB, scolB, v, sm.a1[stage][0],
+                                  sm.a1[stage][1], wt, lane);
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) mbar_arrive(&sm.a1_full[stage]);
@@ -198,7 +130,7 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
                 if (VOLUME) {
                     const long long view = gidx / a.per_view;
                     n = gidx - view * a.per_view;
-                    dest = view * a.per_view + volume_dest(n, a.vol_res);
+                    dest = view * a.per_view + volume_dest(n, a.vol.res);
                 }
                 if (a.out_rgb) {
 #pragma unroll
@@ -217,18 +149,13 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
                     const float sg = d2[16 + 2 * rs] + sm.b2s;
                     a.out_sigma[dest] = sg;
                     if (VOLUME && a.out_density) {
-                        // sigma2density, then the crop / cull overwrites; the reference applies cull_clouds_mask to the DENSITIES
-                        // (eg3d_metrics3d.py:155-162 -> renderer.py:150-153): the threshold acts on the twice-transformed value
                         float x, y, z;
-                        volume_point(n, a.vol_res, a.vol_size, a.vol_origin, x, y, z);
-                        float dens = 1.f - expf(-softplus_t(__fsub_rn(sg, 1.f)));
-                        if (a.vol_crop_on && !((fabsf(x) <= a.vol_crop) && (fabsf(z) <= a.vol_crop))) dens = -1e3f;
-                        if (a.vol_cull_on && (1.f - expf(-softplus_t(__fsub_rn(dens, 1.f)))) < a.vol_cull) dens = -1e3f;
-                        a.out_density[dest] = dens;
+                        volume_point(n, a.vol.res, a.vol.size, a.vol.origin, x, y, z);
+                        a.out_density[dest] = volume_density(a.vol, sg, x, z);
                     }
                 } else if (VOLUME && a.out_coords && (lane & 3) == 1) {
                     float x, y, z;
-                    volume_point(n, a.vol_res, a.vol_size, a.vol_origin, x, y, z);
+                    volume_point(n, a.vol.res, a.vol.size, a.vol.origin, x, y, z);
                     a.out_coords[dest * 3 + 0] = x; a.out_coords[dest * 3 + 1] = y; a.out_coords[dest * 3 + 2] = z;
                 }
             }
@@ -238,20 +165,15 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
 
 template <bool VOLUME>
 int launch_decode(const Geom& g, const p3d_render_params* p, DecArgs& a, cudaStream_t stream) {
-    static int n_sm = 0;
-    if (!n_sm) {
-        int dev = 0;
-        P3D_CUDA_TRY(cudaGetDevice(&dev));
-        P3D_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    }
+    int n_sm, rc;
+    if ((rc = sm_count(&n_sm))) return rc;
     a.g = g;
     a.single_pass = p->mlp_mode == P3D_MLP_TC_BF16;
     a.srow = (int)g.stride_row; a.scol = (int)g.stride_col; a.splane = (int)g.stride_plane;
     a.n_tiles = (int)((a.total + 127) / 128);
-    const int sc = g.stride_col == kC ? 1 : (g.stride_col == 3 * kC ? 2 : 0);      // static texel stride: layout pre-pass / zero-copy channels_last
-#define P3D_PICK(BF) (sc == 1 ? k_decode_tc<BF, VOLUME, kC> : (sc == 2 ? k_decode_tc<BF, VOLUME, 3 * kC> : k_decode_tc<BF, VOLUME, 0>))
-    void (*kern)(DecArgs) = p->planes_bf16 ? P3D_PICK(true) : P3D_PICK(false);
-#undef P3D_PICK
+    void (*kern)(DecArgs) = with_texel_stride(g, [&](auto sc) -> void (*)(DecArgs) {
+        return p->planes_bf16 ? k_decode_tc<true, VOLUME, sc.value> : k_decode_tc<false, VOLUME, sc.value>;
+    });
     const size_t smem = sizeof(DecSmem) + 1024;
     P3D_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = a.n_tiles < n_sm ? a.n_tiles : n_sm;
@@ -263,11 +185,9 @@ int launch_decode(const Geom& g, const p3d_render_params* p, DecArgs& a, cudaStr
 
 }  // namespace
 
-// 32-bit tap offsets inside one view's tri-plane, 2 x 2 footprints clamped into the plane, 16-byte vector loads
+// int tile indices, and the view index in the 24 high bits of a tap row's flags
 bool decode_tc_supported(const Geom& g, long long total) {
-    const long long span = 2 * g.stride_plane + (long long)(g.H - 1) * g.stride_row + (long long)(g.W - 1) * g.stride_col + kC;
-    if (g.H < 2 || g.W < 2 || total >= (128ll << 31) || g.N >= (1 << 24)) return false;
-    return g.stride_plane >= 0 && g.stride_row >= 0 && g.stride_col >= 0 && span < (1ll << 31);
+    return total < (128ll << 31) && g.N < (1 << 24) && tap_offsets_fit(g);
 }
 
 int decode_points_tc(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
@@ -281,18 +201,13 @@ int decode_points_tc(const Geom& g, const p3d_render_params* p, const void* plan
 }
 
 int volume_query_tc(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
-                    const float* w2, const float* b2, int res, double cube_length, double triplane_crop, double cull_clouds,
-                    float* out_sigma, float* out_rgb, float* out_density, float* out_coords, cudaStream_t stream) {
+                    const float* w2, const float* b2, const VolumeSpec& vol, float* out_sigma, float* out_rgb,
+                    float* out_density, float* out_coords, cudaStream_t stream) {
     DecArgs a{};
     a.planes = planes; a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2;
     a.out_sigma = out_sigma; a.out_rgb = out_rgb; a.out_density = out_density; a.out_coords = out_coords;
-    a.per_view = (long long)res * res * res; a.total = (long long)g.N * a.per_view;
-    a.vol_res = res;
-    a.vol_size = (float)(cube_length / (double)(res - 1));          // python float -> fp32 scalar operand
-    a.vol_origin = (float)(0.0 - cube_length / 2.0);
-    a.vol_crop = triplane_crop >= 0 ? (float)(p->box_warp / 2.0 - triplane_crop) : -1.f;    // renderer.py:139-148
-    a.vol_cull = cull_clouds >= 0 ? (float)cull_clouds : -1.f;
-    a.vol_crop_on = triplane_crop >= 0; a.vol_cull_on = cull_clouds >= 0;
+    a.per_view = (long long)vol.res * vol.res * vol.res; a.total = (long long)g.N * a.per_view;
+    a.vol = vol;
     return launch_decode<true>(g, p, a, stream);
 }
 

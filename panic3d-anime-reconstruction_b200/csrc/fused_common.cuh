@@ -1,6 +1,7 @@
 // PTX wrappers (mbarrier, Hopper wgmma) and the tri-plane gather / decoder helpers shared by the fused tensor-core
 // kernels: render_fused_ws3.cu (the renderer) and decode_tc.cu (point / volume decode).
 #pragma once
+#include <type_traits>
 #include "render_device.cuh"
 
 namespace p3d {
@@ -9,6 +10,7 @@ namespace fused {
 using namespace dev;
 
 constexpr int kSBO = 128;                        // byte distance between 8-row groups of a K-major no-swizzle wgmma operand tile
+constexpr int kLBO_A1 = 2080, kLBO_W1 = 1024;    // byte distance between K groups of the A1 tile (128 x 32) / the W1' tile (64 x 32)
 constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
 
 // ------------------------------------------------------------------------------------------ PTX
@@ -96,6 +98,45 @@ __device__ __forceinline__ void split1(float x, unsigned short& hi, unsigned sho
 }
 __device__ __forceinline__ int tile_off(int row, int k, int lbo) { return (row >> 3) * kSBO + (k >> 3) * lbo + (row & 7) * 16 + (k & 7) * 2; }
 
+// ------------------------------------------------------------------------------------------ decoder weights
+// The tensor-core decoder runs in base 2 (decoder_hidden's softplus2, the epilogues' ex2), so the weights are staged with the
+// scale factors folded in:
+//   W1' = W1 * gain * log2(e) / 3 (the 1/3 is the plane mean)       b1' = b1 * gain * log2(e)
+//   colour rows 1..32 of W2: -W2 * gain                               colour biases: -b2 * gain * log2(e)
+//   sigma row 0 of W2: W2 * gain * ln 2                               sigma bias: b2 * gain
+// so a colour is rcp(1 + ex2(logit')) and sigma is the plain sum.  Weights are split into bf16 hi / lo K-major tiles.
+template <int B>
+__device__ __forceinline__ void put_weight(unsigned char (&tile)[2][B], int row, int k, int lbo, float w) {
+    unsigned short hi, lo;
+    split1(w, hi, lo);
+    const int off = tile_off(row, k, lbo);
+    *reinterpret_cast<unsigned short*>(tile[0] + off) = hi;
+    *reinterpret_cast<unsigned short*>(tile[1] + off) = lo;
+}
+// W1' (64 x 32) and all biases; threads tid = 0 .. nthreads - 1 share the work
+template <int B>
+__device__ __forceinline__ void stage_w1_biases(const Geom& g, const float* w1, const float* b1, const float* b2, unsigned char (&sw1)[2][B],
+                                                float* sb1, float* sb2c, float& sb2s, int tid, int nthreads) {
+    for (int i = tid; i < kHidden * kC; i += nthreads) put_weight(sw1, i / kC, i % kC, kLBO_W1, __fmul_rn(w1[i], g.w1_gain) * (kLog2e / 3.f));
+    if (tid < kHidden) sb1[tid] = __fmul_rn(b1[tid], g.b1_gain) * kLog2e;
+    if (tid < kRgb) sb2c[tid] = -__fmul_rn(b2[tid + 1], g.b2_gain) * kLog2e;
+    if (tid == 0) sb2s = __fmul_rn(b2[0], g.b2_gain);
+}
+// rows [0, rows) of a layer-2 weight tile (K = 64): tile row n holds W2 row w2_row(n) (0 = sigma, 1..32 = colours, -1 = zeros)
+template <int B, class RowMap>
+__device__ __forceinline__ void stage_w2(const Geom& g, const float* w2, unsigned char (&tile)[2][B], int rows, int lbo, RowMap w2_row,
+                                         int tid, int nthreads) {
+    for (int i = tid; i < rows * kHidden; i += nthreads) {
+        const int n = i / kHidden, k = i % kHidden, r = w2_row(n);
+        float w = 0.f;
+        if (r >= 0) {
+            const float wg = __fmul_rn(w2[r * kHidden + k], g.w2_gain);
+            w = r == 0 ? wg * kLn2 : -wg;
+        }
+        put_weight(tile, n, k, lbo, w);
+    }
+}
+
 // ------------------------------------------------------------------------------------------ gather
 // Tap table: one 64 B record per row - chunk 0 = {o[0], o[1], o[2], flags}, chunk 1+p = the four bilinear weights of plane p
 // (w00, w01, w10, w11; rows y, y+1 x columns x, x+1) - chunk c of row r stored at position c ^ ((r >> 1) & 3), which makes
@@ -107,22 +148,28 @@ __device__ __forceinline__ int tile_off(int row, int k, int lbo) { return (row >
 // plane whose bit is clear are predicated off (its registers keep older, finite texel values that meet weights of 0).
 __device__ __forceinline__ uint32_t tab_off(int row, int chunk) { return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4)); }
 
-__device__ __forceinline__ bool plane_taps_rec(const Geom& g, int srow, int scol, int pbase, float ca, float cb, uint32_t& o, float4& w) {
-    const float gx = __fmul_rn(ca, g.coord_scale), gy = __fmul_rn(cb, g.coord_scale);
-    const float fx = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)g.W), 1.f), 0.5f);
-    const float fy = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)g.H), 1.f), 0.5f);
-    const bool sane = (fx > -2.f) && (fx < (float)g.W + 1.f) && (fy > -2.f) && (fy < (float)g.H + 1.f);   // false for NaN too
-    const float x0f = floorf(fx), y0f = floorf(fy);
-    const float wx1 = fx - x0f, wy1 = fy - y0f;
-    const float wx0 = 1.f - wx1, wy0 = 1.f - wy1;
-    const int x0 = sane ? (int)x0f : -4, y0 = sane ? (int)y0f : -4;
-    const int xa = min(max(x0, 0), g.W - 2), ya = min(max(y0, 0), g.H - 2);
-    const int dx = x0 - xa, dy = y0 - ya;                     // 0 inside, -1 / +1: the footprint hangs over the low / high edge
-    const float wl = dx == 0 ? wx0 : (dx == -1 ? wx1 : 0.f), wr = dx == 0 ? wx1 : (dx == 1 ? wx0 : 0.f);
-    const float wt = dy == 0 ? wy0 : (dy == -1 ? wy1 : 0.f), wb = dy == 0 ? wy1 : (dy == 1 ? wy0 : 0.f);
+__device__ __forceinline__ bool plane_taps_rec(const Geom& g, int srow, int scol, int pbase, float2 c, uint32_t& o, float4& w) {
+    const Footprint f = bilinear_footprint(g, c.x, c.y);
+    const int xa = min(max(f.x0, 0), g.W - 2), ya = min(max(f.y0, 0), g.H - 2);
+    const int dx = f.x0 - xa, dy = f.y0 - ya;                 // 0 inside, -1 / +1: the footprint hangs over the low / high edge
+    const float wl = dx == 0 ? f.wx0 : (dx == -1 ? f.wx1 : 0.f), wr = dx == 0 ? f.wx1 : (dx == 1 ? f.wx0 : 0.f);
+    const float wt = dy == 0 ? f.wy0 : (dy == -1 ? f.wy1 : 0.f), wb = dy == 0 ? f.wy1 : (dy == 1 ? f.wy0 : 0.f);
     o = (uint32_t)(pbase + ya * srow + xa * scol);
     w = make_float4(wl * wt, wr * wt, wl * wb, wr * wb);
     return ((unsigned)(dx + 1) < 3u) && ((unsigned)(dy + 1) < 3u);
+}
+// tap-table row `row` for the point (x, y, z); `view` goes to bits 8.. of the flags word (0 when the caller knows the view)
+__device__ __forceinline__ void write_tap_row(unsigned char* tab, int row, const Geom& g, int srow, int scol, int splane, float x, float y,
+                                              float z, uint32_t view) {
+    uint32_t o0, o1, o2;
+    float4 w0, w1, w2;
+    const bool f0 = plane_taps_rec(g, srow, scol, 0, plane_coords(g, 0, x, y, z), o0, w0);
+    const bool f1 = plane_taps_rec(g, srow, scol, splane, plane_coords(g, 1, x, y, z), o1, w1);
+    const bool f2 = plane_taps_rec(g, srow, scol, 2 * splane, plane_coords(g, 2, x, y, z), o2, w2);
+    *reinterpret_cast<uint4*>(tab + tab_off(row, 0)) = make_uint4(o0, o1, o2, (f0 ? 1u : 0u) | (f1 ? 2u : 0u) | (f2 ? 4u : 0u) | (view << 8));
+    *reinterpret_cast<float4*>(tab + tab_off(row, 1)) = w0;
+    *reinterpret_cast<float4*>(tab + tab_off(row, 2)) = w1;
+    *reinterpret_cast<float4*>(tab + tab_off(row, 3)) = w2;
 }
 // four consecutive channels of one texel (16 B fp32 / 8 B bf16) at addr + IMM bytes, predicated; v keeps its old value when !pred
 template <bool BF16, int IMM>
@@ -140,6 +187,49 @@ __device__ __forceinline__ void load_quad_p(float (&v)[4], const char* addr, boo
 __device__ __forceinline__ void fma4(float (&acc)[4], const float (&v)[4], float w) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[j] = fmaf(v[j], w, acc[j]);
+}
+// The tap table of one gather warp -> rows [32 wt, 32 wt + 32) of an A1 stage (bf16 hi / lo planes a1h / a1l).  8 rounds of 4
+// rows: lane (sub, qd) loads channels [4 qd, 4 qd + 4) of the 12 taps of row 4 round + sub - twelve 128-bit loads in flight
+// per lane, each warp-wide load covers four whole 128 B texels (one L1 wavefront per texel) - and lerps them with one FMA
+// chain.  A row's view starts at `planes` + (flags >> 8) * view_bytes.  SCOL != 0 is the texel stride in elements, which
+// makes the x + 1 texel an immediate offset.  v: the caller's texel registers, zeroed once (a plane whose loads are predicated
+// off keeps older, finite values, which meet weights of 0).
+template <bool BF16, int SCOL>
+__device__ __forceinline__ void gather_a1(const unsigned char* tab, const char* planes, long long view_bytes, long long srowB, long long scolB,
+                                          float (&v)[12][4], unsigned char* a1h, unsigned char* a1l, int wt, int lane) {
+    constexpr int kEsz = BF16 ? 2 : 4;
+    constexpr int kImmX4 = SCOL * kEsz;
+    const int sub = lane >> 3, qd = lane & 7;
+    const char* pq = planes + (long long)(4 * qd) * kEsz;
+#pragma unroll 1
+    for (int round = 0; round < 8; ++round) {
+        const int lrow = round * 4 + sub;
+        const uint4 c0 = *reinterpret_cast<const uint4*>(tab + tab_off(lrow, 0));
+        const char* vq4 = pq + (long long)(c0.w >> 8) * view_bytes;
+        const uint32_t o[3] = {c0.x, c0.y, c0.z};
+#pragma unroll
+        for (int p = 0; p < 3; ++p) {
+            const bool pr = c0.w & (1u << p);
+            const char* b = vq4 + (unsigned long long)o[p] * kEsz;
+            load_quad_p<BF16, 0>(v[4 * p], b, pr);
+            if (SCOL) load_quad_p<BF16, kImmX4>(v[4 * p + 1], b, pr); else load_quad_p<BF16, 0>(v[4 * p + 1], b + scolB, pr);
+            load_quad_p<BF16, 0>(v[4 * p + 2], b + srowB, pr);
+            if (SCOL) load_quad_p<BF16, kImmX4>(v[4 * p + 3], b + srowB, pr); else load_quad_p<BF16, 0>(v[4 * p + 3], b + srowB + scolB, pr);
+        }
+        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int p = 0; p < 3; ++p) {
+            const float4 w = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 1 + p));
+            fma4(acc, v[4 * p], w.x); fma4(acc, v[4 * p + 1], w.y); fma4(acc, v[4 * p + 2], w.z); fma4(acc, v[4 * p + 3], w.w);
+        }
+        uint32_t h[2], l[2];
+        split2(acc[0], acc[1], h[0], l[0]);
+        split2(acc[2], acc[3], h[1], l[1]);
+        const int trow = wt * 32 + lrow;
+        const int off = (trow >> 3) * kSBO + (qd >> 1) * kLBO_A1 + (trow & 7) * 16 + (qd & 1) * 8;
+        *reinterpret_cast<uint2*>(a1h + off) = make_uint2(h[0], h[1]);
+        *reinterpret_cast<uint2*>(a1l + off) = make_uint2(l[0], l[1]);
+    }
 }
 
 // ------------------------------------------------------------------------------------------ decoder (one warpgroup, 64 rows)
@@ -201,4 +291,32 @@ __device__ __forceinline__ void decoder_layer2_issue(float (&d)[N / 2], const ui
 }
 
 }  // namespace fused
+
+// ------------------------------------------------------------------------------------------ host side of both fused kernels
+// SM count of the current device, read once: both kernels run a persistent grid of at most one CTA per SM
+inline int sm_count(int* n) {
+    static int n_sm = 0;
+    if (!n_sm) {
+        int dev = 0;
+        P3D_CUDA_TRY(cudaGetDevice(&dev));
+        P3D_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    }
+    *n = n_sm;
+    return P3D_OK;
+}
+// The texel stride the gather takes as a template argument (SCOL): kC (the layout pre-pass: one plane's texels contiguous),
+// 3 kC (a (N,96,H,W) channels_last backbone output consumed zero-copy) or 0 (any other stride, read at run time).
+// pick(std::integral_constant<int, SCOL>) returns the kernel instantiation.
+template <class Pick>
+auto with_texel_stride(const Geom& g, Pick pick) {
+    if (g.stride_col == kC) return pick(std::integral_constant<int, kC>{});
+    if (g.stride_col == 3 * kC) return pick(std::integral_constant<int, 3 * kC>{});
+    return pick(std::integral_constant<int, 0>{});
+}
+// The tap table holds 32-bit element offsets inside one view's tri-plane and 2 x 2 footprints clamped into the plane
+inline bool tap_offsets_fit(const Geom& g) {
+    const long long span = 2 * g.stride_plane + (long long)(g.H - 1) * g.stride_row + (long long)(g.W - 1) * g.stride_col + kC;
+    return g.H >= 2 && g.W >= 2 && g.stride_plane >= 0 && g.stride_row >= 0 && g.stride_col >= 0 && span < (1ll << 31);
+}
+
 }  // namespace p3d

@@ -49,25 +49,7 @@ __global__ void __launch_bounds__(128) k_ray_backward(const RayBwdArgs a) {
     float* q = Tr + L;            // g_rgb . c_j per merged sample, later dL/dsigmabar_i
     int* src = reinterpret_cast<int*>(q + L);
 
-    const float* tc = a.depth_c + ray * S;
-    const float* tf = a.depth_f + ray * Sf;
-    const bool rev = tc[0] > tc[S - 1];
-    for (int i = lane; i < S; i += 32) {
-        const int ci = rev ? S - 1 - i : i;
-        const float v = tc[ci];
-        int lo = 0, hi = Sf;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (tf[mid] < v) lo = mid + 1; else hi = mid; }
-        const int pos = i + lo;
-        t[pos] = v; sg[pos] = a.sigma_c[ray * S + ci]; src[pos] = ci;
-    }
-    for (int j = lane; j < Sf; j += 32) {
-        const float v = tf[j];
-        int lo = 0, hi = S;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (tc[rev ? S - 1 - mid : mid] <= v) lo = mid + 1; else hi = mid; }
-        const int pos = j + lo;
-        t[pos] = v; sg[pos] = a.sigma_f[ray * Sf + j]; src[pos] = S + j;
-    }
-    __syncwarp();
+    merge_by_rank(a.depth_c + ray * S, a.sigma_c + ray * S, a.depth_f + ray * Sf, a.sigma_f + ray * Sf, S, Sf, t, sg, src, lane);
     // forward quantities per interval
     float carry = 1.f, acc_w = 0.f, acc_d = 0.f;
     for (int base = 0; base < L - 1; base += 32) {
@@ -176,20 +158,14 @@ constexpr int kXs = 33, kHs = 65, kDs = 36;
 constexpr size_t kBwdSmemFloats = (size_t)kHidden * kC + kOut * kHidden + kHidden + 36 +
                                   (size_t)kT * (kXs + kHs + kHs + kDs + kHs + kXs) + kT * 12 * 2 + kT * 2 + kT;
 
-// texel indices (p*H*W + y*W + x, or -1) and bilinear weights of one plane; same arithmetic as dev::plane_taps
-__device__ __forceinline__ void tap_texels(const Geom& g, int plane, float ca, float cb, int2* out) {
-    const float gx = __fmul_rn(ca, g.coord_scale), gy = __fmul_rn(cb, g.coord_scale);
-    const float fx = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)g.W), 1.f), 0.5f);
-    const float fy = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)g.H), 1.f), 0.5f);
-    const bool sane = (fx > -2.f) && (fx < (float)g.W + 1.f) && (fy > -2.f) && (fy < (float)g.H + 1.f);
-    const float x0f = floorf(fx), y0f = floorf(fy);
-    const float wx1 = fx - x0f, wy1 = fy - y0f, wx0 = 1.f - wx1, wy0 = 1.f - wy1;
-    const int x0 = sane ? (int)x0f : -4, y0 = sane ? (int)y0f : -4;
+// texel indices (p*H*W + y*W + x, or -1) and bilinear weights of one plane, from the forward's dev::bilinear_footprint
+__device__ __forceinline__ void tap_texels(const Geom& g, int plane, float2 c, int2* out) {
+    const Footprint f = bilinear_footprint(g, c.x, c.y);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const int xi = x0 + (k & 1), yi = y0 + (k >> 1);
+        const int xi = f.x0 + (k & 1), yi = f.y0 + (k >> 1);
         const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H);
-        const float wgt = ((k & 1) ? wx1 : wx0) * ((k >> 1) ? wy1 : wy0);
+        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);
         out[k] = make_int2(ok ? (plane * g.H + yi) * g.W + xi : -1, __float_as_int(ok ? wgt : 0.f));
     }
 }
@@ -237,21 +213,14 @@ __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
                 } else {
                     const long long ray = gidx / a.per_ray;
                     view = (int)(ray / g.M);
-                    const float tval = a.depth[gidx];
-                    const float* o = a.ro + ray * 3;
-                    const float* d = a.rd + ray * 3;
-                    px = __fadd_rn(o[0], __fmul_rn(tval, d[0]));
-                    py = __fadd_rn(o[1], __fmul_rn(tval, d[1]));
-                    pz = __fadd_rn(o[2], __fmul_rn(tval, d[2]));
+                    const float3 pt = ray_point(a.ro + ray * 3, a.rd + ray * 3, a.depth[gidx]);
+                    px = pt.x; py = pt.y; pz = pt.z;
                 }
                 f = gather_features<BF16>(a.planes, g, view, px, py, pz, qd);
             }
             if (qd < 3) {                                         // lanes 0..2 of a sample record plane qd's taps
                 if (ok) {
-                    const bool pm = g.plane_mode == P3D_PLANES_PANIC3D;
-                    const float ca = qd == 2 ? (pm ? py : pz) : px;
-                    const float cb = qd == 0 ? py : (qd == 1 ? pz : (pm ? pz : px));
-                    tap_texels(g, qd, ca, cb, s_tap + local * 12 + qd * 4);
+                    tap_texels(g, qd, plane_coords(g, qd, px, py, pz), s_tap + local * 12 + qd * 4);
                 } else {
 #pragma unroll
                     for (int k = 0; k < 4; ++k) s_tap[local * 12 + qd * 4 + k] = make_int2(-1, 0);

@@ -28,6 +28,23 @@ __device__ __forceinline__ float coarse_depth(const Geom& g, int s, float u, flo
                             : __fsub_rn(g.ray_end, __fmul_rn(g.lin_step, (float)(S - 1 - s)));
     return __fadd_rn(lin, __fmul_rn(u, g.depth_delta));
 }
+// coarse_depth with the ray's 'auto' limits: a ray that misses the box takes the smallest and largest valid start of the
+// whole batch (bounds[2..3], when bounds[4] says there is one).  renderer.py:165-170.  A dead row (live == false) reads
+// no limits.
+__device__ __forceinline__ float coarse_sample_depth(const Geom& g, int s, float u, long long ray, bool live, const float* ray_t0,
+                                                     const float* ray_t1, const unsigned int* bounds) {
+    float t0 = 0.f, t1 = 0.f;
+    if (g.ray_mode == P3D_RAYS_AUTOBOX && live) {
+        t0 = ray_t0[ray]; t1 = ray_t1[ray];
+        if (!(t1 > t0) && bounds[4]) { t0 = ordered_to_float(bounds[2]); t1 = ordered_to_float(bounds[3]); }
+    }
+    return coarse_depth(g, s, u, t0, t1);
+}
+
+// o + t d, rounded per operation like the reference's ATen ops (no FMA contraction)
+__device__ __forceinline__ float3 ray_point(const float* o, const float* d, float t) {
+    return make_float3(__fadd_rn(o[0], __fmul_rn(t, d[0])), __fadd_rn(o[1], __fmul_rn(t, d[1])), __fadd_rn(o[2], __fmul_rn(t, d[2])));
+}
 
 // -------------------------------------------------------------------------------------------
 // Grid point n of the reference's create_samples (eg3d_metrics3d.py:70-92), bit for bit: the z index is the integer
@@ -53,6 +70,15 @@ __device__ __forceinline__ long long volume_dest(long long n, int R) {
     const long long a = n / rr, rest = n - a * rr;
     return ((long long)(R - 1) - a) * rr + rest;
 }
+// The volume query's density at a lattice point (x, z): sigma2density (eg3d_metrics3d.py:65-69), then crop / cull write -1e3
+// (:155-162).  The reference hands the DENSITIES to cull_clouds_mask, which applies softplus(. - 1) -> 1 - exp(-.) once more
+// (renderer.py:150-153): the threshold acts on the twice-transformed value.
+__device__ __forceinline__ float volume_density(const VolumeSpec& v, float sigma, float x, float z) {
+    float dens = 1.f - expf(-softplus_t(__fsub_rn(sigma, 1.f)));
+    if (v.crop_on && !((fabsf(x) <= v.crop) && (fabsf(z) <= v.crop))) dens = -1e3f;
+    if (v.cull_on && (1.f - expf(-softplus_t(__fsub_rn(dens, 1.f)))) < v.cull) dens = -1e3f;
+    return dens;
+}
 
 // -------------------------------------------------------------------------------------------
 // Tri-plane bilinear gather for one sample, channels [4q, 4q+4).  renderer.py:52-81:
@@ -76,26 +102,46 @@ __device__ __forceinline__ float4 load_quad(const void* planes, long long elem_o
     }
 }
 
-struct Tap4 {
-    long long off[4];
-    float w[4];
-};
+// Coordinates (a, b) of a point on plane p: (x, y), (x, z), then (y, z) for P3D_PLANES_PANIC3D or (z, x) otherwise.
+__device__ __forceinline__ float2 plane_coords(const Geom& g, int p, float x, float y, float z) {
+    const bool pm = g.plane_mode == P3D_PLANES_PANIC3D;
+    return make_float2(p == 2 ? (pm ? y : z) : x, p == 0 ? y : (p == 1 ? z : (pm ? z : x)));
+}
 
-__device__ __forceinline__ Tap4 plane_taps(const Geom& g, long long base, float ca, float cb) {
-    Tap4 t;
+// grid_sample's bilinear footprint of plane coordinates (ca, cb): the top-left texel (x0, y0) and the 1-D weights of columns
+// x0, x0 + 1 and rows y0, y0 + 1.  A point that is NaN or lies more than a texel outside the plane gets x0 = y0 = -4, so all
+// four taps fall outside.  The forward gathers (plane_taps, fused::write_tap_row) and the backward scatter (tap_texels)
+// all take their taps from here, so the gradients land on exactly the texels and weights the forward used.
+struct Footprint {
+    int x0, y0;
+    float wx0, wx1, wy0, wy1;
+};
+__device__ __forceinline__ Footprint bilinear_footprint(const Geom& g, float ca, float cb) {
     const float gx = __fmul_rn(ca, g.coord_scale), gy = __fmul_rn(cb, g.coord_scale);
     const float fx = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)g.W), 1.f), 0.5f);
     const float fy = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)g.H), 1.f), 0.5f);
     const bool sane = (fx > -2.f) && (fx < (float)g.W + 1.f) && (fy > -2.f) && (fy < (float)g.H + 1.f);  // false for NaN too
     const float x0f = floorf(fx), y0f = floorf(fy);
-    const float wx1 = fx - x0f, wy1 = fy - y0f;
-    const float wx0 = 1.f - wx1, wy0 = 1.f - wy1;
-    const int x0 = sane ? (int)x0f : -4, y0 = sane ? (int)y0f : -4;
+    Footprint f;
+    f.wx1 = fx - x0f; f.wy1 = fy - y0f;
+    f.wx0 = 1.f - f.wx1; f.wy0 = 1.f - f.wy1;
+    f.x0 = sane ? (int)x0f : -4; f.y0 = sane ? (int)y0f : -4;
+    return f;
+}
+
+struct Tap4 {
+    long long off[4];
+    float w[4];
+};
+
+__device__ __forceinline__ Tap4 plane_taps(const Geom& g, long long base, float2 c) {
+    const Footprint f = bilinear_footprint(g, c.x, c.y);
+    Tap4 t;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const int xi = x0 + (k & 1), yi = y0 + (k >> 1);
+        const int xi = f.x0 + (k & 1), yi = f.y0 + (k >> 1);
         const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H);
-        const float wgt = ((k & 1) ? wx1 : wx0) * ((k >> 1) ? wy1 : wy0);
+        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);
         t.w[k] = ok ? wgt : 0.f;
         t.off[k] = base + (ok ? (long long)yi * g.stride_row + (long long)xi * g.stride_col : 0ll);
     }
@@ -105,11 +151,9 @@ __device__ __forceinline__ Tap4 plane_taps(const Geom& g, long long base, float 
 template <bool BF16>
 __device__ __forceinline__ float4 gather_features(const void* planes, const Geom& g, int view, float x, float y, float z, int q) {
     const long long vbase = (long long)view * g.stride_view + 4 * q;
-    const float a2 = g.plane_mode == P3D_PLANES_PANIC3D ? y : z;
-    const float b2 = g.plane_mode == P3D_PLANES_PANIC3D ? z : x;
-    Tap4 t0 = plane_taps(g, vbase, x, y);
-    Tap4 t1 = plane_taps(g, vbase + g.stride_plane, x, z);
-    Tap4 t2 = plane_taps(g, vbase + 2 * g.stride_plane, a2, b2);
+    Tap4 t0 = plane_taps(g, vbase, plane_coords(g, 0, x, y, z));
+    Tap4 t1 = plane_taps(g, vbase + g.stride_plane, plane_coords(g, 1, x, y, z));
+    Tap4 t2 = plane_taps(g, vbase + 2 * g.stride_plane, plane_coords(g, 2, x, y, z));
     float4 v[12];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -157,8 +201,6 @@ __device__ __forceinline__ float apply_masks(const Geom& g, float sigma, float x
 //   w_i = alpha_i * prod_{k<i} (1 - alpha_k + 1e-10)
 // t, sg: L sorted samples in shared memory; writes w[0..L-2]; returns (sum w, sum w*t_mid) on all lanes.
 // -------------------------------------------------------------------------------------------
-// FAST: MUFU ex2/lg2 based softplus/exp (abs err ~1e-7) for the fused kernel; false: libm-accurate (v1).
-template <bool FAST = false>
 __device__ __forceinline__ void ray_weights(const float* t, const float* sg, float* w, int L, int lane,
                                             float& wsum, float& dnum) {
     float carry = 1.f, acc_w = 0.f, acc_d = 0.f;
@@ -168,8 +210,7 @@ __device__ __forceinline__ void ray_weights(const float* t, const float* sg, flo
         if (i < L - 1) {
             const float delta = t[i + 1] - t[i];
             const float smid = __fsub_rn(__fmul_rn(__fadd_rn(sg[i], sg[i + 1]), 0.5f), 1.f);
-            if (FAST) alpha = 1.f - ex2_approx(-1.4426950408889634f * __fmul_rn(softplus_mufu(smid), delta));
-            else alpha = 1.f - expf(-__fmul_rn(softplus_t(smid), delta));
+            alpha = 1.f - expf(-__fmul_rn(softplus_t(smid), delta));
             factor = __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f);
             tmid = __fmul_rn(__fadd_rn(t[i], t[i + 1]), 0.5f);
         }
@@ -192,13 +233,12 @@ __device__ __forceinline__ void ray_weights(const float* t, const float* sg, flo
 //   fine    : out, sort_pow2 floats; the first Sf entries are the importance depths, ascending
 //   u_fine  : Sf injected uniforms for this ray (global) or nullptr -> Philox(seed, rng_base + f)
 // -------------------------------------------------------------------------------------------
-template <bool FAST = false>
 __device__ __forceinline__ void importance_ray(const Geom& g, const float* t, const float* sg, float* w, float* cdf,
                                                float* fine, int sort_pow2, const float* u_fine,
                                                unsigned long long rng_base, int lane) {
     const int S = g.S, Sf = g.Sf;
     float wsum, dnum;
-    ray_weights<FAST>(t, sg, w, S, lane, wsum, dnum);
+    ray_weights(t, sg, w, S, lane, wsum, dnum);
     __syncwarp();
     // max_pool1d(k=2,s=1,pad=1) -> avg_pool1d(k=2,s=1) -> +0.01 ; keep [1:-1] ; +eps     (:336-343, :360)
     // pooled[i] = (max(w[i-1],w[i]) + max(w[i],w[i+1]))/2 , i in [1, S-3]
@@ -272,22 +312,17 @@ __device__ __forceinline__ void importance_ray(const Geom& g, const float* t, co
 }
 
 // -------------------------------------------------------------------------------------------
-// composite_weights: unify_samples (renderer.py:289-301) + the weight part of the final
-// MipRayMarcher2 pass (ray_marcher.py:25-44) for ONE ray, executed by one warp.
-//   tc, sc : S coarse depths/densities   tf, sf : Sf fine depths (ascending) / densities
-//   t, sg, w : scratch of L = S+Sf floats each; src : L ints
-// On return w[j] holds omega_j = (w_{j-1}+w_j)/2 for merged position j and src[j] names its
-// sample (i < S: coarse i, else fine i-S), so  sum_i w_i (c_i+c_{i+1})/2 == sum_j omega_j c_j.
+// merge_by_rank: unify_samples (renderer.py:289-301) for ONE ray, executed by one warp.  Writes the S + Sf merged depths t,
+// densities sg and sources src (i < S: coarse i, else fine i - S).  Ties keep coarse before fine (stable sort of
+// cat([coarse, fine])).  Coarse depths ascend except for the degenerate 'auto' case where no ray hits the box (t0=-1 > t1=-2,
+// renderer.py:166-170 leaves them untouched): then they descend -> read reversed.  The backward rebuilds the forward's
+// order with this same function.
 // -------------------------------------------------------------------------------------------
-template <bool FAST = false>
-__device__ __forceinline__ void composite_weights(const float* tc, const float* sc, const float* tf, const float* sf,
-                                                  int S, int Sf, float* t, float* sg, float* w, int* src, int lane,
-                                                  float& wsum, float& dnum) {
-    const int L = S + Sf;
-    // merge by rank; ties keep coarse before fine (stable sort of cat([coarse, fine])).
-    // Coarse depths ascend except for the degenerate 'auto' case where no ray hits the box
-    // (t0=-1 > t1=-2, renderer.py:166-170 leaves them untouched): then they descend -> read reversed.
+__device__ __forceinline__ void merge_by_rank(const float* tc, const float* sc, const float* tf, const float* sf, int S, int Sf,
+                                              float* t, float* sg, int* src, int lane) {
     const bool rev = tc[0] > tc[S - 1];
+    // (not unrolled: a lane makes a few trips at most, and unrolled copies of the searches only cost registers)
+#pragma unroll 1
     for (int i = lane; i < S; i += 32) {
         const int ci = rev ? S - 1 - i : i;
         const float v = tc[ci];
@@ -296,6 +331,7 @@ __device__ __forceinline__ void composite_weights(const float* tc, const float* 
         const int pos = i + lo;
         t[pos] = v; sg[pos] = sc[ci]; src[pos] = ci;
     }
+#pragma unroll 1
     for (int j = lane; j < Sf; j += 32) {
         const float v = tf[j];
         int lo = 0, hi = S;
@@ -304,7 +340,22 @@ __device__ __forceinline__ void composite_weights(const float* tc, const float* 
         t[pos] = v; sg[pos] = sf[j]; src[pos] = S + j;
     }
     __syncwarp();
-    ray_weights<FAST>(t, sg, w, L, lane, wsum, dnum);
+}
+
+// -------------------------------------------------------------------------------------------
+// composite_weights: unify_samples (renderer.py:289-301) + the weight part of the final
+// MipRayMarcher2 pass (ray_marcher.py:25-44) for ONE ray, executed by one warp.
+//   tc, sc : S coarse depths/densities   tf, sf : Sf fine depths (ascending) / densities
+//   t, sg, w : scratch of L = S+Sf floats each; src : L ints
+// On return w[j] holds omega_j = (w_{j-1}+w_j)/2 for merged position j and src[j] names its
+// sample (i < S: coarse i, else fine i-S), so  sum_i w_i (c_i+c_{i+1})/2 == sum_j omega_j c_j.
+// -------------------------------------------------------------------------------------------
+__device__ __forceinline__ void composite_weights(const float* tc, const float* sc, const float* tf, const float* sf,
+                                                  int S, int Sf, float* t, float* sg, float* w, int* src, int lane,
+                                                  float& wsum, float& dnum) {
+    const int L = S + Sf;
+    merge_by_rank(tc, sc, tf, sf, S, Sf, t, sg, src, lane);
+    ray_weights(t, sg, w, L, lane, wsum, dnum);
     __syncwarp();
     float om[16];                           // up to 512 merged samples per ray
 #pragma unroll

@@ -21,7 +21,6 @@
 //                          sigma -> group state; colour reduction of a group once its omega is ready
 //   warps 20-23  RAY       a warp per ray: importance sampling after a group's coarse pass, merge / transmittance /
 //                          omega and the per-ray outputs after its fine pass
-#include <stdlib.h>
 #include "fused_common.cuh"
 
 namespace p3d {
@@ -38,7 +37,7 @@ constexpr int kNA = 4;                           // A1 ring depth
 constexpr int kStates = 4;                       // per-group state ring
 constexpr int kRowsG = 384;                      // rows per pass per group
 
-constexpr int kLBO_A1 = 2080, kLBO_W1 = 1024, kLBO_W2C = 512, kLBO_W2S = 256;
+constexpr int kLBO_W2C = 512, kLBO_W2S = 256;
 
 
 struct GroupState {                               // written by G (t_c, crop), E (sg_*), R (t_f)
@@ -80,14 +79,6 @@ struct WsArgs {
     int n_groups, single_pass;
     int srow, scol, splane;
     float sigma_cull;
-    unsigned long long* timing;      // optional [16] cycle counters (debug: P3D_WS_TIMING=1), nullptr = off
-};
-
-// cycle accounting of one gather warp and one epilogue warp of CTA 0 (debug aid, off by default)
-struct Tick {
-    unsigned long long* dst; long long t0; bool on;
-    __device__ Tick(unsigned long long* d, bool enable) : dst(d), t0(0), on(enable && d != nullptr) { if (on) t0 = clock64(); }
-    __device__ void lap(int slot) { if (on) { const long long t1 = clock64(); atomicAdd(dst + slot, (unsigned long long)(t1 - t0)); t0 = t1; } }
 };
 
 // pass j of a CTA with N groups:  C(0) C(1) | F(0) C(2) | F(1) C(3) | ... | F(N-2) F(N-1)   (N == 1: C(0) F(0))
@@ -131,48 +122,23 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         mbar_init(&sm.omega_ready[0], kRW); mbar_init(&sm.omega_ready[1], kRW);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int i = tid; i < kHidden * kC; i += kThreadsWS) {            // W1' = W1 * gain * log2(e)   (64 x 32)
-        const int n = i / kC, k = i % kC;
-        unsigned short hi, lo;
-        split1(__fmul_rn(a.w1[i], g.w1_gain) * (kLog2e / 3.f), hi, lo);      // the 1/3 is the plane mean
-        const int off = tile_off(n, k, kLBO_W1);
-        *reinterpret_cast<unsigned short*>(sm.w1[0] + off) = hi;
-        *reinterpret_cast<unsigned short*>(sm.w1[1] + off) = lo;
-    }
-    for (int i = tid; i < kRgb * kHidden; i += kThreadsWS) {          // colour rows 1..32 of W2, negated   (32 x 64)
-        const int n = i / kHidden, k = i % kHidden;
-        unsigned short hi, lo;
-        split1(-__fmul_rn(a.w2[(n + 1) * kHidden + k], g.w2_gain), hi, lo);
-        const int off = tile_off(n, k, kLBO_W2C);
-        *reinterpret_cast<unsigned short*>(sm.w2c[0] + off) = hi;
-        *reinterpret_cast<unsigned short*>(sm.w2c[1] + off) = lo;
-    }
-    for (int i = tid; i < 16 * kHidden; i += kThreadsWS) {            // sigma row 0 of W2 (* ln2) + 15 zero rows (16 x 64)
-        const int n = i / kHidden, k = i % kHidden;
-        unsigned short hi = 0, lo = 0;
-        if (n == 0) split1(__fmul_rn(a.w2[k], g.w2_gain) * kLn2, hi, lo);
-        const int off = tile_off(n, k, kLBO_W2S);
-        *reinterpret_cast<unsigned short*>(sm.w2s[0] + off) = hi;
-        *reinterpret_cast<unsigned short*>(sm.w2s[1] + off) = lo;
-    }
-    if (tid < kHidden) sm.b1[tid] = __fmul_rn(a.b1[tid], g.b1_gain) * kLog2e;
-    if (tid < kRgb) sm.b2c[tid] = -__fmul_rn(a.b2[tid + 1], g.b2_gain) * kLog2e;
-    if (tid == 0) sm.b2s = __fmul_rn(a.b2[0], g.b2_gain);
+    stage_w1_biases(g, a.w1, a.b1, a.b2, sm.w1, sm.b1, sm.b2c, sm.b2s, tid, kThreadsWS);
+    stage_w2(g, a.w2, sm.w2c, kRgb, kLBO_W2C, [](int n) { return n + 1; }, tid, kThreadsWS);         // the colour rows (32 x 64)
+    stage_w2(g, a.w2, sm.w2s, 16, kLBO_W2S, [](int n) { return n == 0 ? 0 : -1; }, tid, kThreadsWS);  // sigma + 15 zero rows
     fence_proxy_async();
     __syncthreads();
 
     if (warp < kGW) {
         // =========================================================================== GATHER
         const int gw = warp, team = gw >> 2, wt = gw & 3;
-        Tick tk_(a.timing, blockIdx.x == 0 && gw == 0 && lane == 0);
         constexpr int kEsz = BF16 ? 2 : 4;
         const long long scolB = (long long)a.scol * kEsz, srowB = (long long)a.srow * kEsz;
         unsigned char* tab = reinterpret_cast<unsigned char*>(sm.tab[gw]);
-        float v[6][8];
+        float v[12][4];
 #pragma unroll
-        for (int k = 0; k < 6; ++k)
+        for (int k = 0; k < 12; ++k)
 #pragma unroll
-            for (int c = 0; c < 8; ++c) v[k][c] = 0.f;
+            for (int c = 0; c < 4; ++c) v[k][c] = 0.f;
         int it = 0;
         for (int q = 0; q < T; ++q) {
             const TileDesc td = tile_at(q, n_my);
@@ -181,10 +147,8 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             const int grp = (int)blockIdx.x + td.n * (int)gridDim.x;
             const long long ray0 = (long long)grp * GR;
             GroupState& st = sm.st[td.n & 3];
-            tk_.lap(0);
             if (td.pass == 0) mbar_wait(&sm.state_free[td.n & 3], ((td.n >> 2) & 1) ^ 1);
             else mbar_wait(&sm.fine_ready[td.n & 3], (td.n >> 2) & 1);
-            tk_.lap(1);                                                   // [1] wait state_free / fine_ready
             const int view = (int)(ray0 / g.M);
             // ---- tap table of this warp's 32 rows: lane = row
             {
@@ -200,89 +164,24 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                         const long long gidx = ray * S + s;
                         u = a.u_c ? a.u_c[gidx] : philox_uniform(g.seed, (uint64_t)gidx, 0u);
                     }
-                    float t0 = 0.f, t1 = 0.f;
-                    if (g.ray_mode == P3D_RAYS_AUTOBOX && live) {
-                        t0 = a.ray_t0[ray]; t1 = a.ray_t1[ray];
-                        if (!(t1 > t0) && a.bounds[4]) { t0 = ordered_to_float(a.bounds[2]); t1 = ordered_to_float(a.bounds[3]); }
-                    }
-                    tval = coarse_depth(g, s, u, t0, t1);
+                    tval = coarse_sample_depth(g, s, u, ray, live, a.ray_t0, a.ray_t1, a.bounds);
                     st.t_c[srow] = tval;
                 } else {
                     tval = st.t_f[srow];
                 }
-                float px = 1e30f, py = 1e30f, pz = 1e30f;
-                if (live) {
-                    const float* o = a.ro + ray * 3;
-                    const float* d = a.rd + ray * 3;
-                    px = __fadd_rn(o[0], __fmul_rn(tval, d[0]));
-                    py = __fadd_rn(o[1], __fmul_rn(tval, d[1]));
-                    pz = __fadd_rn(o[2], __fmul_rn(tval, d[2]));
-                }
-                const bool pm = g.plane_mode == P3D_PLANES_PANIC3D;
-                uint32_t o0, o1, o2;
-                float4 w0, w1, w2;
-                const bool f0 = plane_taps_rec(g, a.srow, a.scol, 0, px, py, o0, w0);
-                const bool f1 = plane_taps_rec(g, a.srow, a.scol, a.splane, px, pz, o1, w1);
-                const bool f2 = plane_taps_rec(g, a.srow, a.scol, 2 * a.splane, pm ? py : pz, pm ? pz : px, o2, w2);
-                *reinterpret_cast<uint4*>(tab + tab_off(lane, 0)) = make_uint4(o0, o1, o2, (f0 ? 1u : 0u) | (f1 ? 2u : 0u) | (f2 ? 4u : 0u));
-                *reinterpret_cast<float4*>(tab + tab_off(lane, 1)) = w0;
-                *reinterpret_cast<float4*>(tab + tab_off(lane, 2)) = w1;
-                *reinterpret_cast<float4*>(tab + tab_off(lane, 3)) = w2;
-                st.crop[td.pass][srow] = (g.crop_on && !((fabsf(px) <= g.crop_limit) && (fabsf(pz) <= g.crop_limit))) ? 1 : 0;
+                float3 pt = make_float3(1e30f, 1e30f, 1e30f);
+                if (live) pt = ray_point(a.ro + ray * 3, a.rd + ray * 3, tval);
+                write_tap_row(tab, lane, g, a.srow, a.scol, a.splane, pt.x, pt.y, pt.z, 0u);   // the tile lies in one view (M % GR == 0)
+                st.crop[td.pass][srow] = (g.crop_on && !((fabsf(pt.x) <= g.crop_limit) && (fabsf(pt.z) <= g.crop_limit))) ? 1 : 0;
             }
             __syncwarp();
             const int stage = my_it % kNA;
             mbar_wait(&sm.a1_empty[stage], ((my_it / kNA) & 1) ^ 1);
-            tk_.lap(2);                                                   // [2] taps + wait a1_empty
-            unsigned char* a1h = sm.a1[stage][0];
-            unsigned char* a1l = sm.a1[stage][1];
-            {
-                // ---- gather: 8 rounds of 4 rows; lane (sub, qd) loads channels [4 qd, 4 qd + 4) of the 12 taps of row 4 round + sub:
-                //      twelve 128-bit loads in flight per lane, each warp-wide load covers four whole 128 B texels (one L1
-                //      wavefront per texel)
-                const int sub = lane >> 3, qd = lane & 7;
-                const char* vq4 = reinterpret_cast<const char*>(a.planes) + ((long long)view * g.stride_view + 4 * qd) * kEsz;
-                constexpr int kImmX4 = SCOL * kEsz;
-                float (*v4)[4] = reinterpret_cast<float (*)[4]>(&v[0][0]);           // the same 48 registers, as 12 x 4
-#pragma unroll 1
-                for (int round = 0; round < 8; ++round) {
-                    const int lrow = round * 4 + sub;
-                    const uint4 c0 = *reinterpret_cast<const uint4*>(tab + tab_off(lrow, 0));
-                    const bool p0 = c0.w & 1u, p1 = c0.w & 2u, p2 = c0.w & 4u;
-                    const char* b0 = vq4 + (unsigned long long)c0.x * kEsz;
-                    const char* b1 = vq4 + (unsigned long long)c0.y * kEsz;
-                    const char* b2 = vq4 + (unsigned long long)c0.z * kEsz;
-#define P3D_ROW1(base, rbase) (base + srowB)
-#define P3D_LD4(k, base, rbase, pr)                                                                                  \
-                    load_quad_p<BF16, 0>(v4[k], base, pr);                                                            \
-                    if (SCOL) load_quad_p<BF16, kImmX4>(v4[k + 1], base, pr); else load_quad_p<BF16, 0>(v4[k + 1], base + scolB, pr); \
-                    load_quad_p<BF16, 0>(v4[k + 2], P3D_ROW1(base, rbase), pr);                                       \
-                    if (SCOL) load_quad_p<BF16, kImmX4>(v4[k + 3], P3D_ROW1(base, rbase), pr); else load_quad_p<BF16, 0>(v4[k + 3], P3D_ROW1(base, rbase) + scolB, pr);
-                    P3D_LD4(0, b0, r0, p0)
-                    P3D_LD4(4, b1, r1, p1)
-                    P3D_LD4(8, b2, r2, p2)
-#undef P3D_LD4
-#undef P3D_ROW1
-                    const float4 w0 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 1));
-                    const float4 w1 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 2));
-                    const float4 w2 = *reinterpret_cast<const float4*>(tab + tab_off(lrow, 3));
-                    float acc[4] = {0.f, 0.f, 0.f, 0.f};
-                    fma4(acc, v4[0], w0.x); fma4(acc, v4[1], w0.y); fma4(acc, v4[2], w0.z); fma4(acc, v4[3], w0.w);
-                    fma4(acc, v4[4], w1.x); fma4(acc, v4[5], w1.y); fma4(acc, v4[6], w1.z); fma4(acc, v4[7], w1.w);
-                    fma4(acc, v4[8], w2.x); fma4(acc, v4[9], w2.y); fma4(acc, v4[10], w2.z); fma4(acc, v4[11], w2.w);
-                    uint32_t h[2], l[2];
-                    split2(acc[0], acc[1], h[0], l[0]);
-                    split2(acc[2], acc[3], h[1], l[1]);
-                    const int trow = wt * 32 + lrow;
-                    const int off = (trow >> 3) * kSBO + (qd >> 1) * kLBO_A1 + (trow & 7) * 16 + (qd & 1) * 8;
-                    *reinterpret_cast<uint2*>(a1h + off) = make_uint2(h[0], h[1]);
-                    *reinterpret_cast<uint2*>(a1l + off) = make_uint2(l[0], l[1]);
-                }
-            }
+            gather_a1<BF16, SCOL>(tab, reinterpret_cast<const char*>(a.planes) + (long long)view * g.stride_view * kEsz, 0 /* one view */, srowB,
+                                  scolB, v, sm.a1[stage][0], sm.a1[stage][1], wt, lane);
             fence_proxy_async();
             __syncwarp();                                                   // also: the tap table is rewritten by the next tile
             if (lane == 0) mbar_arrive(&sm.a1_full[stage]);
-            tk_.lap(3);                                                   // [3] gather of one tile (32 rows)
         }
     } else if (warp < kGW + kEW) {
         // =========================================================================== DECODER
@@ -317,7 +216,8 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 const float om = live ? sl.om[rl * L + sl.pos[pass * kRowsG + rl * S + s]] : 0.f;
                 const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
                 float v[32];
-                const float4* src = reinterpret_cast<const float4*>(colour_area(n, pass) + (k * 128 + trow) * kRgb);
+                // (an unsigned row offset: with a signed one ptxas spills the extended address across the omega wait at S = 96)
+                const float4* src = reinterpret_cast<const float4*>(colour_area(n, pass) + (unsigned)(k * 128 + trow) * kRgb);
 #pragma unroll
                 for (int c4 = 0; c4 < 8; ++c4) {
                     const float4 q4 = src[c4];
@@ -360,14 +260,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         // after the group's last sigma - which is also the last point before F(n+1) overwrites the fine area.
         const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]);
         const uint32_t w2ch = smem_u32(sm.w2c[0]), w2cl = smem_u32(sm.w2c[1]), w2sh = smem_u32(sm.w2s[0]), w2sl = smem_u32(sm.w2s[1]);
-        Tick tk_(a.timing, blockIdx.x == 0 && e == 0 && lane == 0);
         for (int it = 0; it < T; ++it) {
             const TileDesc td = tile_at(it, n_my);
-            tk_.lap(4);
-            if (td.pass == 1 && td.k == 0 && td.n >= 1) { colours(td.n - 1); tk_.lap(11); }   // [11] colours (incl. wait for omega)
+            if (td.pass == 1 && td.k == 0 && td.n >= 1) colours(td.n - 1);
             const int stage = it % kNA;
             mbar_wait(&sm.a1_full[stage], (it / kNA) & 1);
-            tk_.lap(5);                                                   // [5] wait a1_full
             float d1[32];
             decoder_layer1(d1, smem_u32(sm.a1[stage][0]), smem_u32(sm.a1[stage][1]), kLBO_A1, w1h, w1l, kLBO_W1, chunk, a.single_pass);
             __syncwarp();
@@ -381,7 +278,6 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             wgmma_wait_all();
             fence_operands(dc);
             fence_operands(ds);
-            tk_.lap(6);                                                   // [6] both layers
             // this thread's two rows of the tile (fragment elements 2 rs, 2 rs + 1 of each 8-column block)
             float* area = colour_area(td.n, td.pass) + td.k * 128 * kRgb;
             GroupState& st = sm.st[td.n & 3];
@@ -409,7 +305,6 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 __syncwarp();
                 if (lane == 0) mbar_arrive(td.pass == 0 ? &sm.sigc_ready[td.n & 3] : &sm.sigf_ready[td.n & 3]);
             }
-            tk_.lap(8);                                                   // [8] colour / sigma stores
         }
         colours(n_my - 1);
     } else if (warp < kGW + kEW + kRW) {
@@ -622,24 +517,19 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             __syncwarp();
         };
         // tasks follow the pass schedule: importance(n) after C(n), merge(n) after F(n)
-        Tick tr_(a.timing, blockIdx.x == 0 && rw == 0 && lane == 0);
         for (int j = 0; j < 2 * n_my; ++j) {
             const PassDesc pd = pass_at(j, n_my);
             const int n = pd.n, si = n & 3;
             const uint32_t par = (n >> 2) & 1;
             if (pd.pass == 0) {
                 mbar_wait(&sm.sigc_ready[si], par);
-                tr_.lap(13);                                                  // [13] wait for coarse sigma
                 for (int rl = rw; rl < GR; rl += kRW) importance_ray(n, rl);
                 if (lane == 0) mbar_arrive(&sm.fine_ready[si]);
-                tr_.lap(9);                                                   // [9] importance
             } else {
                 mbar_wait(&sm.sigf_ready[si], par);
                 if (n >= 2) mbar_wait(&sm.state_free[(n - 2) & 3], ((n - 2) >> 2) & 1);       // colours(n-2) has released the omega slot
-                tr_.lap(14);                                                  // [14] wait for fine sigma / slot
                 for (int rl = rw; rl < GR; rl += kRW) composite_ray(n, rl);
                 if (lane == 0) mbar_arrive(&sm.omega_ready[n & 1]);
-                tr_.lap(10);                                                  // [10] merge / weights
             }
         }
     }
@@ -647,16 +537,10 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
 
 }  // namespace
 
-int launch_bounds_init(unsigned int* bounds, cudaStream_t stream);
-int launch_ray_limits(const float* ro, const float* rd, long long R, float h, float* t0, float* t1, unsigned int* bounds, cudaStream_t stream);
-int launch_depth_finalize(float* depth, long long R, const unsigned int* bounds, cudaStream_t stream);
-
 bool fused_ws3_supported(const Geom& g) {
     if (!((g.S == 96 || g.S == 48) && (g.Sf == g.S) && ((long long)g.M % (384 / g.S) == 0))) return false;
-    const long long span = 2 * g.stride_plane + (long long)(g.H - 1) * g.stride_row + (long long)(g.W - 1) * g.stride_col + kC;
-    if (g.H < 2 || g.W < 2) return false;
     if ((g.stride_view | g.stride_plane | g.stride_row | g.stride_col) & 7) return false;
-    return g.stride_plane >= 0 && g.stride_row >= 0 && g.stride_col >= 0 && span < (1ll << 31);
+    return tap_offsets_fit(g);
 }
 
 int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
@@ -687,46 +571,19 @@ int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const vo
         const double thr = (double)g.cull_thresh;
         a.sigma_cull = thr >= 1.0 ? INFINITY : (thr <= 0.0 ? -INFINITY : (float)(1.0 + log(expm1(-log1p(-thr)))));
     }
-    static int n_sm = 0;
-    if (!n_sm) {
-        int dev = 0;
-        P3D_CUDA_TRY(cudaGetDevice(&dev));
-        P3D_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    }
-    static unsigned long long* d_timing = nullptr;
-    static const bool timing_on = getenv("P3D_WS_TIMING") != nullptr;
-    if (timing_on) {
-        if (!d_timing) P3D_CUDA_TRY(cudaMalloc(&d_timing, 16 * sizeof(unsigned long long)));
-        P3D_CUDA_TRY(cudaMemsetAsync(d_timing, 0, 16 * sizeof(unsigned long long), stream));
-        a.timing = d_timing;
-    }
+    int n_sm;
+    if ((rc = sm_count(&n_sm))) return rc;
     const size_t smem = sizeof(WsSmem) + 1024;
-    void (*kern)(WsArgs) = nullptr;
-    // the x+1 texel is an immediate offset when the texel stride is one of the two layouts the host produces: kC (the layout
-    // pre-pass: one plane's texels contiguous) or 3 kC (a (N,96,H,W) channels_last backbone output consumed zero-copy)
-    const int sc = g.stride_col == kC ? 1 : (g.stride_col == 3 * kC ? 2 : 0);
-#define P3D_PICK(BF, S_) (sc == 1 ? k_render_ws3<BF, S_, kC> : (sc == 2 ? k_render_ws3<BF, S_, 3 * kC> : k_render_ws3<BF, S_, 0>))
-    if (g.S == 96) kern = p->planes_bf16 ? P3D_PICK(true, 96) : P3D_PICK(false, 96);
-    else kern = p->planes_bf16 ? P3D_PICK(true, 48) : P3D_PICK(false, 48);
-#undef P3D_PICK
+    void (*kern)(WsArgs) = with_texel_stride(g, [&](auto sc) -> void (*)(WsArgs) {
+        if (g.S == 96) return p->planes_bf16 ? k_render_ws3<true, 96, sc.value> : k_render_ws3<false, 96, sc.value>;
+        return p->planes_bf16 ? k_render_ws3<true, 48, sc.value> : k_render_ws3<false, 48, sc.value>;
+    });
     P3D_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = a.n_groups < n_sm ? a.n_groups : n_sm;
     {
         ProfileScope prof(PROF_FUSED, stream);
         kern<<<grid, kThreadsWS, smem, stream>>>(a);
         P3D_LAUNCH_CHECK();
-    }
-    if (timing_on) {
-        unsigned long long h[16];
-        P3D_CUDA_TRY(cudaMemcpyAsync(h, d_timing, sizeof(h), cudaMemcpyDeviceToHost, stream));
-        P3D_CUDA_TRY(cudaStreamSynchronize(stream));
-        const int groups_cta0 = (a.n_groups + grid - 1) / grid;
-        fprintf(stderr, "[p3d ws timing, CTA0, cycles/group over %d groups] G(warp0: 1/3 of tiles): wait_dep %.0f wait_ring %.0f gather %.0f | "
-                        "D(warp0): wait_a1 %.0f layers %.0f stores %.0f colours(+omega wait) %.0f other %.0f | "
-                        "R(warp0): wait_sigc %.0f importance %.0f wait_sigf %.0f merge %.0f\n",
-                groups_cta0, (double)h[1] / groups_cta0, (double)h[2] / groups_cta0, (double)h[3] / groups_cta0, (double)h[5] / groups_cta0,
-                (double)h[6] / groups_cta0, (double)h[8] / groups_cta0, (double)h[11] / groups_cta0, (double)h[4] / groups_cta0,
-                (double)h[13] / groups_cta0, (double)h[9] / groups_cta0, (double)h[14] / groups_cta0, (double)h[10] / groups_cta0);
     }
     if (p->defer_depth_clamp) return P3D_OK;
     return launch_depth_finalize(out_depth, R, ws.bounds, stream);

@@ -42,6 +42,15 @@ struct Workspace {
     unsigned int* bounds;  // [0] min depth, [1] max depth (ordered-uint), [2] min valid t0, [3] max valid t0, [4] any valid
 };
 
+// The volume query's scalars, each rounded to fp32 once where the reference's Python floats meet an fp32 tensor
+// (_util/eg3d_metrics3d.py:70-183).
+struct VolumeSpec {
+    int res;                  // grid side R: R^3 points per view
+    float size, origin;       // voxel size cube / (R - 1) and corner -cube / 2
+    float crop, cull;         // crop limit box_warp / 2 - triplane_crop (< 0 crops everything, as there) / cull threshold
+    int crop_on, cull_on;
+};
+
 int make_geom(const p3d_render_params* p, Geom* g);
 size_t workspace_layout(const p3d_render_params* p, void* base, Workspace* ws);
 
@@ -55,6 +64,11 @@ int render_backward_v1(const Geom& g, const p3d_render_params* p, const void* pl
                        const float* out_depth, const float* g_rgb, const float* g_depth, const float* g_wsum,
                        const float* g_xyz, void* scratch, size_t scratch_bytes, float* d_planes, float* d_w1, float* d_b1,
                        float* d_w2, float* d_b2, cudaStream_t stream);
+// small launches of render_v1.cu shared by both renderers
+int launch_bounds_init(unsigned int* bounds, cudaStream_t stream);
+int launch_ray_limits(const float* ro, const float* rd, long long R, float h, float* t0, float* t1, unsigned int* bounds,
+                      cudaStream_t stream);
+int launch_depth_finalize(float* depth, long long R, const unsigned int* bounds, cudaStream_t stream);
 int launch_bounds_to_float(const unsigned int* bounds, float* out2, cudaStream_t stream);
 int launch_depth_finalize_f(float* depth, long long R, const float* bounds2, cudaStream_t stream);
 // warp-specialised fused renderer (render_fused_ws3.cu): gather / wgmma decoder / ray roles, three ray groups in flight
@@ -72,14 +86,14 @@ int decode_points_tc(const Geom& g, const p3d_render_params* p, const void* plan
                      const float* w2, const float* b2, const float* coords, long long n_pts, float* out_rgb,
                      float* out_sigma, cudaStream_t stream);
 int volume_query_tc(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
-                    const float* w2, const float* b2, int res, double cube_length, double triplane_crop, double cull_clouds,
-                    float* out_sigma, float* out_rgb, float* out_density, float* out_coords, cudaStream_t stream);
+                    const float* w2, const float* b2, const VolumeSpec& vol, float* out_sigma, float* out_rgb,
+                    float* out_density, float* out_coords, cudaStream_t stream);
 int decode_points_backward_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
                               const float* w2, const float* b2, const float* coords, long long n_pts, const float* g_rgb,
                               const float* g_sigma, float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2,
                               cudaStream_t stream);
 int volume_query_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
-                    const float* w2, const float* b2, int res, double cube_length, double triplane_crop, double cull_clouds,
-                    float* out_sigma, float* out_rgb, float* out_density, float* out_coords, cudaStream_t stream);
+                    const float* w2, const float* b2, const VolumeSpec& vol, float* out_sigma, float* out_rgb,
+                    float* out_density, float* out_coords, cudaStream_t stream);
 
 }  // namespace p3d

@@ -38,11 +38,7 @@ struct SampleArgs {
     long long total;            // samples in this launch
     long long per_view;         // samples per view (M*S, M*Sf or K)
     int per_ray;                // S, Sf (or 1 in points mode)
-    // volume mode (dense grid query, _util/eg3d_metrics3d.py:70-183)
-    int vol_res;                // grid side R: per_view = R^3
-    float vol_size, vol_origin; // voxel size cube/(R-1) and corner -cube/2, both rounded to fp32 like torch's scalar ops
-    float vol_crop, vol_cull;   // crop limit bw/2 - triplane_crop / cull threshold
-    bool vol_crop_on, vol_cull_on;
+    VolumeSpec vol;             // volume mode (dense grid query): per_view = vol.res^3
     float* density_out;         // (total) or nullptr
     float* coords_out;          // (total,3) or nullptr
 };
@@ -89,31 +85,20 @@ __global__ void __launch_bounds__(kTile) k_sample_decode(const SampleArgs a) {
             if (MODE == MODE_POINTS) {
                 px = a.coords[gidx * 3 + 0]; py = a.coords[gidx * 3 + 1]; pz = a.coords[gidx * 3 + 2];
             } else if (MODE == MODE_VOLUME) {
-                volume_point(gidx - (long long)view * a.per_view, a.vol_res, a.vol_size, a.vol_origin, px, py, pz);
+                volume_point(gidx - (long long)view * a.per_view, a.vol.res, a.vol.size, a.vol.origin, px, py, pz);
             } else {
                 const long long ray = gidx / a.per_ray;
                 const int s = (int)(gidx - ray * a.per_ray);
                 float t;
                 if (MODE == MODE_COARSE) {
                     const float u = a.u ? a.u[gidx] : philox_uniform(g.seed, (uint64_t)gidx, 0u);
-                    float t0 = 0.f, t1 = 0.f;
-                    if (g.ray_mode == P3D_RAYS_AUTOBOX) {
-                        t0 = a.ray_t0[ray]; t1 = a.ray_t1[ray];
-                        if (!(t1 > t0) && a.bounds[4]) {           // renderer.py:167-170
-                            t0 = ordered_to_float(a.bounds[2]);
-                            t1 = ordered_to_float(a.bounds[3]);
-                        }
-                    }
-                    t = coarse_depth(g, s, u, t0, t1);
+                    t = coarse_sample_depth(g, s, u, ray, true, a.ray_t0, a.ray_t1, a.bounds);
                     if (q == 0) a.depth_out[gidx] = t;
                 } else {
                     t = a.depth_in[gidx];
                 }
-                const float* o = a.ro + ray * 3;
-                const float* d = a.rd + ray * 3;
-                px = __fadd_rn(o[0], __fmul_rn(t, d[0]));
-                py = __fadd_rn(o[1], __fmul_rn(t, d[1]));
-                pz = __fadd_rn(o[2], __fmul_rn(t, d[2]));
+                const float3 pt = ray_point(a.ro + ray * 3, a.rd + ray * 3, t);
+                px = pt.x; py = pt.y; pz = pt.z;
             }
             f = gather_features<BF16>(a.planes, g, view, px, py, pz, q);
         }
@@ -160,21 +145,12 @@ __global__ void __launch_bounds__(kTile) k_sample_decode(const SampleArgs a) {
         if (gidx < a.total) {
             const int view = (int)(gidx / a.per_view);
             const long long n = gidx - (long long)view * a.per_view;
-            const long long dest = (long long)view * a.per_view + volume_dest(n, a.vol_res);
+            const long long dest = (long long)view * a.per_view + volume_dest(n, a.vol.res);
             a.sigma_out[dest] = sigma;
-            if (a.density_out) {
-                // densities = sigma2density(sigma) (eg3d_metrics3d.py:65-69), then crop / cull write -1e3 (:155-162).  The
-                // reference hands the DENSITIES to cull_clouds_mask, which applies softplus(. - 1) -> 1 - exp(-.) once more
-                // (renderer.py:150-153): the threshold acts on the twice-transformed value.
-                float dens = 1.f - expf(-softplus_t(__fsub_rn(sigma, 1.f)));
-                const float px = s_xz[tid * 2], pz = s_xz[tid * 2 + 1];
-                if (a.vol_crop_on && !((fabsf(px) <= a.vol_crop) && (fabsf(pz) <= a.vol_crop))) dens = -1e3f;
-                if (a.vol_cull_on && (1.f - expf(-softplus_t(__fsub_rn(dens, 1.f)))) < a.vol_cull) dens = -1e3f;
-                a.density_out[dest] = dens;
-            }
+            if (a.density_out) a.density_out[dest] = volume_density(a.vol, sigma, s_xz[tid * 2], s_xz[tid * 2 + 1]);
             if (a.coords_out) {
                 float x, y, z;
-                volume_point(n, a.vol_res, a.vol_size, a.vol_origin, x, y, z);
+                volume_point(n, a.vol.res, a.vol.size, a.vol.origin, x, y, z);
                 a.coords_out[dest * 3 + 0] = x; a.coords_out[dest * 3 + 1] = y; a.coords_out[dest * 3 + 2] = z;
             }
         }
@@ -195,7 +171,7 @@ __global__ void __launch_bounds__(kTile) k_sample_decode(const SampleArgs a) {
         if (gi >= a.total) continue;
         if (MODE == MODE_VOLUME) {
             const long long view = gi / a.per_view, n = gi - view * a.per_view;
-            gi = view * a.per_view + volume_dest(n, a.vol_res);
+            gi = view * a.per_view + volume_dest(n, a.vol.res);
         }
         a.rgb_out[gi * kRgb + col] = s_feat[row * kFeatStride + col];
     }
@@ -352,7 +328,6 @@ int launch_sample_decode(const SampleArgs& a, bool bf16, cudaStream_t stream) {
 
 }  // namespace
 
-// small launches shared with the fused renderer (render_fused_ws3.cu)
 int launch_bounds_init(unsigned int* bounds, cudaStream_t stream) {
     k_init_bounds<<<1, 32, 0, stream>>>(bounds);
     P3D_LAUNCH_CHECK();
@@ -389,20 +364,17 @@ int render_forward_v1(const Geom& g, const p3d_render_params* p, const void* pla
     P3D_REQUIRE(g.Sf == 0 || g.S >= 4, "importance sampling needs depth_resolution >= 4");
     P3D_REQUIRE(g.Sf >= 0 && g.S + g.Sf <= 512, "depth_resolution + depth_resolution_importance must be <= 512");
 
-    k_init_bounds<<<1, 32, 0, stream>>>(ws.bounds);
-    P3D_LAUNCH_CHECK();
-    if (g.ray_mode == P3D_RAYS_AUTOBOX) {
-        k_ray_limits<<<(unsigned)((R + 255) / 256), 256, 0, stream>>>(ro, rd, R, g.half_box, ws.ray_t0, ws.ray_t1, ws.bounds);
-        P3D_LAUNCH_CHECK();
-    }
+    int rc;
+    if ((rc = launch_bounds_init(ws.bounds, stream))) return rc;
+    if (g.ray_mode == P3D_RAYS_AUTOBOX)
+        if ((rc = launch_ray_limits(ro, rd, R, g.half_box, ws.ray_t0, ws.ray_t1, ws.bounds, stream))) return rc;
     SampleArgs sa{};
     sa.g = g; sa.planes = planes; sa.w1 = w1; sa.b1 = b1; sa.w2 = w2; sa.b2 = b2; sa.ro = ro; sa.rd = rd;
     sa.ray_t0 = ws.ray_t0; sa.ray_t1 = ws.ray_t1; sa.bounds = ws.bounds;
     // coarse pass
     sa.u = u_c; sa.depth_out = ws.depth_c; sa.sigma_out = ws.sigma_c; sa.rgb_out = ws.rgb_c;
     sa.total = R * g.S; sa.per_view = (long long)g.M * g.S; sa.per_ray = g.S;
-    int rc = launch_sample_decode<MODE_COARSE>(sa, p->planes_bf16 != 0, stream);
-    if (rc) return rc;
+    if ((rc = launch_sample_decode<MODE_COARSE>(sa, p->planes_bf16 != 0, stream))) return rc;
     if (g.Sf > 0) {
         ImportanceArgs ia{};
         ia.g = g; ia.depth_c = ws.depth_c; ia.sigma_c = ws.sigma_c; ia.u_fine = u_f; ia.depth_f = ws.depth_f;
@@ -431,9 +403,7 @@ int render_forward_v1(const Geom& g, const p3d_render_params* p, const void* pla
         P3D_LAUNCH_CHECK();
     }
     if (p->defer_depth_clamp) return P3D_OK;
-    k_depth_finalize<<<(unsigned)((R + 255) / 256), 256, 0, stream>>>(out_depth, R, ws.bounds);
-    P3D_LAUNCH_CHECK();
-    return P3D_OK;
+    return launch_depth_finalize(out_depth, R, ws.bounds, stream);
 }
 
 int decode_points_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
@@ -447,18 +417,13 @@ int decode_points_v1(const Geom& g, const p3d_render_params* p, const void* plan
 }
 
 int volume_query_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
-                    const float* w2, const float* b2, int res, double cube_length, double triplane_crop, double cull_clouds,
-                    float* out_sigma, float* out_rgb, float* out_density, float* out_coords, cudaStream_t stream) {
+                    const float* w2, const float* b2, const VolumeSpec& vol, float* out_sigma, float* out_rgb,
+                    float* out_density, float* out_coords, cudaStream_t stream) {
     SampleArgs sa{};
     sa.g = g; sa.planes = planes; sa.w1 = w1; sa.b1 = b1; sa.w2 = w2; sa.b2 = b2;
     sa.sigma_out = out_sigma; sa.rgb_out = out_rgb; sa.density_out = out_density; sa.coords_out = out_coords;
-    sa.per_view = (long long)res * res * res; sa.total = (long long)g.N * sa.per_view; sa.per_ray = 1;
-    sa.vol_res = res;
-    sa.vol_size = (float)(cube_length / (double)(res - 1));          // python float -> fp32 scalar operand
-    sa.vol_origin = (float)(0.0 - cube_length / 2.0);
-    sa.vol_crop = triplane_crop >= 0 ? (float)(p->box_warp / 2.0 - triplane_crop) : -1.f;    // renderer.py:139-148 (a limit < 0 crops everything, as there)
-    sa.vol_cull = cull_clouds >= 0 ? (float)cull_clouds : -1.f;
-    sa.vol_crop_on = triplane_crop >= 0; sa.vol_cull_on = cull_clouds >= 0;
+    sa.per_view = (long long)vol.res * vol.res * vol.res; sa.total = (long long)g.N * sa.per_view; sa.per_ray = 1;
+    sa.vol = vol;
     return launch_sample_decode<MODE_VOLUME>(sa, p->planes_bf16 != 0, stream);
 }
 
