@@ -80,13 +80,6 @@ int p3d_filtered_lrelu(const void* x, const float* fu, const float* fd, const vo
                        int32_t s_h, int32_t s_w, int32_t sx, int32_t sy,
                        float gain, float slope, float clamp, int32_t flip, int32_t sign_mode, void* stream);
 
-/* filtered_lrelu_plugin.filtered_lrelu_act_(x, si, sx, sy, gain, slope, clamp, writeSigns) -> so
-   (ops/filtered_lrelu.cpp:217-296, kernel ops/filtered_lrelu.cu:1109-1215): in-place gain*lrelu+clamp on x
-   with the same 2-bit sign tensor protocol (sign_mode 0 none, 1 write, 2 read). */
-int p3d_filtered_lrelu_act(void* x, uint8_t* s, int32_t dtype, int32_t n, int32_t c, int32_t h, int32_t w,
-                           const int64_t* x_stride, int32_t s_h, int32_t s_w, int32_t sx, int32_t sy,
-                           float gain, float slope, float clamp, int32_t sign_mode, void* stream);
-
 #ifdef __cplusplus
 }
 #endif

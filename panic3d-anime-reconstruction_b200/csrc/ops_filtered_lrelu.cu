@@ -222,55 +222,6 @@ int launch_fl(FlParams p, cudaStream_t stream) {
     return P3D_OK;
 }
 
-// ------------------------------------------------------------------------------------------ act-only kernel
-struct ActParams {
-    void* x;
-    unsigned char* s;
-    int N, C, H, W;
-    long long xs[4];
-    int sH, sW, sx, sy;
-    float gain, slope, clamp;
-    int sign_mode;
-};
-
-template <typename T>
-__global__ void __launch_bounds__(256) k_filtered_lrelu_act(const ActParams p) {
-    // one thread per group of 4 horizontally adjacent pixels (= one sign byte in write mode)
-    const int W4 = ((p.sign_mode == 1 ? max(p.W, p.sW) : p.W) + 3) >> 2;
-    const int rows = p.sign_mode == 1 ? max(p.H, p.sH) : p.H;
-    const long long total = (long long)p.N * p.C * rows * W4;
-    T* xp = reinterpret_cast<T*>(p.x);
-    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-        long long r = idx;
-        const int x4 = (int)(r % W4); r /= W4;
-        const int y = (int)(r % rows); r /= rows;
-        const int c = (int)(r % p.C);
-        const int n = (int)(r / p.C);
-        unsigned int code = 0;
-        for (int e = 0; e < 4; ++e) {
-            const int x = x4 * 4 + e;
-            if (x >= p.W || y >= p.H) continue;
-            T* pv = xp + n * p.xs[0] + c * p.xs[1] + y * p.xs[2] + x * p.xs[3];
-            float v = Fx<T>::ld(*pv) * p.gain;
-            if (p.sign_mode == 2) {
-                const int qx = x + p.sx, qy = y + p.sy;
-                if (qx >= 0 && qx < p.sW && qy >= 0 && qy < p.sH) {
-                    const unsigned int sc = (p.s[((size_t)(n * p.C + c) * p.sH + qy) * (p.sW >> 2) + (qx >> 2)] >> ((qx & 3) << 1)) & 3u;
-                    if (sc & 1u) v *= p.slope;
-                    if (sc & 2u) v = 0.f;
-                }
-            } else {
-                unsigned int sc = 0;
-                if (v < 0.f) { v *= p.slope; sc = 1; }
-                if (fabsf(v) > p.clamp) { v = v < 0.f ? -p.clamp : p.clamp; sc = 2; }
-                code |= sc << (2 * e);
-            }
-            *pv = Fx<T>::st(v);
-        }
-        if (p.sign_mode == 1 && y < p.sH && x4 * 4 < p.sW) p.s[((size_t)(n * p.C + c) * p.sH + y) * (p.sW >> 2) + x4] = (unsigned char)code;
-    }
-}
-
 }  // namespace
 }  // namespace p3d
 
@@ -310,35 +261,4 @@ extern "C" int p3d_filtered_lrelu(const void* x, const float* fu, const float* f
     }
     set_error("filtered_lrelu supports fp32 / fp16 / bf16 (dtype %d)", dtype);
     return P3D_EINVAL;
-}
-
-extern "C" int p3d_filtered_lrelu_act(void* x, uint8_t* s, int32_t dtype, int32_t n, int32_t c, int32_t h, int32_t w,
-                                      const int64_t* x_stride, int32_t s_h, int32_t s_w, int32_t sx, int32_t sy, float gain,
-                                      float slope, float clamp, int32_t sign_mode, void* stream) {
-    P3D_REQUIRE(x && x_stride, "null pointer");
-    P3D_REQUIRE(sign_mode >= 0 && sign_mode <= 2, "bad sign_mode");
-    P3D_REQUIRE(sign_mode == 0 || (s != nullptr && s_w % 16 == 0), "sign tensor needs s != NULL and a width that is a multiple of 16");
-    if ((long long)n * c * h * w == 0) return P3D_OK;
-    ActParams p{};
-    p.x = x; p.s = s; p.N = n; p.C = c; p.H = h; p.W = w;
-    for (int i = 0; i < 4; ++i) p.xs[i] = x_stride[i];
-    p.sH = sign_mode ? s_h : 0; p.sW = sign_mode ? s_w : 0; p.sx = sx; p.sy = sy; p.gain = gain; p.slope = slope; p.clamp = clamp; p.sign_mode = sign_mode;
-    const long long total = (long long)n * c * (sign_mode == 1 ? (h > s_h ? h : s_h) : h) * (((sign_mode == 1 ? (w > s_w ? w : s_w) : w) + 3) / 4);
-    static int n_sm = 0;
-    if (!n_sm) {
-        int dev = 0;
-        P3D_CUDA_TRY(cudaGetDevice(&dev));
-        P3D_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    }
-    const long long cap = (long long)n_sm * 16;                               // 16 CTAs of 256 threads per SM, grid-stride beyond
-    const int grid = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (dtype) {
-        case P3D_F32: k_filtered_lrelu_act<float><<<grid, 256, 0, st>>>(p); break;
-        case P3D_F16: k_filtered_lrelu_act<__half><<<grid, 256, 0, st>>>(p); break;
-        case P3D_BF16: k_filtered_lrelu_act<__nv_bfloat16><<<grid, 256, 0, st>>>(p); break;
-        default: set_error("filtered_lrelu_act supports fp32 / fp16 / bf16 (dtype %d)", dtype); return P3D_EINVAL;
-    }
-    P3D_LAUNCH_CHECK();
-    return P3D_OK;
 }

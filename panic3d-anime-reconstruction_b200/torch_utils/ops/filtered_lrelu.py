@@ -19,7 +19,6 @@ _P64 = _C.POINTER(_C.c_int64)
 _lib.register_protos({
     'p3d_filtered_lrelu': (_C.c_int, [_lib._VP] * 6 + [_C.c_int32] * 5 + [_P64, _C.c_int32, _C.c_int32, _P64] + [_C.c_int32] * 16 +
                            [_C.c_float] * 3 + [_C.c_int32, _C.c_int32, _lib._VP]),
-    'p3d_filtered_lrelu_act': (_C.c_int, [_lib._VP, _lib._VP] + [_C.c_int32] * 5 + [_P64] + [_C.c_int32] * 4 + [_C.c_float] * 3 + [_C.c_int32, _lib._VP]),
 })
 _DTYPES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
