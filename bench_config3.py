@@ -105,6 +105,7 @@ def main():
     ap.add_argument('--return_more', action='store_true', help='call G.f(x, return_more=True) like generate.py:130 (with --graphs: lean_return_more)')
     ap.add_argument('--graphs', action='store_true', help='ours arm: panic3d_b200.graphs.enable_cuda_graphs(G) - backbone and SR head replayed as CUDA graphs')
     ap.add_argument('--reuse_triplane', action='store_true', help='ours arm: dropin.install_paste(reuse_triplane=True)')
+    ap.add_argument('--modconv', action='store_true', help='ours arm: dropin.install_modconv() - the synthesis layers and SR head on the fused modulated-conv kernel')
     ap.add_argument('--paste', action='store_true', help="run the sweep with the eval script's paste_params (generate.py:59-65)")
     args = ap.parse_args()
     import torch
@@ -148,6 +149,8 @@ def main():
     import training.triplane as tp
     if args.paste and args.arm == 'ours':
         dropin.install_paste(tp, reuse_triplane=args.reuse_triplane)
+    if args.modconv and args.arm == 'ours':
+        dropin.install_modconv()
     mod_file = sys.modules[tp.ImportanceRenderer.__module__].__file__
     assert ('baseline/_ref' in mod_file.replace(os.sep, '/')) == (args.arm == 'reference'), mod_file
     G, R = build_generator(args, torch)

@@ -38,7 +38,7 @@ inline void count_launch(int n = 1) { g_launches.fetch_add((uint64_t)n, std::mem
 // Optional per-kernel device timing (bench.py's roofline leg): when enabled, launch sites bracket
 // their kernel with CUDA events on the launching stream; p3d_profile_read() sums them per slot.
 enum ProfileSlot { PROF_SAMPLE_DECODE = 0, PROF_IMPORTANCE = 1, PROF_COMPOSITE = 2, PROF_LAYOUT = 3, PROF_RAYGEN = 4,
-                   PROF_FUSED = 5, PROF_OTHER = 6, PROF_SLOTS = 8 };
+                   PROF_FUSED = 5, PROF_OTHER = 6, PROF_MODCONV = 7, PROF_SLOTS = 8 };
 bool profile_enabled();
 void profile_begin(int slot, cudaStream_t stream);
 void profile_end(int slot, cudaStream_t stream);

@@ -77,6 +77,26 @@ def install_paste(module=None, reuse_triplane=False):
     return names
 
 
+def install_modconv(module=None):
+    """Rebind ``SynthesisLayer.forward`` and ``ToRGBLayer.forward`` of the reference's ``training.networks_stylegan2`` to
+    ``panic3d_b200.modconv`` (the fused modulated convolution at inference).  ``superresolution.py`` imports the same
+    classes, so this covers the backbone and the super-resolution head.  Calls the kernel does not cover (CPU, training,
+    ``fused_modconv=False``, TF32 disallowed for fp32 layers, unsupported shapes) run the original method, which stays
+    reachable as ``<class>._p3d_reference_forward``.  ``module``: the already-imported module (default: import it by that
+    name).  Returns the names that were rebound."""
+    from . import modconv
+    if module is None:
+        module = importlib.import_module('training.networks_stylegan2')
+    names = []
+    for cls_name, fn in (('SynthesisLayer', modconv.synthesis_layer_forward), ('ToRGBLayer', modconv.torgb_forward)):
+        cls = getattr(module, cls_name)
+        if '_p3d_reference_forward' not in cls.__dict__:
+            cls._p3d_reference_forward = cls.forward                  # keep the original reachable for A/B runs
+        cls.forward = fn
+        names.append(cls_name + '.forward')
+    return names
+
+
 def patch_generator(G):
     """For a TriPlaneGenerator that was built BEFORE install() (e.g. unpickled): swap its two hot-path
     sub-modules in place.  Both are parameter-free, so no weights move."""
