@@ -37,6 +37,10 @@ restatement of bilinear/zero-pad/align_corners=False, the one parity tests use)
 and ``gather='aten'`` (``F.grid_sample`` - the same ATen op the reference calls,
 used when this oracle is *timed* as the CPU baseline so the baseline is not
 handicapped by a slow Python gather).
+
+The decode path (``sample_planes``, ``decode``, ``run_model``) allocates on the device and in the dtype of its inputs, so
+the GPU tests run it in fp64 on the device at sizes the CPU could not reach in time (tests/test_decode_tc_depth_gpu.py,
+which pins that run to this CPU fp32 one).
 """
 from __future__ import annotations
 
@@ -182,7 +186,7 @@ def plane_coords(xyz: Tensor, use_triplane: bool) -> Tensor:
 
 def _third_plane(xyz: Tensor, use_triplane: bool) -> Tensor:
     axes = torch.tensor([[0, 1, 0], [0, 0, 1], [1, 0, 0]] if use_triplane else
-                        [[0, 0, 1], [1, 0, 0], [0, 1, 0]], dtype=torch.float32)
+                        [[0, 0, 1], [1, 0, 0], [0, 1, 0]], dtype=xyz.dtype, device=xyz.device)
     inv = torch.linalg.inv(axes)
     return (xyz @ inv)[..., :2]
 
@@ -198,7 +202,7 @@ def _bilinear_zero_pad(plane: Tensor, gx: Tensor, gy: Tensor) -> Tensor:
     wx0, wy0 = 1 - wx1, 1 - wy1
     x0, y0 = x0f.long(), y0f.long()
     flat = plane.reshape(C, H * W)
-    out = torch.zeros(gx.shape[0], C, dtype=plane.dtype)
+    out = torch.zeros(gx.shape[0], C, dtype=plane.dtype, device=plane.device)
     for dy, wy in ((0, wy0), (1, wy1)):
         for dx, wx in ((0, wx0), (1, wx1)):
             xi, yi = x0 + dx, y0 + dy
@@ -219,7 +223,7 @@ def sample_planes(planes: Tensor, xyz: Tensor, box_warp: float, use_triplane: bo
         o = F.grid_sample(planes.reshape(N * P, C, H, W), g, mode='bilinear',
                           padding_mode='zeros', align_corners=False)
         return o.permute(0, 3, 2, 1).reshape(N, P, -1, C)
-    out = torch.empty(N, P, xyz.shape[1], C, dtype=planes.dtype)
+    out = torch.empty(N, P, xyz.shape[1], C, dtype=planes.dtype, device=planes.device)
     for n in range(N):
         for p in range(P):
             out[n, p] = _bilinear_zero_pad(planes[n, p], grid[n, p, :, 0], grid[n, p, :, 1])
