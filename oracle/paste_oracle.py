@@ -30,8 +30,8 @@ import torch.nn.functional as F
 def sobel_magnitude(x, eps=1e-6):
     """kornia.filters.sobel(x, normalized=True, eps=1e-6) for x (B,C,H,W): per-channel gradient magnitude."""
     b, c, h, w = x.shape
-    kx = torch.tensor([[-1., 0., 1.], [-2., 0., 2.], [-1., 0., 1.]], dtype=x.dtype) / 8
-    k = torch.stack([kx, kx.t()])[:, None].to(x.device)                                   # (2,1,3,3): d/dx, d/dy; conv = cross-correlation
+    kx = torch.tensor([[-1., 0., 1.], [-2., 0., 2.], [-1., 0., 1.]], dtype=x.dtype, device=x.device) / 8
+    k = torch.stack([kx, kx.t()])[:, None]                                                # (2,1,3,3): d/dx, d/dy; conv = cross-correlation
     g = F.conv2d(F.pad(x.reshape(b * c, 1, h, w), [1, 1, 1, 1], mode='replicate'), k).view(b, c, 2, h, w)
     return torch.sqrt(g[:, :, 0] * g[:, :, 0] + g[:, :, 1] * g[:, :, 1] + eps)
 
@@ -57,6 +57,21 @@ def kornia_shim():
 
 
 # ---------------------------------------------------------------- reference restatement
+def _flip(t):
+    """The reference's ``[-1, 1, -1]`` channel factor, on t's device and in t's dtype."""
+    return torch.tensor([-1., 1., -1.], dtype=t.dtype, device=t.device)[None, :, None, None]
+
+
+def orthofront_coords(view_xyz, bw, size):
+    """The unnormalised ``grid_sample`` source coordinates (row, column) of ``sample_orthofront``'s lookup in a
+    ``size`` x ``size`` image, BEFORE border clipping (aten GridSampler.h, align_corners=False): rows follow world y,
+    columns world x.  Tests use them to tell a clipped, a cell-boundary or an interior lookup apart."""
+    vij = 1 - (view_xyz[:, [1, 0]] + bw / 2) / bw
+    g = vij * 2 - 1
+    ix = ((g + 1) * size - 1) / 2
+    return ix[:, 0:1], ix[:, 1:2]
+
+
 def sample_orthofront(front, view_xyz, bw):
     """triplane.py:555-564: look the front image up at the (y, x) world position of every pixel."""
     vij = 1 - (view_xyz[:, [1, 0]] + bw / 2) / bw
@@ -66,7 +81,7 @@ def sample_orthofront(front, view_xyz, bw):
 
 def occlusion_rays(image_xyz, ray_start, offset=0.01):
     """triplane.py:565-570 (get_front_occlusion): rays from just in front of the visible surface, along +z."""
-    ro = image_xyz * torch.tensor([-1., 1., -1.])[None, :, None, None]
+    ro = image_xyz * _flip(image_xyz)
     ro[:, 2] -= ray_start - offset
     rd = torch.zeros_like(image_xyz)
     rd[:, 2] = 1
@@ -75,7 +90,7 @@ def occlusion_rays(image_xyz, ray_start, offset=0.01):
 
 def xyz_discrepancy(xyz, ro, rd):
     """triplane.py:601-606: distance of the rendered point from its own ray."""
-    p = xyz * torch.tensor([-1., 1., -1.])[None, :, None, None]
+    p = xyz * _flip(xyz)
     d = p - ro
     return (d - (d * rd).sum(dim=1, keepdim=True) * rd).norm(2, dim=1, keepdim=True)
 
@@ -83,36 +98,46 @@ def xyz_discrepancy(xyz, ro, rd):
 def paste_front(image, image_xyz, image_weights, front_rgb, occ, ro, rd, box_warp, frontw=None, normalize_images=False,
                 thresh_weight=0.95, thresh_edges=0.02, thresh_occ=0.05, thresh_dxyz=0.01, front_weight_erosion=0):
     """triplane.py:608-691 with the two G.f calls replaced by their results (occ, frontw).  Returns the reference's
-    dict plus the quantities in front of each threshold (``q_*``) so tests can tell a borderline pixel from an error."""
+    dict plus the quantities in front of each threshold (``q_*``) and the source coordinates of every lookup (``src_*``:
+    the paste's and the eroded weights' ``grid_sample`` row / column before clipping, the ``nearest`` up-sampling's
+    exact ``dst * R / S``) so tests can tell a borderline pixel from an error.  Runs on the inputs' device and dtype."""
     S = front_rgb.shape[-1]
+    R = image_xyz.shape[-1]
     with torch.no_grad():                                                      # the masks carry no gradient (:622)
         q_w = F.interpolate(image_weights, S, mode='bilinear')
-        wmask = (q_w > thresh_weight).float()
+        wmask = (q_w > thresh_weight).to(q_w.dtype)
         q_s = sobel_magnitude(F.interpolate(image_xyz, S, mode='bilinear')).norm(2, dim=1, keepdim=True)
-        smask = (q_s < thresh_edges).float()
-        fmask = F.interpolate((occ < thresh_occ).float(), S, mode='bilinear')
+        smask = (q_s < thresh_edges).to(q_s.dtype)
+        fmask = F.interpolate((occ < thresh_occ).to(occ.dtype), S, mode='bilinear')
         q_d_lo = xyz_discrepancy(image_xyz, ro, rd)
         q_d = F.interpolate(q_d_lo, S, mode='nearest')
-        dmask = (q_d < thresh_dxyz).float()
+        dmask = (q_d < thresh_dxyz).to(q_d.dtype)
         if front_weight_erosion >= 1:
-            eroded = erosion_ones((frontw > 0.5).float(), front_weight_erosion)
+            eroded = erosion_ones((frontw > 0.5).to(frontw.dtype), front_weight_erosion)
             fwmask = F.interpolate(sample_orthofront(eroded, F.interpolate(image_xyz, S, mode='bilinear'), box_warp), S, mode='nearest')
+            fw_row, fw_col = orthofront_coords(F.interpolate(image_xyz, S, mode='bilinear'), box_warp, eroded.shape[-1])
         else:
             fwmask = torch.ones_like(dmask)
+            fw_row = fw_col = None
         mask = wmask * smask * fmask * dmask * fwmask
     up_xyz = F.interpolate(image_xyz, S, mode='bilinear')                      # with gradient when grad_sample (:674-679)
     tocopy = front_rgb * 2 - 1 if normalize_images else front_rgb
     paste = sample_orthofront(tocopy, up_xyz, box_warp)
     out = torch.lerp(image, paste, mask)
+    with torch.no_grad():
+        src_row, src_col = orthofront_coords(up_xyz, box_warp, S)
     return {'image': out, 'paste': paste, 'mask': mask, 'mask_weights': wmask, 'mask_edges': smask, 'mask_occ': fmask,
             'mask_dxyz': dmask, 'mask_frontweight': fwmask, 'q_weights': q_w, 'q_edges': q_s, 'q_dxyz': q_d, 'q_occ_lo': occ,
-            'q_dxyz_lo': q_d_lo}
+            'q_dxyz_lo': q_d_lo, 'src_row': src_row, 'src_col': src_col, 'src_fw_row': fw_row, 'src_fw_col': fw_col,
+            'src_nearest': torch.arange(S, dtype=torch.float64, device=image_xyz.device) * R / S}
 
 
 # ---------------------------------------------------------------- seeded inputs (regenerated, never stored)
-def synth_paste_inputs(seed, N, R, S, box_warp=0.7, ray_start=0.5):
+def synth_paste_inputs(seed, N, R, S, box_warp=0.7, ray_start=0.5, reach=0.9):
     """Plausible render outputs: a smooth bumpy surface seen from the front with one depth step (so every mask has
-    both values), weights with a soft silhouette, rays that agree with the surface except for a band of noise."""
+    both values), weights with a soft silhouette, rays that agree with the surface except for a band of noise.
+    ``reach``: the fraction of the box the surface spans in x and y; above 1 a band of pixels on every side of the
+    image looks the front image up outside the box (the lookup clips, as for real background and silhouette pixels)."""
     g = np.random.Generator(np.random.PCG64(seed))
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
     lin = (np.arange(R, dtype=np.float64) + 0.5) / R
@@ -121,8 +146,8 @@ def synth_paste_inputs(seed, N, R, S, box_warp=0.7, ray_start=0.5):
     ro = np.zeros((N, 3, R, R)); rd = np.zeros((N, 3, R, R))
     for n in range(N):
         ph = g.uniform(0, 2 * np.pi, 4)
-        x = (0.5 - xx) * box_warp * 0.9 + 0.004 * np.sin(9 * yy + ph[0])
-        y = (0.5 - yy) * box_warp * 0.9 + 0.004 * np.sin(7 * xx + ph[1])
+        x = (0.5 - xx) * box_warp * reach + 0.004 * np.sin(9 * yy + ph[0])
+        y = (0.5 - yy) * box_warp * reach + 0.004 * np.sin(7 * xx + ph[1])
         z = 0.08 * np.sin(5 * xx + ph[2]) * np.cos(4 * yy + ph[3]) + 0.12 * (xx + 0.3 * yy > 0.8 + 0.1 * n)
         z = z + g.normal(0, 0.004, (R, R)) * (yy > 0.75)                      # a rough band: sobel above threshold
         xyz[n] = np.stack([x, y, z])

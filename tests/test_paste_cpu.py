@@ -52,6 +52,27 @@ def test_bad_arguments_fail_loudly():
     assert L.p3d_paste_occlusion_rays(None, 1, 8, 0.5, 0.01, None, None, None) != 0
 
 
+@pytest.mark.parametrize('guard', ['image', 'render'])
+def test_32bit_offset_guard_at_its_boundary(guard):
+    """Offsets inside a view and the (5, N, 1, S, S) parts stride are 32-bit in the kernels; check_params refuses a batch
+    with 5 * N * S^2 >= 2^31 or 3 * N * R^2 >= 2^31.  The largest N that passes gets as far as the NULL-input check."""
+    import __graft_entry__ as g
+    g.build()
+    import panic3d_b200.paste as pp
+    from panic3d_b200 import _lib
+    L = _lib.lib()
+    S, R, n_ok = (512, 8, 1638) if guard == 'image' else (16, 512, 2730)
+    assert 5 * n_ok * S * S < 2 ** 31 <= 5 * (n_ok + 1) * S * S if guard == 'image' else 3 * n_ok * R * R < 2 ** 31 <= 3 * (n_ok + 1) * R * R
+    p = pp.PasteParams()
+    p.res_render, p.res_image, p.box_warp = R, S, 0.7
+    for n, want in ((n_ok, b'NULL'), (n_ok + 1, b'32-bit offsets')):
+        p.n_views = n
+        assert L.p3d_paste_front(C.byref(p), *([None] * 8), *([None] * 4), None) != 0
+        assert want in L.p3d_last_error(), (n, L.p3d_last_error())
+        assert L.p3d_paste_front_backward(C.byref(p), *([None] * 7), None) != 0
+        assert want in L.p3d_last_error(), (n, L.p3d_last_error())
+
+
 def test_install_paste_rebinds_and_keeps_the_original():
     import panic3d_b200.dropin as dropin
     import panic3d_b200.paste as pp
