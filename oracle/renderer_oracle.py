@@ -132,14 +132,14 @@ def stratified_depths(u: Tensor, ray_start, ray_end, disparity: bool = False) ->
     """renderer.py:303-326.  u: (N,M,S,1) uniform [0,1)."""
     N, M, S, _ = u.shape
     if disparity:
-        t = torch.linspace(0, 1, S).reshape(1, 1, S, 1) + u * (1.0 / (S - 1))
+        t = torch.linspace(0, 1, S, dtype=u.dtype, device=u.device).reshape(1, 1, S, 1) + u * (1.0 / (S - 1))
         return 1.0 / (1.0 / ray_start * (1.0 - t) + 1.0 / ray_end * t)
     if isinstance(ray_start, torch.Tensor):          # per-ray limits ('auto' mode)
-        steps = (torch.arange(S, dtype=torch.float32) / (S - 1)).reshape(1, 1, S, 1)
+        steps = (torch.arange(S, dtype=u.dtype, device=u.device) / (S - 1)).reshape(1, 1, S, 1)
         base = ray_start[:, :, None, :] + steps * (ray_end - ray_start)[:, :, None, :]
         delta = (ray_end - ray_start) / (S - 1)
         return base + u * delta[..., None]
-    base = torch.linspace(ray_start, ray_end, S).reshape(1, 1, S, 1)
+    base = torch.linspace(ray_start, ray_end, S, dtype=u.dtype, device=u.device).reshape(1, 1, S, 1)
     return base + u * ((ray_end - ray_start) / (S - 1))
 
 
@@ -264,9 +264,17 @@ def cull_mask(sigma: Tensor, thresh: float) -> Tensor:
     return (1 - torch.exp(-F.softplus(sigma - 1))) < thresh
 
 
-def apply_masks(sigma: Tensor, xyz: Tensor, box_warp: float, triplane_crop, cull_clouds, binarize_clouds) -> Tensor:
-    """renderer.py:187-198 / :227-238 (order: crop, then binarize XOR cull)."""
+def apply_masks(sigma: Tensor, xyz: Tensor, box_warp: float, triplane_crop, cull_clouds, binarize_clouds,
+                mask: Optional[Tensor] = None) -> Tensor:
+    """renderer.py:187-198 / :227-238 (order: crop, then binarize XOR cull).  `mask` (bool, like sigma), when given, replaces
+    the decision: True where the density is forced to -1e3; under binarize every other density is forced to 1e3."""
     sigma = sigma.clone()
+    if mask is not None:
+        if triplane_crop or cull_clouds or binarize_clouds:
+            sigma[mask] = -1e3
+            if binarize_clouds:
+                sigma[~mask] = 1e3
+        return sigma
     if triplane_crop:
         sigma[crop_mask(xyz, triplane_crop, box_warp)] = -1e3
     if binarize_clouds:
@@ -314,7 +322,7 @@ def importance_depths(z: Tensor, w: Tensor, u: Tensor, eps: float = 1e-5) -> Ten
     bins = 0.5 * (z[:, :-1] + z[:, 1:])                        # R,S-1
     wi = wp[:, 1:-1] + eps                                     # R,S-3
     pdf = wi / wi.sum(-1, keepdim=True)
-    cdf = torch.cat([torch.zeros(R, 1), torch.cumsum(pdf, -1)], -1)   # R,S-2
+    cdf = torch.cat([torch.zeros(R, 1, dtype=pdf.dtype, device=pdf.device), torch.cumsum(pdf, -1)], -1)   # R,S-2
     nb = wi.shape[1]
     inds = torch.searchsorted(cdf, u.contiguous(), right=True)
     below = (inds - 1).clamp_min(0)
@@ -340,15 +348,25 @@ def run_model(planes, dec, xyz, opts, use_triplane, gather='manual'):
 def render(planes: Tensor, dec: Dict, ro: Tensor, rd: Tensor, opts: Dict,
            u_coarse: Tensor, u_fine: Optional[Tensor], use_triplane: bool = True,
            triplane_crop=None, cull_clouds=None, binarize_clouds=None,
-           gather: str = 'manual', depth_bounds: Optional[Tuple[Tensor, Tensor]] = None, return_bounds: bool = False):
+           gather: str = 'manual', depth_bounds: Optional[Tuple[Tensor, Tensor]] = None, return_bounds: bool = False,
+           depths: Optional[Tuple[Tensor, Optional[Tensor]]] = None, masks: Optional[Tuple[Tensor, Optional[Tensor]]] = None,
+           return_samples: bool = False):
     """ImportanceRenderer.forward, renderer.py:162-264.
-    Returns rgb (N,M,32), depth (N,M,1), wsum (N,M,1), xyz (N,M,3)."""
+    Returns rgb (N,M,32), depth (N,M,1), wsum (N,M,1), xyz (N,M,3).
+
+    `depths` = (coarse (N,M,S,1), fine (N,M,Sf,1) or None) and `masks` = (coarse (N,M*S,1), fine (N,M*Sf,1) or None, bool:
+    True where apply_masks forced the density to -1e3) replace the ones render would compute.  Both are constants of the
+    reference graph (the fine depths come from no_grad, the masks are in-place overwrites), so injecting another run's
+    values - a kernel's fp32 ones into an fp64 run - changes no derivative, only which samples exist and which are masked.
+    return_samples appends dict(depths=..., masks=...) of this run, in the form these arguments take."""
     N, M, _ = ro.shape
     S = int(opts['depth_resolution'])
     Sf = int(opts['depth_resolution_importance'])
     bw = opts['box_warp']
     white = bool(opts.get('white_back', False))
-    if opts['ray_start'] == 'auto' and opts['ray_end'] == 'auto':
+    if depths is not None:
+        d_c = depths[0]
+    elif opts['ray_start'] == 'auto' and opts['ray_end'] == 'auto':
         t0, t1 = ray_limits_box(ro, rd, bw)
         ok = t1 > t0
         if bool(ok.any()):
@@ -359,19 +377,24 @@ def render(planes: Tensor, dec: Dict, ro: Tensor, rd: Tensor, opts: Dict,
         d_c = stratified_depths(u_coarse, opts['ray_start'], opts['ray_end'],
                                 opts.get('disparity_space_sampling', False))
     lo, hi = (None, None) if depth_bounds is None else depth_bounds
+    m_c, m_f = (None, None) if masks is None else masks
+    flags = (triplane_crop, cull_clouds, binarize_clouds)
 
     xyz_c = (ro[:, :, None] + d_c * rd[:, :, None]).reshape(N, -1, 3)
     rgb_c, sig_c = run_model(planes, dec, xyz_c, opts, use_triplane, gather)
-    sig_c = apply_masks(sig_c, xyz_c, bw, triplane_crop, cull_clouds, binarize_clouds)
+    sig_c = apply_masks(sig_c, xyz_c, bw, *flags, mask=m_c)
     rgb_c = rgb_c.reshape(N, M, S, -1)
     sig_c = sig_c.reshape(N, M, S, 1)
     xyz_c = xyz_c.reshape(N, M, S, 3)
     if Sf > 0:
         _, _, w = march(rgb_c, sig_c, d_c, white, lo, hi)
-        d_f = importance_depths(d_c.reshape(N * M, S), w.reshape(N * M, S - 1), u_fine).reshape(N, M, Sf, 1).detach()   # no_grad in the reference (renderer.py:332)
+        if depths is not None:
+            d_f = depths[1]
+        else:
+            d_f = importance_depths(d_c.reshape(N * M, S), w.reshape(N * M, S - 1), u_fine).reshape(N, M, Sf, 1).detach()   # no_grad in the reference (renderer.py:332)
         xyz_f = (ro[:, :, None] + d_f * rd[:, :, None]).reshape(N, -1, 3)
         rgb_f, sig_f = run_model(planes, dec, xyz_f, opts, use_triplane, gather)
-        sig_f = apply_masks(sig_f, xyz_f, bw, triplane_crop, cull_clouds, binarize_clouds)
+        sig_f = apply_masks(sig_f, xyz_f, bw, *flags, mask=m_f)
         d_all = torch.cat([d_c, d_f], -2)
         order = torch.sort(d_all, dim=-2, stable=True)[1]
         d_all = torch.gather(d_all, -2, order)
@@ -383,9 +406,13 @@ def render(planes: Tensor, dec: Dict, ro: Tensor, rd: Tensor, opts: Dict,
         d_all, col, sig = d_c, torch.cat([rgb_c, xyz_c], -1), sig_c
     out, depth, w = march(col, sig, d_all, white, lo, hi)
     res = (out[..., :-3], depth, w.sum(2), out[..., -3:])
+    extra = []
     if return_bounds:          # (min, max) over every depth of this batch: what ray_marcher.py:50 clamps to
-        return res, (d_all.min(), d_all.max())
-    return res
+        extra.append((d_all.min(), d_all.max()))
+    if return_samples:
+        extra.append(dict(depths=(d_c, d_f if Sf > 0 else None),
+                          masks=(sig_c.reshape(N, -1, 1) == -1e3, sig_f == -1e3 if Sf > 0 else None)))
+    return (res, *extra) if extra else res
 
 
 # --------------------------------------------------------------------------
