@@ -25,8 +25,6 @@ constexpr int kGW = 12, kEW = 8, kTeams = 3;
 constexpr int kWarpsD = kGW + kEW;
 constexpr int kThreadsD = kWarpsD * 32;          // 640
 constexpr int kNA = 4;                           // A1 ring depth
-constexpr int kD2Cols = 48;
-constexpr int kLBO_W2 = 768;
 
 struct __align__(1024) DecSmem {
     unsigned char a1[kNA][2][4 * kLBO_A1];
@@ -62,8 +60,7 @@ __global__ void __launch_bounds__(kThreadsD, 1) k_decode_tc(const DecArgs a) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     stage_w1_biases(g, a.w1, a.b1, a.b2, sm.w1, sm.b1, sm.b2c, sm.b2s, tid, kThreadsD);
-    // tile rows 0..31: the colour rows; row 32: the sigma row; 33..47: zeros
-    stage_w2(g, a.w2, sm.w2, kD2Cols, kLBO_W2, [](int n) { return n < kRgb ? n + 1 : (n == kRgb ? 0 : -1); }, tid, kThreadsD);
+    stage_w2(g, a.w2, sm.w2, kD2Cols, kLBO_W2, w2_row_n48, tid, kThreadsD);
     fence_proxy_async();
     __syncthreads();
 

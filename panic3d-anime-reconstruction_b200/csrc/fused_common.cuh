@@ -36,6 +36,28 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t pari
     asm volatile("trap;");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// per-warpgroup register budget (every thread of the warpgroup executes it); N a multiple of 8 in [24, 256]
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+// ---- bulk copies (TMA without a tensor map): contiguous, 16-byte aligned, sizes a multiple of 16.
+// shared -> global, tracked by the issuing thread's bulk groups: wait_read() frees the source, wait_all() completes the writes
+__device__ __forceinline__ void bulk_store(void* gdst, uint32_t ssrc, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// global -> shared, completes `bytes` of the transaction count of `bar`
+__device__ __forceinline__ void bulk_load(uint32_t sdst, const void* gsrc, uint32_t bytes, unsigned long long* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(sdst), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
 // ---- warpgroup MMA (sm_90a).  Operands in shared memory use the K-major, no-swizzle canonical layout of tile_off():
 // 8-row x 16-byte core matrices, kSBO bytes between 8-row groups, `lbo` bytes between 8-column (16-byte) groups along K.
 // A warpgroup's accumulator fragment of m64nN: element i of thread (warp w, lane l) is row 16 w + l / 4 + 8 ((i / 2) & 1),
@@ -149,6 +171,11 @@ __device__ __forceinline__ void stage_w1_biases(const Geom& g, const float* w1, 
     if (tid < kRgb) sb2c[tid] = -__fmul_rn(b2[tid + 1], g.b2_gain) * kLog2e;
     if (tid == 0) sb2s = __fmul_rn(b2[0], g.b2_gain);
 }
+// Layer 2 as one N = 48 wgmma tile: rows 0..31 the colour rows (W2 rows 1..32), row 32 sigma (W2 row 0), rows 33..47 zero -
+// so the accumulator holds the 32 colour logits in fragment elements 0..15 and sigma in column 32 (elements 16, 18 of the
+// threads with lane % 4 == 0).
+constexpr int kD2Cols = 48, kLBO_W2 = 768;
+__device__ __forceinline__ int w2_row_n48(int n) { return n < kRgb ? n + 1 : (n == kRgb ? 0 : -1); }
 // rows [0, rows) of a layer-2 weight tile (K = 64): tile row n holds W2 row w2_row(n) (0 = sigma, 1..32 = colours, -1 = zeros)
 template <int B, class RowMap>
 __device__ __forceinline__ void stage_w2(const Geom& g, const float* w2, unsigned char (&tile)[2][B], int rows, int lbo, RowMap w2_row,

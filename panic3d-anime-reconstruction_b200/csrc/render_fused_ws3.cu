@@ -6,7 +6,9 @@
 // staged in global memory, in this CTA's own slice of the workspace colour buffers (see colour_area: coarse areas
 // CA[n % 3] and one fine area FA, 4 x 48 KB per CTA, ~25 MB on 132 SMs).  The areas are rewritten every few groups, so
 // their footprint fits the 50 MB L2, but they share it with the streamed tri-plane gather; how much of the round trip is
-// served by L2 rather than HBM has not been measured.  Only
+// served by L2 rather than HBM has not been measured.  Both directions are bulk copies of whole 8 KB tile halves: the
+// epilogue stages them in shared memory for one cp.async.bulk store, and a group's tiles come back into shared memory
+// buffers (mbarrier complete_tx) while the decoder runs C(n+2), so colours(n) reduces from shared memory.  Only
 // the COARSE colours of a group have to wait through a whole fine pass; the fine ones are consumed right after the group's
 // merge, so all groups share one fine area.  With F(n) followed by C(n+2):
 //   * importance(n) has two passes of slack (F(n-1), C(n+1)) before the gather of F(n) needs its depths;
@@ -17,8 +19,9 @@
 //
 //   warps  0-11  GATHER    three teams of four warps; team j takes tiles j, j+3, ... of the tile sequence
 //   warps 12-19  DECODER   two warpgroups, one per 64-row half of every tile: layer 1 (wgmma, A1 and W1 from shared memory)
-//                          -> softplus2 in registers -> layer 2 (wgmma, A from the registers): colour sigmoids -> colour area,
-//                          sigma -> group state; colour reduction of a group once its omega is ready
+//                          -> softplus2 in registers -> layer 2 (one m64n48 wgmma, A from the registers): colour sigmoids ->
+//                          staging tile -> bulk store to the colour area, sigma -> group state; bulk loads of a group's
+//                          colours and their reduction once its omega is ready
 //   warps 20-23  RAY       a warp per ray: importance sampling after a group's coarse pass, merge / transmittance /
 //                          omega and the per-ray outputs after its fine pass
 #include "fused_common.cuh"
@@ -34,10 +37,14 @@ constexpr int kGW = 12, kEW = 8, kRW = 4, kTeams = 3;   // 24 warps = 6 warpgrou
 constexpr int kWarpsWS = kGW + kEW + kRW;
 constexpr int kThreadsWS = kWarpsWS * 32;        // 768
 constexpr int kNA = 4;                           // A1 ring depth
+// registers per thread by role (launched with 80 = 65536 / 768 rounded down to 8): the decoder warpgroups hold the layer-2
+// A operands and accumulators at once and take what the ray warpgroup does not need; 3 x 80 + 2 x kRegE + kRegR <= 6 x 80
+constexpr int kRegE = 88, kRegR = 64;
+static_assert(3 * 80 + 2 * kRegE + kRegR <= 6 * 80, "per-role registers exceed what the launch allocates");
 constexpr int kStates = 4;                       // per-group state ring
 constexpr int kRowsG = 384;                      // rows per pass per group
-
-constexpr int kLBO_W2C = 512, kLBO_W2S = 256;
+constexpr int kColBufs = 3;                      // colour tiles of a group in shared memory at once (colours())
+constexpr int kHalfBytes = 64 * kRgb * 4;        // one decoder warpgroup's 64 rows of colour sigmoids: 8 KB
 
 
 struct GroupState {                               // written by G (t_c, crop), E (sg_*), R (t_f)
@@ -53,7 +60,9 @@ struct SlotState {                                // written by R (composite), r
 
 struct __align__(1024) WsSmem {
     unsigned char a1[kNA][2][4 * kLBO_A1];
-    unsigned char w1[2][4096], w2c[2][4096], w2s[2][2048];
+    float col_stage[2][64 * kRgb];                // per decoder warpgroup: its half of the tile being stored (col_idx layout)
+    float col_buf[kColBufs][128 * kRgb];          // colour tiles loaded back for colours(), same layout
+    unsigned char w1[2][4096], w2[2][kD2Cols * 128];
     float b1[kHidden], b2c[kRgb], b2s, pad0[3];
     uint4 tab[kGW][32][4];                        // tap table of a gather warp's 32 rows (see "gather" below)
     GroupState st[kStates];
@@ -62,7 +71,13 @@ struct __align__(1024) WsSmem {
     unsigned long long a1_full[kNA], a1_empty[kNA];
     unsigned long long fine_ready[kStates], state_free[kStates];
     unsigned long long sigc_ready[kStates], sigf_ready[kStates], omega_ready[2];   // E -> R (sigma in smem), R -> E (omega)
+    unsigned long long col_full[kColBufs];        // both warpgroups' halves of a col_buf tile have landed (complete_tx)
 };
+
+// Float index of colour (row, c) in a staged / loaded colour tile: 128 B rows, 16-byte chunk (c / 4) XOR (row % 8).  The
+// epilogue's float2 stores (8 rows x 4 column pairs per instruction) and the reduction's lane = channel loads are both
+// conflict-free.  The colour areas in global memory are byte copies of the tiles, so they hold the same layout.
+__device__ __forceinline__ int col_idx(int row, int c) { return row * kRgb + ((((c >> 2) ^ row) & 7) << 2) + (c & 3); }
 
 static_assert(sizeof(WsSmem) + 1024 <= 232448, "WsSmem + alignment slack exceeds the 227 KB a CTA can opt into");
 
@@ -120,11 +135,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             mbar_init(&sm.sigc_ready[i], kEW); mbar_init(&sm.sigf_ready[i], kEW);
         }
         mbar_init(&sm.omega_ready[0], kRW); mbar_init(&sm.omega_ready[1], kRW);
+        for (int i = 0; i < kColBufs; ++i) mbar_init(&sm.col_full[i], 2);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     stage_w1_biases(g, a.w1, a.b1, a.b2, sm.w1, sm.b1, sm.b2c, sm.b2s, tid, kThreadsWS);
-    stage_w2(g, a.w2, sm.w2c, kRgb, kLBO_W2C, [](int n) { return n + 1; }, tid, kThreadsWS);         // the colour rows (32 x 64)
-    stage_w2(g, a.w2, sm.w2s, 16, kLBO_W2S, [](int n) { return n == 0 ? 0 : -1; }, tid, kThreadsWS);  // sigma + 15 zero rows
+    stage_w2(g, a.w2, sm.w2, kD2Cols, kLBO_W2, w2_row_n48, tid, kThreadsWS);
     fence_proxy_async();
     __syncthreads();
 
@@ -185,68 +200,75 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         }
     } else if (warp < kGW + kEW) {
         // =========================================================================== DECODER
+        setmaxnreg_inc<kRegE>();
         const int e = warp - kGW, quarter = e & 3, chunk = e >> 2;      // chunk = warpgroup = 64-row half of a tile
         const int etid = tid - kGW * 32;                                  // 0..255 inside the decoder group
-        // this CTA's colour area of (group n, pass): 384 rows x 32 sigmoids, row = 128 k + row of tile k.  Areas are slices of
-        // the workspace colour buffers that belong to this CTA's own first two groups (coarse and fine buffer each), so they
-        // exist whenever they are used: CA[0..2] = slices 0..2, FA = slice 3 (slice 1 when the CTA has a single group)
+        const bool elect = (etid & 127) == 0;                             // the warpgroup's bulk-copy thread
+        // this CTA's colour area of (group n, pass): 384 rows x 32 sigmoids, row = 128 k + row of tile k, each tile in the
+        // col_idx layout (a byte copy of the staged tile).  Areas are slices of the workspace colour buffers that belong to this
+        // CTA's own first two groups (coarse and fine buffer each), so they exist whenever they are used: CA[0..2] = slices
+        // 0..2, FA = slice 3 (slice 1 when the CTA has a single group)
         auto colour_area = [&](int n, int pass) -> float* {
             const int j = pass == 0 ? n % 3 : (n_my >= 2 ? 3 : 1);
             return ((j & 1) ? a.col_f : a.col_c) + ((long long)blockIdx.x + (long long)(j >> 1) * gridDim.x) * (kRowsG * kRgb);
         };
         auto ebar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };   // the eight decoder warps
+        auto wgbar = [chunk] { asm volatile("bar.sync %0, 128;" ::"r"(2 + chunk) : "memory"); };   // this warpgroup's four warps
+        // Colour tile t of a group (t = 0..2: coarse tile t, 3..5: fine tile t - 3) is loaded into col_buf[t % kColBufs].  Each
+        // warpgroup loads back the half it stored itself, so the only stores a load depends on are the issuing thread's own.
+        auto load_tile = [&](int n, int t) {                             // elected thread only
+            const int pass = t / 3, b = t % kColBufs;
+            mbar_arrive_expect_tx(&sm.col_full[b], kHalfBytes);
+            bulk_load(smem_u32(sm.col_buf[b]) + chunk * kHalfBytes, colour_area(n, pass) + ((t - 3 * pass) * 128 + 64 * chunk) * kRgb,
+                      kHalfBytes, &sm.col_full[b]);
+        };
+        // The first kColBufs tiles of group n are requested once its fine pass is stored: in the epilogue of the next tile,
+        // C(n+2)'s first, so they arrive while the decoder runs C(n+2) - or at the top of colours(n) where no C(n+2) exists.
+        // A full wait_group (the stores are written, not just read) and the proxy fence make the area readable by the loads.
+        int stored = -1, loaded = -1;                                     // last group whose fine pass was stored / first tiles requested
+        auto first_loads = [&](int n) {
+            if (elect) {
+                bulk_wait_all();
+                fence_proxy_async_global();
+#pragma unroll 1
+                for (int t = 0; t < kColBufs; ++t) load_tile(n, t);
+            }
+            loaded = n;
+        };
         auto colours = [&](int n) {                                        // sum_j omega_j * rgb_j for group n
+            if (loaded < n) first_loads(n);
             const int slot_i = n & 1;
             SlotState& sl = sm.slot[slot_i];
             mbar_wait(&sm.omega_ready[slot_i], (n >> 1) & 1);              // omega / pos / back of group n (ray warps)
             const int grp = (int)blockIdx.x + n * (int)gridDim.x;
             const long long ray0 = (long long)grp * GR;
-            // A warp's 32 rows are the same ray(s) in each of its three tiles, so the per-tile column sums are first added
-            // up in a register and published once: every (ray, channel) cell of sl.acc then receives exactly two
-            // shared-memory adds (one per chunk), whose order cannot change the rounded sum - the kernel is
-            // bit-reproducible run to run and independent of how the rays are batched.
-            float part[2] = {0.f, 0.f};
-            const int rl_first = (quarter * 32) / RPT;
-            for (int i = 0; i < 3; ++i) {
-                const int tile6 = chunk + 2 * i;                           // this warp's tiles: {0,2,4} or {1,3,5}
-                const int pass = tile6 / 3, k = tile6 - pass * 3;
-                const int trow = quarter * 32 + lane;
-                const int rl = trow / RPT, s = k * RPT + (trow - rl * RPT);
-                const bool live = ray0 + rl < a.R;
-                const float om = live ? sl.om[rl * L + sl.pos[pass * kRowsG + rl * S + s]] : 0.f;
-                const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
-                float v[32];
-                // (an unsigned row offset: with a signed one ptxas spills the extended address across the omega wait at S = 96)
-                const float4* src = reinterpret_cast<const float4*>(colour_area(n, pass) + (unsigned)(k * 128 + trow) * kRgb);
-#pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) {
-                    const float4 q4 = src[c4];
-                    v[4 * c4] = q4.x; v[4 * c4 + 1] = q4.y; v[4 * c4 + 2] = q4.z; v[4 * c4 + 3] = q4.w;
+            // Warp e sums rows [16 e, 16 e + 16) of each of the six tiles - always one ray, rl - with lane = channel, in a fixed
+            // order.  The partial sums of a ray meet in sl.acc as one (S = 48) or two (S = 96: warps 2 rl, 2 rl + 1)
+            // shared-memory adds onto 0, whose order cannot change the rounded sum: the kernel is bit-reproducible run to run
+            // and independent of how the rays are batched.
+            const int rl = 16 * e / RPT;
+            const bool live = ray0 + rl < a.R;
+            float part = 0.f;
+#pragma unroll 1
+            for (int t = 0; t < 6; ++t) {
+                const int pass = t / 3, k = t - 3 * pass, b = t % kColBufs;
+                mbar_wait(&sm.col_full[b], ((6 * n + t) / kColBufs) & 1);
+                const float* buf = sm.col_buf[b];
+                const unsigned short* pos = sl.pos + pass * kRowsG + rl * S + k * RPT - rl * RPT;   // pos[trow]: the row's merged position
+#pragma unroll 4
+                for (int j = 0; j < 16; ++j) {
+                    const int trow = 16 * e + j;
+                    const float om = live ? sl.om[rl * L + pos[trow]] : 0.f;
+                    const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
+                    part += fmaf(buf[col_idx(trow, lane)], ca, cb);
                 }
-#pragma unroll
-                for (int c = 0; c < kRgb; ++c) v[c] = fmaf(v[c], ca, cb);
-#pragma unroll
-                for (int t2 = 0; t2 < 32 / RPT; ++t2) {
-                    const int target = rl_first + t2;
-                    float r[32];
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) r[c] = (RPT == 32 || rl == target) ? v[c] : 0.f;
-#pragma unroll
-                    for (int off = 16; off >= 1; off >>= 1) {
-                        const bool up = (lane & off) != 0;
-#pragma unroll
-                        for (int j = 0; j < off; ++j) {
-                            const float send = up ? r[j] : r[j + off];
-                            const float keep = up ? r[j + off] : r[j];
-                            r[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                        }
-                    }
-                    part[t2] += r[0];
+                if (t + kColBufs < 6) {
+                    wgbar();                                               // this warpgroup's half of col_buf[b] is read
+                    if (elect) load_tile(n, t + kColBufs);
                 }
             }
-#pragma unroll
-            for (int t2 = 0; t2 < 32 / RPT; ++t2) atomicAdd(&sl.acc[rl_first + t2][lane], part[t2]);
-            ebar();                                                        // all eight decoder warps (also: the areas are read)
+            atomicAdd(&sl.acc[rl][lane], part);
+            ebar();                                                        // all eight decoder warps (also: the buffers are read)
             if (etid < GR * kRgb) {
                 const int rl = etid >> 5, c = etid & 31;
                 const long long ray = ray0 + rl;
@@ -258,8 +280,8 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
 
         // colours(n) needs omega from the ray warps; it runs at the top of the first tile of F(n+1) - three tiles (C(n+2))
         // after the group's last sigma - which is also the last point before F(n+1) overwrites the fine area.
-        const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]);
-        const uint32_t w2ch = smem_u32(sm.w2c[0]), w2cl = smem_u32(sm.w2c[1]), w2sh = smem_u32(sm.w2s[0]), w2sl = smem_u32(sm.w2s[1]);
+        const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]), w2h = smem_u32(sm.w2[0]), w2l = smem_u32(sm.w2[1]);
+        float* stage_tile = sm.col_stage[chunk];
         for (int it = 0; it < T; ++it) {
             const TileDesc td = tile_at(it, n_my);
             if (td.pass == 1 && td.k == 0 && td.n >= 1) colours(td.n - 1);
@@ -271,27 +293,28 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             if (lane == 0) mbar_arrive(&sm.a1_empty[stage]);
             uint32_t ah[16], al[16];
             decoder_hidden(d1, sm.b1, lane, ah, al);
-            float dc[16], ds[4];
-            decoder_layer2_issue<kRgb>(dc, ah, al, w2ch, w2cl, kLBO_W2C, a.single_pass);
-            decoder_layer2_issue<8>(ds, ah, al, w2sh, w2sl, kLBO_W2S, a.single_pass);
+            float d2[kD2Cols / 2];
+            decoder_layer2_issue<kD2Cols>(d2, ah, al, w2h, w2l, kLBO_W2, a.single_pass);
             wgmma_commit();
             wgmma_wait_all();
-            fence_operands(dc);
-            fence_operands(ds);
-            // this thread's two rows of the tile (fragment elements 2 rs, 2 rs + 1 of each 8-column block)
-            float* area = colour_area(td.n, td.pass) + td.k * 128 * kRgb;
+            fence_operands(d2);
+            // the staging half is free once the bulk store of the previous tile has read it
+            if (stored > loaded) first_loads(stored);
+            else if (elect) bulk_wait_read();
+            wgbar();
             GroupState& st = sm.st[td.n & 3];
+            // this thread's two rows of the half (fragment elements 2 rs, 2 rs + 1 of each 8-column block)
 #pragma unroll
             for (int rs = 0; rs < 2; ++rs) {
-                const int trow = 64 * chunk + frag_row(2 * rs, lane, quarter);
+                const int hrow = frag_row(2 * rs, lane, quarter), trow = 64 * chunk + hrow;
 #pragma unroll
                 for (int blk = 0; blk < 4; ++blk) {
                     const int i = 4 * blk + 2 * rs, c = frag_col(i, lane);
-                    *reinterpret_cast<float2*>(area + trow * kRgb + c) =
-                        make_float2(rcp_approx(1.f + ex2_approx(dc[i] + sm.b2c[c])), rcp_approx(1.f + ex2_approx(dc[i + 1] + sm.b2c[c + 1])));
+                    *reinterpret_cast<float2*>(stage_tile + col_idx(hrow, c)) =
+                        make_float2(rcp_approx(1.f + ex2_approx(d2[i] + sm.b2c[c])), rcp_approx(1.f + ex2_approx(d2[i + 1] + sm.b2c[c + 1])));
                 }
-                if ((lane & 3) == 0) {                                    // column 0 of the sigma accumulator
-                    float sg = ds[2 * rs] + sm.b2s;
+                if ((lane & 3) == 0) {                                    // column 32: sigma
+                    float sg = d2[16 + 2 * rs] + sm.b2s;
                     const int rl = trow / RPT, s = td.k * RPT + (trow - rl * RPT);
                     const int srow = rl * S + s;
                     if (st.crop[td.pass][srow]) sg = -1e3f;
@@ -300,8 +323,14 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                     (td.pass == 0 ? st.sg_c : st.sg_f)[srow] = sg;
                 }
             }
-            if (td.k == 2) {                                              // the group's pass is complete: hand it to the ray warps
-                __threadfence_block();                                    // (its colour-area stores included)
+            fence_proxy_async();                                          // the staging writes, seen by the bulk store
+            wgbar();
+            if (elect) {
+                bulk_store(colour_area(td.n, td.pass) + (td.k * 128 + 64 * chunk) * kRgb, smem_u32(stage_tile), kHalfBytes);
+                bulk_commit();
+            }
+            if (td.k == 2) {                                              // the group's pass is complete: hand its sigma to the ray warps
+                if (td.pass == 1) stored = td.n;
                 __syncwarp();
                 if (lane == 0) mbar_arrive(td.pass == 0 ? &sm.sigc_ready[td.n & 3] : &sm.sigf_ready[td.n & 3]);
             }
@@ -309,6 +338,7 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         colours(n_my - 1);
     } else if (warp < kGW + kEW + kRW) {
         // =========================================================================== RAY (one warp per ray)
+        setmaxnreg_dec<kRegR>();
         const int rw = warp - kGW - kEW;
         float* scr = sm.rscratch[rw];
         constexpr int NC = (S + 31) / 32, nb = S - 3;
