@@ -10,6 +10,7 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB = os.path.join(PKG, 'lib', 'libp3d.so')
+OBJDIR = os.path.join(PKG, 'lib', 'obj')                          # per-source objects (git-ignored build products)
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 NVCC_FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
@@ -27,9 +28,30 @@ def _stale():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
+def object_path(src):
+    return os.path.join(OBJDIR, os.path.basename(src)[:-3] + '.o')
+
+
+def find_nvcc():
+    nvcc = shutil.which('nvcc') or '/usr/local/cuda/bin/nvcc'
+    if not os.path.exists(nvcc):
+        raise RuntimeError('nvcc not found: cannot build libp3d.so')
+    return nvcc
+
+
+def compile_cmd(nvcc, src, obj, extra=()):
+    """nvcc command line that compiles one translation unit into a relocatable object; `extra` goes before -c."""
+    return [nvcc] + [x for x in NVCC_FLAGS if x != '-shared'] + list(extra) + ['-c', src, '-o', obj]
+
+
+def link_cmd(nvcc, lib, objs):
+    """nvcc command line that links the objects into the shared library."""
+    return [nvcc] + ARCH + ['-shared', '-o', lib] + list(objs) + ['-lz']     # zlib: deflate + crc32 of the PNG writer (csrc/image_io.cu)
+
+
 def _compile_one(nvcc, src, obj, verbose):
-    cmd = [nvcc] + [x for x in NVCC_FLAGS if x != '-shared'] + (['-Xptxas', '-v'] if verbose else []) + ['-c', src, '-o', obj]
-    r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    r = subprocess.run(compile_cmd(nvcc, src, obj, ['-Xptxas', '-v'] if verbose else []),
+                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     return src, r.returncode, r.stdout
 
 
@@ -41,16 +63,13 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not _stale():
         return LIB
     from concurrent.futures import ThreadPoolExecutor
-    nvcc = shutil.which('nvcc') or '/usr/local/cuda/bin/nvcc'
-    if not os.path.exists(nvcc):
-        raise RuntimeError('nvcc not found: cannot build libp3d.so')
-    objdir = os.path.join(PKG, 'lib', 'obj')                      # per-source objects (git-ignored build products)
-    os.makedirs(objdir, exist_ok=True)
+    nvcc = find_nvcc()
+    os.makedirs(OBJDIR, exist_ok=True)
     headers = glob.glob(os.path.join(CSRC, '*.cuh')) + glob.glob(os.path.join(PKG, '..', 'include', '*.h')) + [os.path.abspath(__file__)]
     t_hdr = max(os.path.getmtime(h) for h in headers)
     jobs, objs = [], []
     for src in sources():
-        obj = os.path.join(objdir, os.path.basename(src)[:-3] + '.o')
+        obj = object_path(src)
         objs.append(obj)
         if force or not os.path.exists(obj) or os.path.getmtime(obj) < max(t_hdr, os.path.getmtime(src)):
             jobs.append((src, obj))
@@ -63,8 +82,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose:
             print(out)
     tmp = LIB + '.tmp.%d' % os.getpid()
-    r = subprocess.run([nvcc] + ARCH + ['-shared', '-o', tmp] + objs + ['-lz'],     # zlib: deflate + crc32 of the PNG writer (csrc/image_io.cu)
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    r = subprocess.run(link_cmd(nvcc, tmp, objs), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)
         raise RuntimeError('nvcc failed linking libp3d.so')

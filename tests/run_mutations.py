@@ -1,0 +1,155 @@
+"""Mutation check of the GPU tests (needs an H100): build libp3d.so once per single-line value mutation of a target's CUDA
+source into a temporary directory, run the target's GPU test file against it (P3D_LIBP3D), and report whether the file
+fails it, as it must.  The tree is not modified.
+
+    python tests/run_mutations.py TARGET [TARGET ...] [--files F ...] [--json out.json] [--build-only]
+
+TARGET is one of decode_tc, paste_front, render_backward, modconv.  --files runs other GPU files against the same mutants
+instead (to see which of them the rest of the suite catches); the exit code then only reports that the run completed.
+--build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from panic3d_b200 import _build  # noqa: E402
+
+# decode_tc.cu: every mutation keeps all memory accesses in bounds and leaves the mbarrier protocol alone (stage index,
+# parities, arrival counts and the team stride are untouched), so none can hang.
+TILE = 'const long long tile = (long long)blockIdx.x + (long long)it * gridDim.x;'
+DECODE_TC = {
+    # the gather computes tile it % 3 instead of tile it from the fourth tile of a CTA on
+    'gather tile it % kTeams': (TILE + '\n            // ---- tap table',
+                                TILE.replace('(long long)it *', '(long long)(it % kTeams) *') + '\n            // ---- tap table'),
+    # the decoder writes tile it % 4's outputs from the fifth tile of a CTA on
+    'decoder output tile it % kNA': (TILE + '\n#pragma unroll\n            for (int rs',
+                                     TILE.replace('(long long)it *', '(long long)(it % kNA) *') + '\n#pragma unroll\n            for (int rs'),
+    'tap-row view index 0': ('px, py, pz, (uint32_t)view);', 'px, py, pz, 0u);'),
+    'single pass never set': ('a.single_pass = p->mlp_mode == P3D_MLP_TC_BF16;', 'a.single_pass = 0;'),
+    'tiles per CTA rounded down': ('(a.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x',
+                                   '(a.n_tiles - (int)blockIdx.x) / (int)gridDim.x'),
+    'gather row shifted by one within the tile': ('tile * 128 + wt * 32 + lane;', 'tile * 128 + ((wt * 32 + lane + 1) & 127);'),
+}
+
+# paste_front.cu: every mutation keeps all memory accesses in bounds (checked against the file's shapes next to each
+# entry) and none is equivalent at every scale the file runs.
+PASTE_FRONT = {
+    # a coordinate clipped at the lower border keeps its gradient (grid_sample's border padding gives it none)
+    'lower clip keeps its gradient': ('if (ix <= 0.f) { ix = 0.f; mul = 0.f; }', 'if (ix <= 0.f) { ix = 0.f; }'),
+    # the backward differentiates the front image without normalize_images' factor 2
+    'backward ignores normalize_images': ('if (a.normalize) { f00 *= 2.f; f10 *= 2.f; f01 *= 2.f; f11 *= 2.f; }',
+                                          'if (a.normalize) { }'),
+    # eroded weights looked up at size min(R, Rf): indices stay below Rf; differs from the kernel only when R < Rf
+    'eroded lookup at size min(R, Rf)': ('Tap tr = ortho_tap(vy, a.half_bw, a.inv_bw, a.Rf), tc = ortho_tap(vx, a.half_bw, a.inv_bw, a.Rf);',
+                                         'Tap tr = ortho_tap(vy, a.half_bw, a.inv_bw, min(a.R, a.Rf)), tc = ortho_tap(vx, a.half_bw, a.inv_bw, min(a.R, a.Rf));'),
+    # output row 0 is up-sampled from the row of output 1 (the halo row clamp starts at 1; every S here is >= 3).  At
+    # scale <= 1/4 both rows clamp to source row 0, so only same_res, down and tiny_2x3 can see it
+    'first image row sampled from row 1': ('min(max(ty0 + (int)threadIdx.x - 1, 0), a.S - 1)', 'min(max(ty0 + (int)threadIdx.x - 1, 1), a.S - 1)'),
+    # the backward's up-sampling weights of taps (0, 1) and (1, 0) swapped
+    'backward weights w01 / w10 swapped': ('w01 = by.l0 * bx.l1, w10 = by.l1 * bx.l0', 'w01 = by.l1 * bx.l0, w10 = by.l0 * bx.l1'),
+    # the nearest source row rounded half up (its min(.., R - 1) keeps it in bounds); equal to the kernel at scales 1/4,
+    # 1/8 and 1, different at 0.096 and 1.5
+    'nearest row rounded half up': ('floorf((float)oy * a.scale)', 'floorf(((float)oy + 0.5f) * a.scale)'),
+}
+
+# render_backward.cu: every mutation changes a value, never an index or a bound that guards a memory access (the tap
+# mutation narrows the bound, so it only drops taps).
+# The depth gate `depth_raw >= lo_b` is not mutated: a ray's unclamped depth is a weighted mean of its interval midpoints,
+# which lie strictly inside [min depth, max depth] of the batch, so no case can put it on the bound and `>` equals `>=`.
+RENDER_BACKWARD = {
+    'colour factor 1.002 -> 1': ('(g.force_sigmoid ? 1.f : 1.002f)', '(g.force_sigmoid ? 1.f : 1.f)'),
+    'hidden softplus derivative threshold 20 -> 5': ('(pre > 20.f ? 1.f : sigmoid_t(pre))', '(pre > 5.f ? 1.f : sigmoid_t(pre))'),
+    'interval softplus derivative linear branch 1 -> 0': ('smid > 20.f ? 1.f : sigmoid_t(smid)', 'smid > 20.f ? 0.f : sigmoid_t(smid)'),
+    'white background term without g_xyz': ('2.f * back * (grgb_sum + gx_sum)', '2.f * back * (grgb_sum)'),
+    'suffix term not divided by 1 - alpha': ('Tr[i] * P - suffix / fc[i];', 'Tr[i] * P - suffix;'),
+    'tap bound xi < W - 1': ('const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H);\n        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);\n        out[k]',
+                             'const bool ok = (xi >= 0) && (xi < g.W - 1) && (yi >= 0) && (yi < g.H);\n        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);\n        out[k]'),
+    'd_w1 scaled by the bias gain': ('acc[i][j] * g.w1_gain);', 'acc[i][j] * g.b1_gain);'),
+    'd_b2 scaled by the weight gain': ('atomicAdd(a.d_b2 + tid, acc * g.b2_gain);', 'atomicAdd(a.d_b2 + tid, acc * g.w2_gain);'),
+    'omega without its 1/2': ('om = 0.5f * (wl + wr);', 'om = (wl + wr);'),
+}
+
+# modconv.cu: every mutation keeps all memory accesses in bounds.
+MODCONV = {
+    'demod epsilon dropped': ('block_reduce(ss, false, red) + 1e-8f', 'block_reduce(ss, false, red)'),
+    'style applied per output channel': ('s = srow[ci];', 's = srow[co % a.Cin];'),
+    'sub-pixel phases 1 and 2 swapped': ('    t.ntaps = s;\n',
+                                         '    t.ntaps = s;\n    if (t.nphase == 4) { const int b1 = t.base[1]; t.base[1] = t.base[2]; t.base[2] = b1; }\n'),
+    'last partial channel chunk skipped': ('const int ksteps = min(KCE, a.Cin - q * KCE) * ES / 32;',
+                                           'const int ksteps = a.Cin - q * KCE < KCE ? 0 : KCE * ES / 32;'),
+    'gain applied after the clamp': ('        v *= a.gain;\n        if (a.clamp >= 0.f) v = (v > -a.clamp && v < a.clamp) ? v : (v >= 0.f ? a.clamp : -a.clamp);\n',
+                                     '        if (a.clamp >= 0.f) v = (v > -a.clamp && v < a.clamp) ? v : (v >= 0.f ? a.clamp : -a.clamp);\n        v *= a.gain;\n'),
+    'noise indexed per channel': ('(long long)oy * a.snh', '(long long)(co % a.H) * a.snh'),
+}
+
+# target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
+TARGETS = {
+    'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
+    'paste_front': ('paste_front.cu', 'tests/test_paste_paths_gpu.py', PASTE_FRONT),
+    'render_backward': ('render_backward.cu', 'tests/test_render_backward_paths_gpu.py', RENDER_BACKWARD),
+    'modconv': ('modconv.cu', 'tests/test_modconv_gpu.py', MODCONV),
+}
+
+
+def build_mutant(nvcc, d, target, name):
+    """Compile the mutated source into d and link it with the tree's other objects; returns the library's path."""
+    src_name, _, mutations = TARGETS[target]
+    src = os.path.join(_build.CSRC, src_name)
+    text = open(src).read()
+    old, new = mutations[name]
+    assert text.count(old) == 1, f'{target}: {name}'
+    os.makedirs(d)
+    cu, obj, lib = os.path.join(d, src_name), os.path.join(d, src_name[:-3] + '.o'), os.path.join(d, 'libp3d.so')
+    open(cu, 'w').write(text.replace(old, new))
+    objs = [obj if s == src else _build.object_path(s) for s in _build.sources()]
+    # -I csrc: the copy finds csrc's headers, and its "../../include/..." resolves from csrc to the repository's include/
+    for cmd in (_build.compile_cmd(nvcc, cu, obj, ['-I', _build.CSRC]), _build.link_cmd(nvcc, lib, objs)):
+        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+        if r.returncode:
+            raise RuntimeError(f'{target}: {name}: nvcc failed\n{r.stdout}')
+    return lib
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('targets', nargs='+', choices=sorted(TARGETS), metavar='TARGET')
+    ap.add_argument('--files', nargs='+')
+    ap.add_argument('--json')
+    ap.add_argument('--build-only', action='store_true')
+    args = ap.parse_args()
+    import __graft_entry__ as g
+    g.build()
+    nvcc = _build.find_nvcc()
+    mutants = [(t, name) for t in dict.fromkeys(args.targets) for name in TARGETS[t][2]]
+    results = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        with ThreadPoolExecutor(max_workers=max(1, min(len(mutants), os.cpu_count() or 1))) as ex:
+            libs = list(ex.map(lambda i: build_mutant(nvcc, os.path.join(tmp, f'm{i}'), *mutants[i]), range(len(mutants))))
+        if args.build_only:
+            print(f'built {len(libs)} mutants', flush=True)
+            return
+        for (target, name), lib in zip(mutants, libs):
+            files = args.files or [TARGETS[target][1]]
+            r = subprocess.run([sys.executable, '-m', 'pytest', '-q', '-x', '-m', 'gpu', '-p', 'no:cacheprovider'] +
+                               [os.path.join(ROOT, f) for f in files],
+                               cwd=ROOT, env=dict(os.environ, P3D_LIBP3D=lib), stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
+                               text=True)
+            failed = [ln for ln in r.stdout.splitlines() if ln.startswith('FAILED') or ln.startswith('ERROR')]
+            res = results.setdefault(target, {})[name] = {'killed': r.returncode != 0, 'failures': failed,
+                                                          'summary': r.stdout.strip().splitlines()[-1]}
+            print(f'{target}: {name:50s} {"killed" if r.returncode else "SURVIVED"}: {res["summary"][:120]}', flush=True)
+            for ln in failed:
+                print(f'    {ln[:160]}', flush=True)
+    if args.json:
+        json.dump(results, open(args.json, 'w'), indent=1)
+    sys.exit(0 if args.files or all(v['killed'] for t in results.values() for v in t.values()) else 1)
+
+
+if __name__ == '__main__':
+    main()
