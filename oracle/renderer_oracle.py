@@ -290,15 +290,22 @@ def apply_masks(sigma: Tensor, xyz: Tensor, box_warp: float, triplane_crop, cull
 # compositing
 # --------------------------------------------------------------------------
 def march(colors: Tensor, sigma: Tensor, depths: Tensor, white_back: bool,
-          depth_lo: Optional[Tensor] = None, depth_hi: Optional[Tensor] = None
+          depth_lo: Optional[Tensor] = None, depth_hi: Optional[Tensor] = None,
+          alpha_eps: Optional[Tensor] = None, left_colours: bool = False
           ) -> Tuple[Tensor, Tensor, Tensor]:
     """MipRayMarcher2.run_forward, ray_marcher.py:25-57.
-    colors (N,M,S,Cc), sigma (N,M,S,1), depths (N,M,S,1), depth sorted along S."""
+    colors (N,M,S,Cc), sigma (N,M,S,1), depths (N,M,S,1), depth sorted along S.
+
+    For tests only: `alpha_eps` (N,M,S-1,1) is added to every interval's alpha (a perturbation to differentiate against;
+    adding zeros changes nothing), and `left_colours` weights each interval by its first sample's colour instead of the
+    mean of its two (a deliberately wrong variant for negative controls)."""
     delta = depths[:, :, 1:] - depths[:, :, :-1]
-    c_mid = (colors[:, :, :-1] + colors[:, :, 1:]) / 2
+    c_mid = colors[:, :, :-1] if left_colours else (colors[:, :, :-1] + colors[:, :, 1:]) / 2
     s_mid = F.softplus((sigma[:, :, :-1] + sigma[:, :, 1:]) / 2 - 1)
     d_mid = (depths[:, :, :-1] + depths[:, :, 1:]) / 2
     alpha = 1 - torch.exp(-(s_mid * delta))
+    if alpha_eps is not None:
+        alpha = alpha + alpha_eps
     trans = torch.cumprod(torch.cat([torch.ones_like(alpha[:, :, :1]), 1 - alpha + 1e-10], -2), -2)[:, :, :-1]
     w = alpha * trans
     rgb = (w * c_mid).sum(-2)
@@ -313,16 +320,22 @@ def march(colors: Tensor, sigma: Tensor, depths: Tensor, white_back: bool,
     return rgb * 2 - 1, depth, w
 
 
-def importance_depths(z: Tensor, w: Tensor, u: Tensor, eps: float = 1e-5) -> Tensor:
+def importance_depths(z: Tensor, w: Tensor, u: Tensor, eps: float = 1e-5, floor: float = 0.01,
+                      cdf_eps: Optional[Tensor] = None) -> Tensor:
     """sample_importance + sample_pdf, renderer.py:328-387.
-    z (R,S) coarse depths, w (R,S-1) coarse weights, u (R,Sf) uniforms -> (R,Sf)."""
+    z (R,S) coarse depths, w (R,S-1) coarse weights, u (R,Sf) uniforms -> (R,Sf).
+
+    For tests only: `floor` is the pdf floor the reference adds (0.01), and `cdf_eps` (R,S-2) is added to the cdf (a
+    perturbation to differentiate against; adding zeros changes nothing)."""
     R, S = z.shape
     wp = F.max_pool1d(w[:, None, :], 2, 1, padding=1)          # R,1,S
-    wp = F.avg_pool1d(wp, 2, 1)[:, 0] + 0.01                   # R,S-1
+    wp = F.avg_pool1d(wp, 2, 1)[:, 0] + floor                  # R,S-1
     bins = 0.5 * (z[:, :-1] + z[:, 1:])                        # R,S-1
     wi = wp[:, 1:-1] + eps                                     # R,S-3
     pdf = wi / wi.sum(-1, keepdim=True)
     cdf = torch.cat([torch.zeros(R, 1, dtype=pdf.dtype, device=pdf.device), torch.cumsum(pdf, -1)], -1)   # R,S-2
+    if cdf_eps is not None:
+        cdf = cdf + cdf_eps
     nb = wi.shape[1]
     inds = torch.searchsorted(cdf, u.contiguous(), right=True)
     below = (inds - 1).clamp_min(0)

@@ -345,8 +345,10 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         // A single warp has no other warp to hide its latencies behind, so both phases are written for instruction-level
         // parallelism: the 32-lane chunks of a ray are processed as independent chains (per-chunk scans, carries
         // combined afterwards), every search is a fixed-trip branchless bisection, and the importance depths are put in
-        // order by sorting the UNIFORMS with a bitonic network (the inverse CDF is monotone, so mapping sorted uniforms
-        // yields sorted depths - this replaces the O(S^2) rank sort).
+        // order by sorting them with a bitonic network after the inverse CDF, as the reference sorts them before the merge.
+        // Sorting the uniforms instead would only order the depths when the inverse CDF ascends: descending coarse depths
+        // ('auto' limits when no ray of the call hits the box, numeric ray_start > ray_end) give negative weights and a
+        // cdf that is neither, and the merge by rank needs ascending fine depths.
         // ---- importance sampling of ray rl of group n (renderer.py:328-387)
         auto importance_ray = [&](int n, int rl) {
             GroupState& st = sm.st[n & 3];
@@ -411,7 +413,32 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 csum = __shfl_sync(0xffffffffu, incl, 31);
             }
             if (lane == 0) i_cdf[0] = 0.f;
-            // bitonic sort of the 128 (padded) uniforms, element e = c*32 + lane, ascending
+            __syncwarp();                         // i_cdf is complete
+#pragma unroll
+            for (int c = 0; c < NC; ++c) {        // inverse CDF (searchsorted right=True), lerp between bin midpoints
+                const int f = c * 32 + lane;
+                if (f >= Sf) continue;
+                float val = INFINITY;
+                if (ray < a.R) {
+                    const float u = us[c];
+                    int lo = 0;                   // number of cdf[0..nb] entries <= u
+#pragma unroll
+                    for (int step = 64; step >= 1; step >>= 1) {
+                        const int p = lo + step;
+                        const float x = i_cdf[min(p, nb + 1) - 1];
+                        if (p <= nb + 1 && x <= u) lo = p;
+                    }
+                    const int below = max(lo - 1, 0), above = min(lo, nb);
+                    const float c0 = i_cdf[below], c1 = i_cdf[above];
+                    const float b0 = __fmul_rn(0.5f, __fadd_rn(tc[below], tc[below + 1]));
+                    const float b1 = __fmul_rn(0.5f, __fadd_rn(tc[above], tc[above + 1]));
+                    float den = __fsub_rn(c1, c0);
+                    if (den < 1e-5f) den = 1.f;
+                    val = __fadd_rn(b0, __fmul_rn(__fdiv_rn(__fsub_rn(u, c0), den), __fsub_rn(b1, b0)));
+                }
+                us[c] = val;
+            }
+            // bitonic sort of the 128 (padded) depths, element e = c*32 + lane, ascending
 #pragma unroll
             for (int k = 2; k <= 128; k <<= 1) {
 #pragma unroll
@@ -437,30 +464,10 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                     }
                 }
             }
-            __syncwarp();                         // i_cdf is complete
 #pragma unroll
-            for (int c = 0; c < NC; ++c) {        // inverse CDF (searchsorted right=True), lerp between bin midpoints
+            for (int c = 0; c < NC; ++c) {
                 const int f = c * 32 + lane;
-                if (f >= Sf) continue;
-                float val = INFINITY;
-                if (ray < a.R) {
-                    const float u = us[c];
-                    int lo = 0;                   // number of cdf[0..nb] entries <= u
-#pragma unroll
-                    for (int step = 64; step >= 1; step >>= 1) {
-                        const int p = lo + step;
-                        const float x = i_cdf[min(p, nb + 1) - 1];
-                        if (p <= nb + 1 && x <= u) lo = p;
-                    }
-                    const int below = max(lo - 1, 0), above = min(lo, nb);
-                    const float c0 = i_cdf[below], c1 = i_cdf[above];
-                    const float b0 = __fmul_rn(0.5f, __fadd_rn(tc[below], tc[below + 1]));
-                    const float b1 = __fmul_rn(0.5f, __fadd_rn(tc[above], tc[above + 1]));
-                    float den = __fsub_rn(c1, c0);
-                    if (den < 1e-5f) den = 1.f;
-                    val = __fadd_rn(b0, __fmul_rn(__fdiv_rn(__fsub_rn(u, c0), den), __fsub_rn(b1, b0)));
-                }
-                st.t_f[rl * Sf + f] = val;
+                if (f < Sf) st.t_f[rl * Sf + f] = us[c];
             }
             __syncwarp();
         };

@@ -4,7 +4,7 @@ fails it, as it must.  The tree is not modified.
 
     python tests/run_mutations.py TARGET [TARGET ...] [--files F ...] [--json out.json] [--build-only]
 
-TARGET is one of decode_tc, paste_front, render_backward, modconv.  --files runs other GPU files against the same mutants
+TARGET is one of decode_tc, paste_front, render_backward, modconv, render_fused.  --files runs other GPU files against the same mutants
 instead (to see which of them the rest of the suite catches); the exit code then only reports that the run completed.
 --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
 """
@@ -88,12 +88,28 @@ MODCONV = {
     'noise indexed per channel': ('(long long)oy * a.snh', '(long long)(co % a.H) * a.snh'),
 }
 
+# render_fused_ws3.cu: value mutations only - no stage index, parity, arrival count or transaction size changes, and every
+# access stays in bounds (trow ^ 1 stays inside the 128-row tile), so none can hang.
+RENDER_FUSED = {
+    'colour factor 1.002 -> 1': ('const float ca = g.force_sigmoid ? om : 1.002f * om', 'const float ca = g.force_sigmoid ? om : om'),
+    'colour offset also under force_sigmoid': ('cb = g.force_sigmoid ? 0.f : -0.001f * om', 'cb = -0.001f * om'),
+    'neighbouring sample\'s colour': ('part += fmaf(buf[col_idx(trow, lane)], ca, cb);', 'part += fmaf(buf[col_idx(trow ^ 1, lane)], ca, cb);'),
+    'omega = w_i': ('sl.om[rl * L + i] = __fmul_rn(__fadd_rn(wl, wi), 0.5f);', 'sl.om[rl * L + i] = wi;'),
+    'pdf floor 0.005': ('fmaxf(w[1], w[2])), 0.5f), 0.01f), 1e-5f);', 'fmaxf(w[1], w[2])), 0.5f), 0.005f), 1e-5f);'),
+    'crop flag of the coarse pass in the epilogue': ('if (st.crop[td.pass][srow]) sg = -1e3f;', 'if (st.crop[0][srow]) sg = -1e3f;'),
+    'cull threshold without 1 +': ('(float)(1.0 + log(expm1(-log1p(-thr))))', '(float)(log(expm1(-log1p(-thr))))'),
+    'depth from the merged depth, not the midpoint': ('acc_d = fmaf(wi, tm[c], acc_d);', 'acc_d = fmaf(wi, m_t[i], acc_d);'),
+    'single pass never set': ('a.single_pass = p->mlp_mode == P3D_MLP_TC_BF16;', 'a.single_pass = 0;'),
+    'fine depths stored in descending order': ('if (f < Sf) st.t_f[rl * Sf + f] = us[c];', 'if (f < Sf) st.t_f[rl * Sf + Sf - 1 - f] = us[c];'),
+}
+
 # target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
 TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
     'paste_front': ('paste_front.cu', 'tests/test_paste_paths_gpu.py', PASTE_FRONT),
     'render_backward': ('render_backward.cu', 'tests/test_render_backward_paths_gpu.py', RENDER_BACKWARD),
     'modconv': ('modconv.cu', 'tests/test_modconv_gpu.py', MODCONV),
+    'render_fused': ('render_fused_ws3.cu', 'tests/test_render_fused_paths_gpu.py', RENDER_FUSED),
 }
 
 
@@ -141,10 +157,11 @@ def main():
                                cwd=ROOT, env=dict(os.environ, P3D_LIBP3D=lib), stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                                text=True)
             failed = [ln for ln in r.stdout.splitlines() if ln.startswith('FAILED') or ln.startswith('ERROR')]
-            res = results.setdefault(target, {})[name] = {'killed': r.returncode != 0, 'failures': failed,
+            errors = [ln for ln in r.stdout.splitlines() if ln.startswith('E ')][:8]
+            res = results.setdefault(target, {})[name] = {'killed': r.returncode != 0, 'failures': failed, 'errors': errors,
                                                           'summary': r.stdout.strip().splitlines()[-1]}
             print(f'{target}: {name:50s} {"killed" if r.returncode else "SURVIVED"}: {res["summary"][:120]}', flush=True)
-            for ln in failed:
+            for ln in failed + errors[:2]:
                 print(f'    {ln[:160]}', flush=True)
     if args.json:
         json.dump(results, open(args.json, 'w'), indent=1)

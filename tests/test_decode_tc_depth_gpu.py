@@ -257,6 +257,54 @@ def _single_pass_bars(p64, d64, x64):
     return 1.002 * LN2 / 4 * (dh @ w2[1:].t()) + BAR, LN2 * (dh @ w2[:1].t()) + BAR
 
 
+U32 = 2.0 ** -24                  # unit roundoff of fp32
+MUFU_EX2, MUFU_LG2, MUFU_RCP = 2.0 ** -22, 2.0 ** -22, 2.0 ** -23
+
+
+def _three_pass_bars(p64, d64, x64, force_sigmoid=False, use_triplane=True):
+    """Per-point bars (rgb (N,K,32), sigma (N,K,1)) for mlp_mode 1 (3-pass split bf16), at exact fp32 point coordinates.
+    The error of the coordinates themselves (ray_point, the grid transform) is the caller's: it moves the point.
+
+    In the base-2 form of `_single_pass_bars`, with u = 2^-8 (bf16) and v = 2^-24 (fp32):
+      gather    A1 = sum over 3 planes x 4 taps of w t (one fp32 fma chain, weights from three roundings):
+                |dA1_c| <= 16 v sum |w| |t_c|
+      split     an operand x = hi + lo + r, |lo| <= u |x|, |r| <= u |lo| <= u^2 |x|; the kernel forms hi hi + hi lo + lo hi
+                and drops lo lo, r_a b and a r_b: e3 = 3 u^2 (+ O(u^3)) of |a| |b| per product
+      accumulation  fp32 in the wgmma, 3K products: <= 3K v of sum |a| |b| (K = 32 for layer 1, 64 for layer 2)
+      staging   W1' and the biases carry <= 3 roundings (v each) of their own magnitude, W2' <= 2
+      layer 1   |dx'_j| <= (e3 + 100 v) sum_c |A1_c| |W1'_jc| + sum_c |dA1_c| |W1'_jc| + 4 v (|b1'_j| + |x'_j|)
+      hidden    h' = max(x', 0) + lg2(1 + ex2(-|x'|)), slope <= 1: |dh'_j| <= |dx'_j| + (ex2 + 2 v) / ln 2 + lg2 + v |h'_j|
+                with the MUFU bounds of the PTX ISA (ex2.approx.f32: relative error 2^-22, lg2.approx.f32: absolute 2^-22,
+                rcp.approx.f32: 1 ulp = relative 2^-23)
+      layer 2   |dl_k| <= (e3 + 200 v) sum_j |h'_j| |W2'_kj| + sum_j |dh'_j| |W2'_kj| + 3 v (|b2'_k| + |l_k|)
+      sigma     dl_0 (the sigma row is the plain sum)
+      colour    s = rcp(1 + ex2(l')): |ds| <= s (1 - s) (ln 2 |dl| + ex2) + s (v + rcp), times 1.002 for the colour map
+    """
+    C_ = d64['w1'].shape[1]
+    lr = d64.get('lr_mul', 1.0)
+    g1, g2 = lr / math.sqrt(C_), lr / math.sqrt(d64['w2'].shape[1])
+    a = orc.sample_planes(p64, x64, BW, use_triplane).sum(1)                  # (N,K,C)
+    # sum over planes and taps of |w| |t|: the bilinear gather of |planes| (weights are non-negative)
+    a_abs = orc.sample_planes(p64.abs(), x64, BW, use_triplane).sum(1)
+    da = 16 * U32 * a_abs
+    e3 = 3 * U_BF16 ** 2
+    w1p = d64['w1'] * (g1 * LOG2E / 3)
+    b1p = d64['b1'] * (lr * LOG2E)
+    x2 = a @ w1p.t() + b1p
+    dx = (e3 + 100 * U32) * (a.abs() @ w1p.abs().t()) + da @ w1p.abs().t() + 4 * U32 * (b1p.abs() + x2.abs())
+    h2 = F.softplus(x2 * LN2) * LOG2E
+    dh = dx + (MUFU_EX2 + 2 * U32) / LN2 + MUFU_LG2 + U32 * h2.abs()
+    w2p = d64['w2'] * g2
+    w2p = torch.cat([w2p[:1] * LN2, -w2p[1:]], 0)                             # sigma row, then the colour rows
+    b2p = d64['b2'] * lr
+    b2p = torch.cat([b2p[:1], -b2p[1:] * LOG2E], 0)
+    lg = h2 @ w2p.t() + b2p
+    dl = (e3 + 200 * U32) * (h2.abs() @ w2p.abs().t()) + dh @ w2p.abs().t() + 3 * U32 * (b2p.abs() + lg.abs())
+    s = torch.sigmoid(-lg[..., 1:] * LN2)
+    ds = s * (1 - s) * (LN2 * dl[..., 1:] + MUFU_EX2) + s * (U32 + MUFU_RCP)
+    return (ds if force_sigmoid else 1.002 * ds), dl[..., :1]
+
+
 class Worst:
     """Worst |got - want| and worst |got - want| / bar of one output over pieces; NaN counts as infinitely wrong."""
 

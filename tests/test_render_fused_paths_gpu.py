@@ -1,0 +1,708 @@
+"""GPU: the fused renderer (k_render_ws3, csrc/render_fused_ws3.cu) at the bench size, against the fp64 oracle with a bar
+per ray and output component.
+
+k_render_ws3 is the default kernel of ImportanceRenderer, smoke() and bench.py.  The other GPU files compare it with one
+flat bar; here every call goes through the C ABI (p3d_render_forward, mlp_mode 1 or 2) with injected uniforms, NaN-filled
+outputs and a NaN-filled workspace (its rgb_c / rgb_f buffers are the kernel's colour areas, so a colour tile read before
+its bulk store lands, or from the wrong slice, turns into NaN).  Every call is made twice: exactly one launch in profile
+slot 5 each, bit-identical results, no NaN anywhere (checked after the values, which a kernel reading memory it never
+wrote can get wrong while still repeating itself).
+
+Cases (each asserts the property it exists for):
+  headline      2 views, 128^2 rays, 96+96, 512^2 planes: 62-63 groups per CTA on 132 SMs
+  bench8        bench.py's batch, 8 views: 248-249 groups per CTA (the colour areas and col_full parities wrap many times);
+                bars on every BENCH_STRIDE-th ray, NaN and repeat checks on every ray
+  train48       4 views, 64^2, 48+48, 256^2: bench.py's training context
+  eval_flags96  crop 0.1, cull 0.5, force_sigmoid, sigma bias centred on the cull: 20-50 % of the uncropped samples culled
+  binarize48    binarize 0.5 + crop
+  auto_eg3d     'auto' limits, EG3D plane order, black background, lr_mul 0.5, cameras at distance 2: some rays miss the
+                box and take the batch-bound fallback
+  ortho, disparity, shared_planes
+  bf16_cl       bf16 (N,96,H,W) channels_last planes consumed zero-copy, against the oracle on the bf16-rounded planes
+  n_my_1/2/3    fewer groups than SMs, then exactly 2 and 3 groups on the deepest CTA
+  all_miss48/96 'auto' limits, every ray of the call misses the box: bounds[4] == 0 and the coarse depths descend (t0 = -1,
+                t1 = -2); sigma bias -4 keeps every ray's importance pdf positive, so every ray is compared
+  all_miss_negpdf48  all_miss48 without that bias: every ray's pdf is non-positive somewhere (see below)
+  descending96  numeric ray_start 1.5 > ray_end 0.5: descending coarse depths
+  single_pass   mlp_mode 2 against its own bars, and >= 10x mode 1's error
+  saturated48, dense48  the negative controls' cases (CONTROL_CASES)
+The descending cases are also checked against the fp32 SIMT kernel (mlp_mode 0) at its 1e-4 bar.
+
+Reference: oracle/renderer_oracle.py in float64 on the device, a view and CHUNK rays at a time (its depth clamp is applied
+with the batch's bounds afterwards).  test_gpu_fp64_oracle_equals_cpu_oracle pins that run to the CPU fp32 oracle on the
+config1 and mid_eval96 fixtures.
+
+Bars.  The kernel's error is bounded per sample and propagated to first order through the oracle:
+  * per sample: the decoder's sigma and colour bars (test_decode_tc_depth_gpu._three_pass_bars for mode 1,
+    _single_pass_bars for mode 2; test_three_pass_bars_hold_on_the_decode checks the first on p3d_decode_points at the
+    oracle's own sample positions), plus the point's fp32 rounding (ray_point, the grid transform: 4 v (|o| + |t d| + box)
+    per coordinate, v = 2^-24) times the one-sided finite-difference slopes of sigma and colour;
+  * per depth: coarse 16 v (|t| + |t0| + |t1|); fine 8 v (|t| + |t1 - t0|) for the lerp, and (2 S + 40) v on every cdf
+    entry (fp32 weights, their sum, the division and the scans);
+  * per interval alpha = 1 - ex2.approx(-log2(e) softplus(smid) dt): 2^-22 (1 - alpha) + v alpha + (1 - alpha) (dt (4
+    2^-22 softplus + 2 2^-22 + sigmoid(smid) v (|s_a| + |s_b| + 2)) + 6 v softplus dt), in both marches.
+  The oracle's render is restated as a graph of these perturbations (zero-valued leaves: `_render_graph`): the coarse
+  sigma / colour / depth perturbations move the coarse weights, the importance depths (kept differentiable) and, through
+  each fine sample's slope along its ray, the fine sigma and colour.  For each output component o_k of a ray (32 rgb,
+  depth, wsum, 3 xyz), one vector-Jacobian product per component over a chunk of rays (rays are independent) gives
+      bar_k = 2 (sum over leaves |do_k / d leaf| beta_leaf) + floor_k
+  floor_k covers the roundings of the sums that form the output ((L + 8) v relative on each weight and on every partial
+  sum; L = S + Sf).  The factor 2 covers second-order terms: every leaf's relative size is <= ~1e-4, so products of two
+  perturbations are below 1e-4 of the first-order sum.
+  The merge of two samples whose depths are within rounding of each other may order them either way; the outputs change by
+  less than the slopes times the depth bar, since both samples sit at the same point.
+Masks: a cull, binarize or crop decision is a jump.  A ray is excluded when one of its samples' fp64 sigma lies within its
+sigma bar (plus the rounding of the host's sigma_cull) of the threshold, or its |x| / |z| within the position bar of the
+crop bound; the excluded rays are counted and bounded (EXCLUDE_SHARE).  Rays whose W is 0 in either run (every sample
+masked) compare their depth with the batch's largest depth.
+
+Negative controls: the oracle with the colour map s - 0.001 instead of 1.002 s - 0.001 (on saturated48, whose colours sit
+near 1, where the gain matters most and the decoder's colour error, scaled by s (1 - s), least), with the importance pdf
+floor 0.005 and with omega = w_i instead of (w_{i-1} + w_i) / 2 (both on dense48, whose weight sits on a few intervals).
+Each must miss the kernel by >= 20x the bar somewhere.
+
+Descending coarse depths make negative weights.  Where the importance pdf they give is non-positive, the cdf is not
+monotone and the reference's own fine depths depend on the probe order of its searchsorted; such rays are counted and not
+compared.  Only all_miss_negpdf48 has any (all of them; it keeps the determinism, NaN and limit checks); every other case
+asserts that it has none.
+
+Run with -s for the worst error / bar of every case and output, the excluded rays, runtime and peak device memory.
+"""
+import ctypes as C
+import functools
+import time
+
+import pytest
+import torch
+
+from oracle import renderer_oracle as orc
+from tests.helpers import profiled
+from tests.test_decode_tc_depth_gpu import U32, _decode_points, _single_pass_bars, _three_pass_bars
+from tests.test_render_backward_paths_gpu import _cull_sigma
+from tests.test_render_gpu import make_decoder
+
+pytestmark = pytest.mark.gpu
+DEV = 'cuda:0'
+PROF_FUSED = 5                    # profile slot of k_render_ws3 (csrc/p3d_common.cuh)
+BW = orc.DEFAULT_OPTS['box_warp']
+CHUNK = 1024                      # rays per oracle call
+BENCH_STRIDE = 16
+SIMT_BAR = 1e-4                   # the SIMT kernel against the oracle (tests/test_render_gpu.py)
+EXCLUDE_SHARE = {1: 0.01, 2: 0.05}
+# The mask cases exclude far more rays: a fine sample's band is its sigma slope along the ray times the bound of how far its
+# depth may move, which is loose (see DESIGN.md section 2).  Measured on an H100: eval_flags96 92 %, binarize48 25 %.
+EXCLUDE_SHARE_MASKS = {'eval_flags96': 0.95, 'binarize48': 0.35}
+PIN = 2e-6                        # fp64 device oracle vs the CPU fp32 one: the fp32 run's rounding (measured 7.6e-7)
+FREE_BYTES = 12 << 30             # the 512^2 cases: measured peak 8.1 GB (bench8), with margin
+MUFU = 2.0 ** -22
+OUT_NAMES = ['rgb'] * 32 + ['depth', 'wsum', 'xyz', 'xyz', 'xyz']
+OUTPUTS = ('rgb', 'depth', 'wsum', 'xyz')
+AUTO = dict(ray_start='auto', ray_end='auto')
+
+CASES = {
+    'headline': dict(N=2, R=128, S=96, P=512, per_cta=(62, 63)),
+    'bench8': dict(N=8, R=128, S=96, P=512, per_cta=(248, 249), stride=BENCH_STRIDE),
+    'train48': dict(N=4, R=64, S=48, P=256),
+    'eval_flags96': dict(N=1, R=64, S=96, P=256, flags=dict(triplane_crop=0.1, cull_clouds=0.5), force_sigmoid=True,
+                         centre_cull=0.5, quantile=0.35),
+    'binarize48': dict(N=2, R=32, S=48, P=64, flags=dict(triplane_crop=0.1, binarize_clouds=0.5), centre_cull=0.5),
+    'auto_eg3d': dict(N=2, R=32, S=48, P=64, opts=dict(AUTO, white_back=False), eg3d=True, lr_mul=0.5, dist=2.0),
+    'ortho': dict(N=1, R=64, S=96, P=128, rays='ortho'),
+    'disparity': dict(N=2, R=32, S=48, P=64, opts=dict(disparity_space_sampling=True)),
+    'shared_planes': dict(N=3, R=32, S=96, P=64, shared=True),
+    'bf16_cl': dict(N=2, R=64, S=96, P=128, bf16=True),
+    'n_my_1': dict(N=1, R=8, S=96, P=64, groups=lambda sms: 16),
+    'n_my_2': dict(N=1, R=64, S=96, P=64, groups=lambda sms: sms + 5),
+    'n_my_3': dict(N=1, R=64, S=48, P=64, groups=lambda sms: 2 * sms + 7),
+    'all_miss48': dict(N=2, R=32, S=48, P=64, rays='miss', opts=dict(AUTO), sigma_bias=-4.0),
+    'all_miss96': dict(N=1, R=32, S=96, P=64, rays='miss', opts=dict(AUTO), sigma_bias=-4.0),
+    'all_miss_negpdf48': dict(N=2, R=32, S=48, P=64, rays='miss', opts=dict(AUTO), seed_as='all_miss48'),
+    'descending96': dict(N=2, R=32, S=96, P=64, opts=dict(ray_start=1.5, ray_end=0.5)),
+    'single_pass': dict(N=1, R=64, S=96, P=128, mode=2),
+    # negative-control cases: colours saturated near 1 (the colour map's gain is all that separates s - 0.001 from the
+    # kernel, and the decoder's colour error is scaled by s (1 - s)), and a dense case (weight on a few intervals, so
+    # omega's neighbour and the pdf floor move the outputs far more than the bars)
+    'saturated48': dict(N=1, R=32, S=48, P=64, colour_bias=8.0),
+    'dense48': dict(N=1, R=32, S=48, P=64, sigma_bias=8.0),
+}
+# input seed of a case: 1300 + its index here (cases added later go at the end, so no other case's inputs change)
+SEEDS = sorted(['headline', 'bench8', 'train48', 'eval_flags96', 'binarize48', 'auto_eg3d', 'ortho', 'disparity', 'shared_planes',
+                'bf16_cl', 'n_my_1', 'n_my_2', 'n_my_3', 'all_miss48', 'all_miss96', 'descending96', 'single_pass']) + ['saturated48', 'dense48']
+DESCENDING = ('all_miss48', 'all_miss96', 'all_miss_negpdf48', 'descending96')
+# the one case whose importance pdf is non-positive on every ray (see _chunk): checked for determinism, no NaN and its
+# limits, not against the oracle
+NEGATIVE_PDF = ('all_miss_negpdf48',)
+
+
+def n_sm():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _per_cta(n_groups, sms):
+    """render_fused_ws3.cu: grid = min(n_groups, n_sm), CTA b runs ceil((n_groups - b) / grid) groups."""
+    grid = min(n_groups, sms)
+    return [(n_groups - b + grid - 1) // grid for b in range(grid)]
+
+
+def _dec64(dec):
+    return {k: (v.to(DEV, torch.float64) if torch.is_tensor(v) else v) for k, v in dec.items()}
+
+
+# ------------------------------------------------------------------------------------------------- inputs
+def _rays(case, N, R):
+    from panic3d_b200 import cameras
+    from panic3d_b200.training.volumetric_rendering.ray_sampler import RaySampler
+    kind = case.get('rays', 'spin')
+    if kind == 'ortho':
+        ro, rd = zip(*(orc.rays_ortho(20.0, -135.0 + 40 * n, 1.0, BW, R) for n in range(N)))
+        f = lambda t: torch.cat(t).permute(0, 2, 3, 1).reshape(N, R * R, 3)
+        return f(ro).to(DEV).contiguous(), f(rd).to(DEV).contiguous()
+    if kind == 'miss':
+        # origins at x in [0.4, 0.6], beyond the box's half side 0.35, directions with no x component: every ray misses the
+        # box, yet the points at t in [-2, -1] ('auto' limits of a miss) project inside the (y, z) plane for many samples
+        g = torch.Generator().manual_seed(7)
+        a, b = torch.rand(N, R * R, generator=g), torch.rand(N, R * R, generator=g)
+        ro = torch.stack([0.4 + 0.2 * a, 0.4 * b - 0.2, torch.full_like(a, 1.0)], -1)
+        rd = torch.nn.functional.normalize(torch.stack([torch.zeros_like(a), 0.3 * (b - 0.5), torch.ones_like(a)], -1), dim=-1)
+        return ro.to(DEV).contiguous(), rd.to(DEV).contiguous()
+    spin = cameras.cam60[cameras.camsubs['spin12']]
+    lab = torch.stack([cameras.camera_params_to_matrix(elev=float(spin[i][0]), azim=float(spin[i][1]), dist=case.get('dist', 1.0),
+                                                       fov=30.0)['camera_label'] for i in range(N)]).to(DEV)
+    ro, rd = RaySampler()(lab[:, :16].view(-1, 4, 4), lab[:, 16:25].view(-1, 3, 3), R)
+    return ro.float().contiguous(), rd.float().contiguous()
+
+
+@functools.lru_cache(maxsize=None)
+def _inputs(name):
+    case = CASES[name]
+    N, R, S, P = (case[k] for k in ('N', 'R', 'S', 'P'))
+    seed = 1300 + SEEDS.index(case.get('seed_as', name))
+    g = torch.Generator().manual_seed(seed)
+    planes = torch.randn(1 if case.get('shared') else N, 3, 32, P, P, generator=g)
+    if case.get('shared'):
+        planes = planes.expand(N, -1, -1, -1, -1)
+    if case.get('bf16'):
+        planes = planes.bfloat16().float()
+    _, dec, *_ = orc.synth_inputs(seed, 1, 1, 2, 0, 2)
+    dec = dict(dec, lr_mul=case.get('lr_mul', 1.0), force_sigmoid=case.get('force_sigmoid', False), b2=dec['b2'].clone())
+    dec['b2'][0] += case.get('sigma_bias', 0.0)
+    dec['b2'][1:] += case.get('colour_bias', 0.0)
+    opts = dict(dict(orc.DEFAULT_OPTS, depth_resolution=S, depth_resolution_importance=S), **case.get('opts', {}))
+    ro, rd = _rays(case, N, R)
+    if case.get('groups'):
+        M = case['groups'](n_sm()) * (384 // S)
+        assert M <= R * R
+        ro, rd = ro[:, :M].contiguous(), rd[:, :M].contiguous()
+    M = ro.shape[1]
+    u_c = torch.rand(N, M, S, 1, generator=g)
+    u_f = torch.rand(N * M, S, generator=g)
+    if case.get('centre_cull'):                     # median coarse sigma on the cull threshold
+        d_c = orc.stratified_depths(u_c.to(DEV), opts['ray_start'], opts['ray_end'])
+        xyz = (ro[:, :, None] + d_c * rd[:, :, None]).reshape(N, -1, 3)[:, ::7]
+        _, sig = orc.run_model(planes.to(DEV, torch.float64), _dec64(dec), xyz, opts, not case.get('eg3d'))
+        dec['b2'][0] += _cull_sigma(case['centre_cull']) - sig.quantile(case.get('quantile', 0.5)).item()
+    return planes, dec, opts, ro, rd, u_c.to(DEV).contiguous(), u_f.to(DEV).contiguous()
+
+
+# ------------------------------------------------------------------------------------------------- the kernel, through the C ABI
+def _kernel(name, mode=None, checks_later=False):
+    """p3d_render_forward twice into NaN-filled outputs and workspace: one launch in slot 5 each, bit-identical, no NaN.
+    Returns (rgb, depth, wsum, xyz), the workspace bounds words; with checks_later, the checks of the two runs are left to
+    the caller (_repeats), which makes them after comparing the values."""
+    from panic3d_b200 import _lib
+    from panic3d_b200.training.volumetric_rendering.renderer import ImportanceRenderer
+    case = CASES[name]
+    planes, dec, opts, ro, rd, u_c, u_f = _inputs(name)
+    mode = case.get('mode', 1) if mode is None else mode
+    N, M = ro.shape[:2]
+    r = ImportanceRenderer(use_triplane=not case.get('eg3d'))
+    r.planes_bf16 = bool(case.get('bf16'))
+    r.mlp_mode = mode
+    decoder = make_decoder(dec, DEV)
+    with torch.no_grad(), torch.cuda.device(DEV):
+        if case.get('bf16'):               # a (N,96,H,W) channels_last backbone output, consumed zero-copy
+            n, p_, c, h, w = planes.shape
+            x = planes.to(DEV, torch.bfloat16).reshape(n, p_ * c, h, w).contiguous(memory_format=torch.channels_last)
+            cl = r._planes_cl(x.view(n, p_, c, h, w))
+            assert cl.data_ptr() == x.data_ptr(), 'bf16 channels_last planes were copied'
+        else:
+            cl = r._planes_cl(planes.to(DEV))
+        fl = case.get('flags', {})
+        p, wts = r._params(cl, N, M, opts, decoder, fl.get('triplane_crop'), fl.get('cull_clouds'), fl.get('binarize_clouds'))
+        assert p.mlp_mode == mode
+        p.defer_depth_clamp = 0
+        wt = [t.detach().float().contiguous() for t in wts]
+        L = _lib.lib()
+        nbytes = int(L.p3d_render_workspace_bytes(C.byref(p)))
+        runs = []
+        for _ in range(2):
+            ws = torch.full((nbytes,), 0xFF, dtype=torch.uint8, device=DEV)          # every float in it NaN
+            out = [torch.full(s, float('nan'), device=DEV) for s in ((N, M, 32), (N, M, 1), (N, M, 1), (N, M, 3))]
+            torch.cuda.synchronize()
+            _, prof = profiled(lambda: _lib.check(L.p3d_render_forward(
+                C.byref(p), cl.data_ptr(), *[t.data_ptr() for t in wt], ro.data_ptr(), rd.data_ptr(), u_c.data_ptr(),
+                u_f.data_ptr(), ws.data_ptr(), ws.numel(), *[o.data_ptr() for o in out], _lib.stream_ptr(DEV))))
+            torch.cuda.synchronize()
+            if mode != 0:
+                assert prof[PROF_FUSED] == 1, prof
+            runs.append((out, ws[:64].view(torch.int32).clone()))
+        if checks_later:
+            return runs[0][0], runs[0][1], runs[1][0]
+        _repeats(name, runs[0][0], runs[1][0])
+        return runs[0]
+
+
+def _repeats(name, first, second):
+    for key, a, b in zip(OUTPUTS, first, second):
+        assert not torch.isnan(a).any(), f'{name}: {key} has NaN (an element never written, or read before it landed)'
+        assert torch.equal(a, b), f'{name}: two runs differ in {key}'
+
+
+# ------------------------------------------------------------------------------------------------- oracle and bars
+def _limits(name):
+    """Per-ray coarse limits (N,M,1) fp64 as oracle.render forms them."""
+    case = CASES[name]
+    _, _, opts, ro, rd, *_ = _inputs(name)
+    if opts['ray_start'] == 'auto':
+        t0, t1 = orc.ray_limits_box(ro.double(), rd.double(), BW)
+        ok = t1 > t0
+        if bool(ok.any()):
+            t0 = torch.where(ok, t0, t0[ok].min())
+            t1 = torch.where(ok, t1, t0[ok].max())
+        return t0, t1
+    full = lambda v: torch.full(ro.shape[:2] + (1,), float(v), device=DEV, dtype=torch.float64)
+    return full(opts['ray_start']), full(opts['ray_end'])
+
+
+def _decoded(name, v, xyz, rd_s, mode):
+    """sigma (1,K,1) and colour (1,K,32) in fp64 at points xyz (1,K,3); their slopes along the ray direction rd_s (central
+    differences); their bars: the decoder's plus the points' fp32 rounding times one-sided slopes."""
+    case = CASES[name]
+    planes, dec, opts, *_ = _inputs(name)
+    tri = not case.get('eg3d')
+    p64, d64 = planes[v:v + 1].to(DEV, torch.float64), _dec64(dec)
+    run = lambda x: orc.run_model(p64, d64, x, opts, tri)
+    rgb, sig = run(xyz)
+    if mode == 1:
+        b_rgb, b_sig = _three_pass_bars(p64, d64, xyz, force_sigmoid=dec['force_sigmoid'], use_triplane=tri)
+    else:
+        assert tri and not dec['force_sigmoid']
+        b_rgb, b_sig = _single_pass_bars(p64, d64, xyz)
+    h = 1e-7
+    beta_x = 4 * U32 * (xyz.abs() + BW)
+    g_sig, g_rgb = torch.zeros_like(sig), torch.zeros_like(rgb)
+    for i in range(3):
+        e = torch.zeros_like(xyz)
+        e[..., i] = h
+        rp, sp = run(xyz + e)
+        rm, sm = run(xyz - e)
+        b_sig = b_sig + torch.maximum((sp - sig).abs(), (sig - sm).abs()) / h * beta_x[..., i:i + 1]
+        b_rgb = b_rgb + torch.maximum((rp - rgb).abs(), (rgb - rm).abs()) / h * beta_x[..., i:i + 1]
+        g_sig = g_sig + (sp - sm) / (2 * h) * rd_s[..., i:i + 1]
+        g_rgb = g_rgb + (rp - rm) / (2 * h) * rd_s[..., i:i + 1]
+    return sig, rgb, g_sig, g_rgb, b_sig, b_rgb
+
+
+def _masks(name, sig, xyz):
+    """(masked sigma, mask) as apply_masks makes them, and the host's cull threshold."""
+    fl = CASES[name].get('flags', {})
+    masked = orc.apply_masks(sig, xyz, BW, fl.get('triplane_crop'), fl.get('cull_clouds'), fl.get('binarize_clouds'))
+    return masked, masked != sig
+
+
+def _alpha_bar(sig, t):
+    """Bound of the kernel's alpha error per interval (module docstring), from the fp64 sigma and depths (..,L,1)."""
+    dt = t[..., 1:, :] - t[..., :-1, :]
+    smid = (sig[..., 1:, :] + sig[..., :-1, :]) / 2 - 1
+    sp = torch.nn.functional.softplus(smid)
+    alpha = 1 - torch.exp(-sp * dt)
+    spread = sig[..., 1:, :].abs() + sig[..., :-1, :].abs() + 2
+    return (MUFU * (1 - alpha) + U32 * alpha +
+            (1 - alpha) * (dt.abs() * (4 * MUFU * sp + 2 * MUFU + torch.sigmoid(smid) * U32 * spread) + 6 * U32 * sp * dt.abs()))
+
+
+def _render_graph(ro, rd, d_c, u_f, c0, f0, white, leaves, floor=0.01, left=False):
+    """The oracle's render of a chunk of rays as a function of zero-valued perturbation leaves.  c0 / f0: (sigma masked,
+    colour, slope of sigma, slope of colour, mask) of the coarse samples and of the fine samples at the unperturbed fine
+    depths f0['t'].  Returns the outputs (m, 37) and the intermediate values the bars need."""
+    e = leaves
+    t_c = d_c + e['t_c']
+    s_c = c0['sig'] + torch.where(c0['mask'], 0, c0['g_sig']) * e['t_c'] + e['s_c']
+    col_c = c0['rgb'] + c0['g_rgb'] * e['t_c'] + e['c_c']
+    x_c = ro[:, None] + t_c * rd[:, None]
+    _, _, w = orc.march(torch.cat([col_c, x_c], -1)[None], s_c[None], t_c[None], white, alpha_eps=e['a_c'][None])
+    t_f = orc.importance_depths(t_c[..., 0], w[0, ..., 0], u_f, floor=floor, cdf_eps=e['cdf'])[..., None] + e['t_f']
+    dtf = t_f - f0['t']
+    s_f = f0['sig'] + torch.where(f0['mask'], 0, f0['g_sig']) * dtf + e['s_f']
+    col_f = f0['rgb'] + f0['g_rgb'] * dtf + e['c_f']
+    x_f = ro[:, None] + t_f * rd[:, None]
+    t_all = torch.cat([t_c, t_f], -2)
+    order = torch.sort(t_all.detach(), dim=-2, stable=True)[1]
+    t_all = torch.gather(t_all, -2, order)
+    col = torch.gather(torch.cat([torch.cat([col_c, x_c], -1), torch.cat([col_f, x_f], -1)], -2), -2,
+                       order.expand(-1, -1, 35))
+    sig = torch.gather(torch.cat([s_c, s_f], -2), -2, order)
+    inf = torch.tensor(float('inf'), device=DEV, dtype=torch.float64)
+    out, depth, w = orc.march(col[None], sig[None], t_all[None], white, -inf, inf, alpha_eps=e['a'][None], left_colours=left)
+    o = torch.cat([out[0, :, :32], depth[0], w[0].sum(1), out[0, :, 32:]], -1)
+    return o, dict(t_all=t_all, sig=sig, col=col, w=w[0], t_f=t_f)
+
+
+def _zero_leaves(m, S, grad=False):
+    L = 2 * S
+    shapes = dict(t_c=(m, S, 1), s_c=(m, S, 1), c_c=(m, S, 32), a_c=(m, S - 1, 1), cdf=(m, S - 2), t_f=(m, S, 1), s_f=(m, S, 1),
+                  c_f=(m, S, 32), a=(m, L - 1, 1))
+    return {k: torch.zeros(s, device=DEV, dtype=torch.float64, requires_grad=grad) for k, s in shapes.items()}
+
+
+def _chunk(name, v, sl, mode, with_bars=True, controls=False):
+    """The oracle's outputs (m, 37) for rays `sl` of view v, and (with_bars) their bars (m, 37), the rays to exclude (m,)
+    and the mutated oracles' outputs (controls)."""
+    case = CASES[name]
+    planes, dec, opts, ro_all, rd_all, u_c_all, u_f_all = _inputs(name)
+    S = case['S']
+    M = ro_all.shape[1]
+    ro, rd = ro_all[v, sl].double(), rd_all[v, sl].double()
+    m = ro.shape[0]
+    u_c = u_c_all[v, sl].double()
+    u_f = u_f_all[v * M:(v + 1) * M][sl].double()
+    t0, t1 = (t[v, sl] for t in _limits(name))
+    if opts['ray_start'] == 'auto':
+        d_c = orc.stratified_depths(u_c[None], t0[None], t1[None])[0]
+    else:
+        d_c = orc.stratified_depths(u_c[None], opts['ray_start'], opts['ray_end'], opts.get('disparity_space_sampling', False))[0]
+    white = bool(opts.get('white_back', False))
+
+    def samples(t):
+        xyz = (ro[:, None] + t * rd[:, None]).reshape(1, -1, 3)
+        rd_s = rd[:, None].expand(-1, t.shape[1], -1).reshape(1, -1, 3)
+        sig, rgb, g_sig, g_rgb, b_sig, b_rgb = _decoded(name, v, xyz, rd_s, mode)
+        sig_m, mask = _masks(name, sig, xyz)
+        r = lambda x: x.reshape(m, t.shape[1], -1)
+        return dict(sig=r(sig_m), raw=r(sig), rgb=r(rgb), g_sig=r(g_sig), g_rgb=r(g_rgb), b_sig=r(torch.where(mask, 0, b_sig)),
+                    b_sig_raw=r(b_sig), g_sig_raw=r(g_sig), b_rgb=r(b_rgb), mask=r(mask), xyz=r(xyz), t=t)
+
+    c0 = samples(d_c)
+    _, _, w = orc.march(torch.cat([c0['rgb'], c0['xyz']], -1)[None], c0['sig'][None], d_c[None], white)
+    t_f0 = orc.importance_depths(d_c[..., 0], w[0, ..., 0], u_f)[..., None]
+    # Descending coarse depths give negative weights; where the pdf they make is not positive, the cdf is not monotone and
+    # the reference's searchsorted (and so its fine depths) depends on the search's probe order: such rays are counted,
+    # not compared
+    wp = torch.nn.functional.avg_pool1d(torch.nn.functional.max_pool1d(w[0, ..., 0][:, None], 2, 1, padding=1), 2, 1)[:, 0] + 0.01
+    illdef = (wp[:, 1:-1] + 1e-5).min(1).values <= 1e-6
+    f0 = samples(t_f0)
+    zero = _zero_leaves(m, S)
+    o, mid = _render_graph(ro, rd, d_c, u_f, c0, f0, white, zero)
+    res = dict(o=o, t_max=mid['t_all'].max(), t_min=mid['t_all'].min(), illdef=illdef)
+    if controls:
+        # the colour map without its gain: s - 0.001 instead of 1.002 s - 0.001
+        dec_s = _dec64(dict(dec, force_sigmoid=True))
+        p64 = planes[v:v + 1].to(DEV, torch.float64)
+        rgb_s = lambda smp: orc.run_model(p64, dec_s, smp['xyz'].reshape(1, -1, 3), opts, not case.get('eg3d'))[0].reshape(m, -1, 32) - 0.001
+        c0s, f0s = dict(c0, rgb=rgb_s(c0)), dict(f0, rgb=rgb_s(f0))
+        res['ctl_colour_map'] = _render_graph(ro, rd, d_c, u_f, c0s, f0s, white, zero)[0]
+        # the pdf floor moves the fine depths: decode at the moved depths
+        t_f5 = orc.importance_depths(d_c[..., 0], w[0, ..., 0], u_f, floor=0.005)[..., None]
+        f5 = samples(t_f5)
+        res['ctl_pdf_floor'] = _render_graph(ro, rd, d_c, u_f, c0, f5, white, zero, floor=0.005)[0]
+        res['ctl_omega'] = _render_graph(ro, rd, d_c, u_f, c0, f0, white, zero, left=True)[0]
+    if not with_bars:
+        return res
+    leaves = _zero_leaves(m, S, grad=True)
+    o, mid = _render_graph(ro, rd, d_c, u_f, c0, f0, white, leaves)
+    # beta of every leaf
+    L = 2 * S
+    span = (t1 - t0).abs()[:, None]
+    beta = dict(t_c=16 * U32 * (d_c.abs() + t0.abs()[:, None] + t1.abs()[:, None]), s_c=c0['b_sig'], c_c=c0['b_rgb'],
+                a_c=_alpha_bar(c0['sig'], d_c), cdf=torch.full((m, S - 2), (2 * S + 40) * U32, device=DEV, dtype=torch.float64),
+                t_f=8 * U32 * (t_f0.abs() + span), s_f=f0['b_sig'], c_f=f0['b_rgb'], a=_alpha_bar(mid['sig'], mid['t_all']))
+    names = list(leaves)
+    bar = torch.zeros(m, 37, device=DEV, dtype=torch.float64)
+    for k in range(37):
+        gs = torch.autograd.grad(o[:, k].sum(), [leaves[n] for n in names], retain_graph=True, allow_unused=True)
+        for n, gk in zip(names, gs):
+            if gk is not None:
+                bar[:, k] += (gk.abs() * beta[n]).reshape(m, -1).sum(1)
+    fine_move = None
+    fl = case.get('flags', {})
+    if fl:                                    # the fine depths' own bars, for the mask borders
+        fine_move = torch.zeros(m, S, device=DEV, dtype=torch.float64)
+        tf = mid['t_f'][..., 0]
+        for f in range(S):
+            gs = torch.autograd.grad(tf[:, f].sum(), [leaves[n] for n in ('t_c', 's_c', 'a_c', 'cdf', 't_f')], retain_graph=True,
+                                     allow_unused=True)
+            for n, gk in zip(('t_c', 's_c', 'a_c', 'cdf', 't_f'), gs):
+                if gk is not None:
+                    fine_move[:, f] += (gk.abs() * beta[n]).reshape(m, -1).sum(1)
+        fine_move = 2 * fine_move
+    # floors: the roundings of the sums that form each output
+    wts = mid['w'][..., 0].detach()
+    W = wts.sum(1)
+    tm = (mid['t_all'][:, 1:] + mid['t_all'][:, :-1])[..., 0] / 2
+    om = torch.cat([wts[:, :1] * 0, wts], 1) / 2 + torch.cat([wts, wts[:, :1] * 0], 1) / 2
+    rel = 2 * (L + 8) * U32
+    fW = rel * W
+    fD = rel * (wts * tm.abs()).sum(1)
+    floor = torch.zeros_like(bar)
+    floor[:, :32] = 2 * rel * (om[..., None] * (mid['col'][..., :32].detach().abs() + 0.002)).sum(1) + (2 * fW[:, None] if white else 0) + 8 * U32
+    dep = (wts * tm).sum(1) / W
+    floor[:, 32] = (fD + dep.abs() * fW) / W + U32 * dep.abs()
+    floor[:, 33] = fW
+    floor[:, 34:] = 2 * (ro.abs() * fW[:, None] + rd.abs() * fD[:, None] + 3 * U32 * (ro.abs() * W[:, None] + rd.abs() * (wts * tm).sum(1)[:, None])
+                         + (fW[:, None] if white else 0)) + 4 * U32
+    res['bar'] = 2 * bar + floor
+    # rays with a sample within its bar of a jump
+    near = torch.zeros(m, dtype=torch.bool, device=DEV)
+    if fl.get('cull_clouds') or fl.get('binarize_clouds'):
+        thr = _cull_sigma(fl.get('cull_clouds') or fl.get('binarize_clouds'))
+        for smp, move in ((c0, beta['t_c'][..., 0]), (f0, fine_move)):
+            cropped = orc.crop_mask(smp['xyz'].reshape(1, -1, 3), fl['triplane_crop'], BW).reshape(m, -1) if fl.get('triplane_crop') \
+                else torch.zeros(m, S, dtype=torch.bool, device=DEV)
+            # the slope of the unmasked sigma along the ray, times how far the sample's depth may move
+            g_raw = smp['g_sig_raw'][..., 0].abs()
+            b = smp['b_sig_raw'][..., 0] + g_raw * move + 2 * U32 * abs(thr) + 1e-12
+            near |= (~cropped & ((smp['raw'][..., 0] - thr).abs() <= b)).any(1)
+    if fl.get('triplane_crop'):
+        lim = BW / 2 - fl['triplane_crop']
+        for smp, move in ((c0, beta['t_c'][..., 0]), (f0, fine_move)):
+            bx = 4 * U32 * (smp['xyz'].abs() + BW) + rd.abs()[:, None] * move[..., None] + 2 * U32 * lim
+            near |= ((smp['xyz'][..., [0, 2]].abs() - lim).abs() <= bx[..., [0, 2]]).any(-1).any(1)
+    res['near'] = near
+    res['cull_share'] = None
+    if fl.get('cull_clouds'):
+        unc = ~orc.crop_mask(c0['xyz'].reshape(1, -1, 3), fl['triplane_crop'], BW).reshape(m, -1) if fl.get('triplane_crop') else \
+            torch.ones(m, S, dtype=torch.bool, device=DEV)
+        res['cull_share'] = ((c0['mask'][..., 0] & unc).sum().item(), unc.sum().item())
+    return res
+
+
+def _rays_of(name):
+    case = CASES[name]
+    M = _inputs(name)[3].shape[1]
+    idx = torch.arange(0, M, case.get('stride', 1), device=DEV)
+    return [(v, idx[i:i + CHUNK]) for v in range(case['N']) for i in range(0, idx.numel(), CHUNK)]
+
+
+class Worst:
+    def __init__(self):
+        self.err = {k: 0.0 for k in OUTPUTS}
+        self.ratio = {k: 0.0 for k in OUTPUTS}
+
+    def add(self, got, want, bar, keep):
+        err = (got.double() - want).abs().nan_to_num(nan=float('inf'))[keep]
+        r = (err / bar[keep])
+        for j, key in enumerate(OUTPUTS):
+            cols = [i for i, n in enumerate(OUT_NAMES) if n == key]
+            if err.shape[0]:
+                self.err[key] = max(self.err[key], err[:, cols].max().item())
+                self.ratio[key] = max(self.ratio[key], r[:, cols].max().item())
+
+
+def _flat(out, v, sl):
+    rgb, depth, wsum, xyz = out
+    return torch.cat([rgb[v, sl], depth[v, sl], wsum[v, sl], xyz[v, sl]], -1)
+
+
+def _compare(name, out, mode, controls=()):
+    """The kernel's outputs against the oracle's, ray by ray.  Returns the worst abs errors, ratios and control ratios."""
+    res_all = [(v, sl, _chunk(name, v, sl, mode, controls=bool(controls))) for v, sl in _rays_of(name)]
+    t_hi = max(r['t_max'].item() for *_, r in res_all)
+    worst = Worst()
+    n_near = n_total = n_ill = 0
+    ctl = {c: 0.0 for c in controls}
+    cull = [0, 0]
+    for v, sl, r in res_all:
+        got = _flat(out, v, sl)
+        want, bar = r['o'].clone(), r['bar'].clone()
+        dead = (want[:, 33] == 0) | (got[:, 33] == 0)
+        want[dead, 32] = t_hi                                  # nan_to_num(inf) then the clamp to the batch's largest depth
+        bar[dead, 32] = 64 * U32 * abs(t_hi)
+        keep = ~r['near'] & ~r['illdef']
+        n_ill += r['illdef'].sum().item()
+        worst.add(got, want, bar, keep)
+        n_near += r['near'].sum().item()
+        n_total += r['near'].numel()
+        for c in controls:
+            err = (got.double() - r[c]).abs()[keep]
+            cols = slice(0, 32) if c != 'ctl_pdf_floor' else slice(0, 37)
+            if err.shape[0]:
+                ctl[c] = max(ctl[c], (err[:, cols] / bar[keep][:, cols]).max().item())
+        if r['cull_share']:
+            cull[0] += r['cull_share'][0]
+            cull[1] += r['cull_share'][1]
+    for key in OUTPUTS:
+        print(f'{name} mode {mode} {key}: max abs err {worst.err[key]:.3e}, worst err / bar {worst.ratio[key]:.4f}')
+    print(f'{name}: {n_near} of {n_total} rays excluded (a sample within its bar of a mask threshold), {n_ill} with a '
+          f'non-positive importance pdf')
+    if name in NEGATIVE_PDF:
+        assert n_ill == n_total, (name, n_ill, n_total)
+    else:
+        assert n_ill == 0, (name, n_ill)
+    return worst, n_near / max(n_total, 1), ctl, cull
+
+
+# ------------------------------------------------------------------------------------------------- tests
+def test_gpu_fp64_oracle_equals_cpu_oracle():
+    """oracle.render in fp64 on the device equals the CPU fp32 oracle that the reference fixtures pin (config1,
+    mid_eval96) within the fp32 run's rounding.  The device run takes the CPU run's depths and mask decisions (as
+    test_render_backward_paths_gpu does): a cull decision within fp32 rounding of its threshold would otherwise move a whole
+    sample, and how the CPU's fp32 sums round depends on the host's thread count."""
+    from tests.golden.cases import RENDER_CASES, build_case_inputs
+    from tests.helpers import case_rays
+    for fixture in ('config1', 'mid_eval96'):
+        case = RENDER_CASES[fixture]
+        planes, dec, c2w, K, u_c, u_f, opts = build_case_inputs(case)
+        ro, rd = case_rays(case, c2w, K)
+        fl = {k: case[k] for k in ('triplane_crop', 'cull_clouds', 'binarize_clouds') if case.get(k)}
+        cpu, smp = orc.render(planes, dec, ro, rd, opts, u_c, u_f, return_samples=True, **fl)
+        to = lambda t: None if t is None else t.to(DEV)
+        gpu = orc.render(planes.to(DEV, torch.float64), _dec64(dec), ro.to(DEV), rd.to(DEV), opts, None, None,
+                         depths=tuple(to(t) for t in smp['depths']), masks=tuple(to(t) for t in smp['masks']), **fl)
+        for key, a, b in zip(OUTPUTS, gpu, cpu):
+            assert a.dtype == torch.float64
+            err = (a.cpu() - b.double()).abs().max().item()
+            print(f'pin {fixture} {key}: {err:.2e}')
+            assert err <= PIN, (fixture, key, err)
+
+
+@pytest.mark.parametrize('name', list(CASES))
+def test_render_graph_is_the_oracle(name):
+    """_chunk's zero-leaf graph gives oracle.render's fp64 outputs, with every case's masks, limits, plane order and
+    background, so the bars are derivatives of the oracle the kernel is compared with.  'auto' cases pass render the
+    whole batch (its fallback limits are reduced over the batch); the others the first 256 rays of view 0.  depth is
+    compared where W > 0 (render clamps the others to its batch's largest depth)."""
+    case = CASES[name]
+    planes, dec, opts, ro, rd, u_c, u_f = _inputs(name)
+    N, M = ro.shape[:2]
+    n = M if opts['ray_start'] == 'auto' else min(256, M)
+    views = range(N) if opts['ray_start'] == 'auto' else range(1)
+    fl = case.get('flags', {})
+    want = orc.render(planes[:len(views)].to(DEV, torch.float64), _dec64(dec), ro[:len(views), :n].double(), rd[:len(views), :n].double(),
+                      opts, u_c[:len(views), :n].double(), u_f.view(N, M, -1)[:len(views), :n].reshape(len(views) * n, -1).double(),
+                      use_triplane=not case.get('eg3d'), **fl)
+    worst = dict.fromkeys(OUTPUTS, 0.0)
+    for v in views:
+        for i in range(0, n, CHUNK):
+            sl = torch.arange(i, min(i + CHUNK, n), device=DEV)
+            got = _chunk(name, v, sl, 1, with_bars=False)['o']
+            ref = _flat(want, v, sl)
+            live = ref[:, 33] > 0
+            for key, a_, b_ in zip(OUTPUTS, ref.split([32, 1, 1, 3], -1), got.split([32, 1, 1, 3], -1)):
+                if key == 'depth':
+                    a_, b_ = a_[live], b_[live]
+                worst[key] = max(worst[key], (a_ - b_).abs().max().item() if a_.numel() else 0.0)
+    print(f'{name} graph vs render: ' + ', '.join(f'{k} {e:.1e}' for k, e in worst.items()))
+    assert max(worst.values()) <= 1e-12, (name, worst)
+
+
+def test_three_pass_bars_hold_on_the_decode():
+    """The per-sample mode 1 bar (_three_pass_bars) holds on p3d_decode_points (the same decoder code, fused_common.cuh) at
+    the oracle's own coarse and fine sample positions of train48's first view."""
+    name = 'train48'
+    planes, dec, opts, ro, rd, u_c, u_f = _inputs(name)
+    n = 1024
+    p64, d64 = planes[:1].to(DEV, torch.float64), _dec64(dec)
+    _, smp = orc.render(p64, d64, ro[:1, :n].double(), rd[:1, :n].double(), opts, u_c[:1, :n].double(), u_f[:n].double(),
+                        return_samples=True)
+    pts = [(ro[:1, :n, None].double() + d * rd[:1, :n, None].double()).reshape(1, -1, 3) for d in smp['depths']]
+    xyz = torch.cat(pts, 1).float()
+    x64 = xyz.double()
+    rgb, sig = orc.run_model(p64, d64, x64, opts, True)
+    b_rgb, b_sig = _three_pass_bars(p64, d64, x64)
+    k_rgb, k_sig = _decode_points(planes[:1].to(DEV), dec, xyz, 1)
+    for key, k, w, b in (('rgb', k_rgb, rgb, b_rgb), ('sigma', k_sig, sig, b_sig)):
+        err = (k.double() - w).abs().nan_to_num(nan=float('inf'))
+        print(f'decode at the render samples {key}: max abs err {err.max().item():.3e}, worst err / bar {(err / b).max().item():.4f}, '
+              f'median bar {b.median().item():.2e}')
+        assert (err / b).max().item() <= 1.0, key
+
+
+CONTROLS = {'ctl_colour_map': 'colour map s - 0.001 instead of 1.002 s - 0.001', 'ctl_pdf_floor': 'importance pdf floor 0.005',
+            'ctl_omega': 'omega = w_i'}
+# control -> the case it must miss the kernel by >= 20x the bar on (every control is computed and printed on each)
+CONTROL_CASES = {'ctl_colour_map': 'saturated48', 'ctl_pdf_floor': 'dense48', 'ctl_omega': 'dense48'}
+CONTROL_MIN = 20.0
+
+
+def _case_checks(name, out, bounds):
+    case = CASES[name]
+    planes, dec, opts, ro, rd, u_c, u_f = _inputs(name)
+    N, M = ro.shape[:2]
+    S = case['S']
+    groups = N * M // (384 // S)
+    per = _per_cta(groups, n_sm())
+    if case.get('per_cta'):
+        assert (min(per), max(per)) == case['per_cta'], (name, min(per), max(per))
+    if name == 'n_my_1':
+        assert groups < n_sm() and max(per) == 1
+    if name == 'n_my_2':
+        assert max(per) == 2, per
+    if name == 'n_my_3':
+        assert max(per) == 3, per
+    if name in ('all_miss48', 'all_miss96', 'all_miss_negpdf48'):
+        assert bounds[4].item() == 0, 'a ray hit the box'
+        t0, t1 = _limits(name)
+        assert (t1 < t0).all(), 'coarse depths do not descend'
+    if name == 'descending96':
+        assert opts['ray_start'] > opts['ray_end']
+    if name == 'saturated48':
+        assert (out[0] > 0.99).double().mean().item() > 0.9, 'colours are not saturated'
+    if name == 'auto_eg3d':
+        t0, t1 = orc.ray_limits_box(ro.double(), rd.double(), BW)
+        miss = (t1 <= t0).double().mean().item()
+        print(f'auto_eg3d: {miss:.3f} of the rays miss the box')
+        assert 0.01 < miss < 0.9, miss
+    print(f'{name}: {groups} groups, {min(per)}-{max(per)} per CTA')
+
+
+@pytest.mark.parametrize('name', [n for n in CASES if n != 'single_pass'])
+def test_fused_matches_fp64_oracle(name):
+    case = CASES[name]
+    if case['P'] >= 512:
+        free, _ = torch.cuda.mem_get_info()
+        if free < FREE_BYTES:
+            pytest.skip(f'needs {FREE_BYTES >> 30} GB of free device memory')
+    t0 = time.time()
+    torch.cuda.reset_peak_memory_stats()
+    # the values first: a kernel that reads memory it never wrote may still repeat itself
+    out, bounds, again = _kernel(name, checks_later=True)
+    _case_checks(name, out, bounds)
+    controls = tuple(CONTROLS) if name in CONTROL_CASES.values() else ()
+    worst, share, ctl, cull = _compare(name, out, 1, controls)
+    if cull[1]:
+        print(f'{name}: cull removes {cull[0] / cull[1]:.3f} of the uncropped coarse samples')
+        if name == 'eval_flags96':
+            assert 0.2 <= cull[0] / cull[1] <= 0.5, cull
+    for c, r in ctl.items():
+        print(f'negative control "{CONTROLS[c]}" on {name}: worst err / bar {r:.1f}')
+    print(f'{name}: {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GB')
+    assert share <= EXCLUDE_SHARE_MASKS.get(name, EXCLUDE_SHARE[1]), share
+    assert max(worst.ratio.values()) <= 1.0, (name, worst.ratio)
+    _repeats(name, out, again)
+    for c, r in ctl.items():
+        if CONTROL_CASES[c] == name:
+            assert r >= CONTROL_MIN, (CONTROLS[c], r)
+    if name in DESCENDING:                 # the SIMT kernel sorts after mapping: the same outputs at its own bar
+        simt, _ = _kernel(name, mode=0)
+        for key, a, b in zip(OUTPUTS, simt, out):
+            err = (a - b).abs().max().item()
+            print(f'{name} SIMT vs fused {key}: {err:.3e}')
+        for v, sl in _rays_of(name):
+            r = _chunk(name, v, sl, 1, with_bars=False)
+            if name in NEGATIVE_PDF:
+                continue
+            err = (_flat(simt, v, sl).double() - r['o']).abs().max().item()
+            assert err <= SIMT_BAR, (name, 'SIMT', err)
+
+
+def test_single_pass_matches_fp64_oracle():
+    """mlp_mode 2 within its propagated bars, and >= 10x further from the oracle than mode 1."""
+    name = 'single_pass'
+    two, _ = _kernel(name, mode=2)
+    one, _ = _kernel(name, mode=1)
+    w2, share2, *_ = _compare(name, two, 2)
+    w1, share1, *_ = _compare(name, one, 1)
+    assert share2 <= EXCLUDE_SHARE[2] and share1 <= EXCLUDE_SHARE[1]
+    assert max(w2.ratio.values()) <= 1.0 and max(w1.ratio.values()) <= 1.0
+    for key in ('rgb', 'wsum'):
+        assert w2.err[key] >= 10 * w1.err[key], ('single pass is not reaching the kernel', key, w2.err[key], w1.err[key])
