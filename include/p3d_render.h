@@ -84,7 +84,16 @@ typedef struct p3d_render_params {
        out-of-band device memory `depth_bounds` (see p3d_render_depth_bounds); the host all-reduces them
        (MIN, MAX) and calls p3d_depth_finalize. */
     int32_t defer_depth_clamp;
-    int32_t reserved0;
+    /* multiplane tri-planes (rendering_kwargs['triplane_depth'] = D > 1; sample_from_planes, renderer.py:84-94): each plane
+       is D slabs of (H, W, C) texels, sampled trilinearly (zero padding, align_corners=False) at the point's two plane
+       coordinates and, across the slabs, its third component of project_onto_planes: z, y, then y (P3D_PLANES_EG3D) or
+       x (P3D_PLANES_PANIC3D).  0 and 1 mean one slab.  Slab d of plane p of view v starts at element
+       v*stride_view + p*stride_plane + d*plane_h*stride_row; texels stay channels-last (channel stride 1).  For D > 1:
+         - stride_plane >= D*plane_h*stride_row and stride_view (unless 0) >= 3*stride_plane, else P3D_EINVAL;
+         - only the fp32 SIMT kernels have a trilinear gather: p3d_render_fused_supported and p3d_decode_tc_supported
+           return 0, an explicit P3D_MLP_TC_* request fails with P3D_EUNSUPPORTED, and so does p3d_render_forward_host;
+         - the gradients of p3d_render_backward and p3d_decode_points_backward are (N,3,D,H,W,C) contiguous fp32. */
+    int32_t plane_depth;
 } p3d_render_params;
 
 const char* p3d_version(void);

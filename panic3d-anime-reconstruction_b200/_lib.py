@@ -31,7 +31,7 @@ class RenderParams(C.Structure):
         ('w1_gain', C.c_float), ('b1_gain', C.c_float), ('w2_gain', C.c_float), ('b2_gain', C.c_float),
         ('force_sigmoid', C.c_int32), ('mlp_mode', C.c_int32),
         ('seed', C.c_uint64),
-        ('defer_depth_clamp', C.c_int32), ('reserved0', C.c_int32),
+        ('defer_depth_clamp', C.c_int32), ('plane_depth', C.c_int32),
     ]
 
 

@@ -67,6 +67,17 @@ int make_geom(const p3d_render_params* p, Geom* g) {
     // quads of 4 channels: 16 B (fp32) / 8 B (bf16) vector loads
     P3D_REQUIRE(p->stride_view % 4 == 0 && p->stride_plane % 4 == 0 && p->stride_row % 4 == 0 && p->stride_col % 4 == 0,
                 "plane strides must be multiples of 4 elements");
+    // multiplane tri-planes: D slabs per plane, slab d at d * plane_h * stride_row inside its plane
+    P3D_REQUIRE(p->plane_depth >= 0, "plane_depth must be >= 0, got %d", p->plane_depth);
+    g->D = p->plane_depth > 1 ? p->plane_depth : 1;
+    if (g->D > 1) {
+        P3D_REQUIRE(p->stride_plane >= (int64_t)g->D * p->plane_h * p->stride_row,
+                    "stride_plane %lld is shorter than plane_depth * plane_h * stride_row = %lld", (long long)p->stride_plane,
+                    (long long)g->D * p->plane_h * p->stride_row);
+        P3D_REQUIRE(p->stride_view == 0 || p->stride_view >= 3 * p->stride_plane,
+                    "stride_view %lld is shorter than 3 * stride_plane = %lld", (long long)p->stride_view,
+                    3 * (long long)p->stride_plane);
+    }
     g->coord_scale = (float)(2.0 / p->box_warp);
     g->half_box = (float)(p->box_warp / 2.0);
     g->ray_mode = p->ray_mode; g->disparity = p->disparity; g->white_back = p->white_back; g->plane_mode = p->plane_mode;
@@ -371,14 +382,23 @@ size_t p3d_render_workspace_bytes(const p3d_render_params* p) {
 
 int p3d_render_fused_supported(const p3d_render_params* p) {
     Geom g;
-    if (!p || make_geom(p, &g)) return 0;
+    if (!p || make_geom(p, &g) || g.D > 1) return 0;      // multiplane planes: fp32 SIMT kernels only
     return fused_ws3_supported(g) ? 1 : 0;
 }
 
 int p3d_decode_tc_supported(const p3d_render_params* p, int64_t n_points_total) {
     Geom g;
-    if (!p || make_geom(p, &g)) return 0;
+    if (!p || make_geom(p, &g) || g.D > 1) return 0;
     return decode_tc_supported(g, n_points_total) ? 1 : 0;
+}
+
+// an explicit tensor-core request for multiplane planes fails: only the fp32 SIMT kernels gather trilinearly
+static int refuse_tc_multiplane(const Geom& g, const p3d_render_params* p) {
+    if (g.D > 1 && (p->mlp_mode == P3D_MLP_TC_3XBF16 || p->mlp_mode == P3D_MLP_TC_BF16)) {
+        set_error("plane_depth %d (multiplane tri-planes) has no tensor-core kernel; use mlp_mode P3D_MLP_FP32_SIMT", g.D);
+        return P3D_EUNSUPPORTED;
+    }
+    return P3D_OK;
 }
 
 int p3d_render_forward(const p3d_render_params* p, const void* planes, const float* w1, const float* b1, const float* w2,
@@ -390,6 +410,7 @@ int p3d_render_forward(const p3d_render_params* p, const void* planes, const flo
     if (rc) return rc;
     P3D_REQUIRE(p->ray_mode == P3D_RAYS_NUMERIC || p->ray_mode == P3D_RAYS_AUTOBOX, "bad ray_mode %d", p->ray_mode);
     P3D_REQUIRE(!(p->ray_mode == P3D_RAYS_AUTOBOX && p->disparity), "disparity sampling needs numeric ray limits");
+    if ((rc = refuse_tc_multiplane(g, p))) return rc;
     if ((long long)g.N * g.M == 0) return P3D_OK;           // empty batch: empty outputs, pointers may be NULL
     P3D_REQUIRE(planes && w1 && b1 && w2 && b2 && ray_origins && ray_dirs, "null input pointer");
     P3D_REQUIRE(out_rgb && out_depth && out_wsum && out_xyz, "null output pointer");
@@ -452,6 +473,7 @@ int p3d_decode_points(const p3d_render_params* p, const void* planes, const floa
     int rc = make_geom(p, &g);
     if (rc) return rc;
     P3D_REQUIRE(n_points_per_view >= 0, "negative point count");
+    if ((rc = refuse_tc_multiplane(g, p))) return rc;
     if ((long long)g.N * n_points_per_view == 0) return P3D_OK;
     P3D_REQUIRE(planes && w1 && b1 && w2 && b2 && coords && out_rgb && out_sigma, "null pointer");
     if (p->mlp_mode == P3D_MLP_TC_3XBF16 || p->mlp_mode == P3D_MLP_TC_BF16) {
@@ -487,6 +509,7 @@ int p3d_volume_query(const p3d_render_params* p, const void* planes, const float
     if (rc) return rc;
     P3D_REQUIRE(resolution >= 2 && resolution <= 1024, "resolution must be in [2, 1024], got %d", resolution);
     P3D_REQUIRE(cube_length > 0, "cube_length must be > 0");
+    if ((rc = refuse_tc_multiplane(g, p))) return rc;
     if (g.N == 0) return P3D_OK;
     P3D_REQUIRE(planes && w1 && b1 && w2 && b2 && out_sigma, "null pointer");
     VolumeSpec vol;
@@ -521,6 +544,11 @@ int p3d_render_forward_host(const p3d_render_params* p_in, const float* planes_n
     P3D_REQUIRE(p_in && planes_nchw && w1 && b1 && w2 && b2 && cam2world && intrinsics, "null input pointer");
     P3D_REQUIRE(out_rgb && out_depth && out_wsum && out_xyz, "null output pointer");
     p3d_render_params p = *p_in;
+    if (p.plane_depth > 1) {
+        set_error("p3d_render_forward_host takes one-slab NCHW tri-planes; render multiplane tri-planes (plane_depth %d) with "
+                  "p3d_render_forward on device buffers", p.plane_depth);
+        return P3D_EUNSUPPORTED;
+    }
     P3D_REQUIRE(p.n_rays == resolution * resolution, "n_rays must equal resolution^2");
     if (p.ray_mode == P3D_RAYS_AUTOBOX) {
         set_error("p3d_render_forward_host renders view by view and cannot reproduce the batch-wide fill of 'auto' ray limits "

@@ -155,8 +155,10 @@ struct SampleBwdArgs {
 };
 
 constexpr int kXs = 33, kHs = 65, kDs = 36;
-constexpr size_t kBwdSmemFloats = (size_t)kHidden * kC + kOut * kHidden + kHidden + 36 +
-                                  (size_t)kT * (kXs + kHs + kHs + kDs + kHs + kXs) + kT * 12 * 2 + kT * 2 + kT;
+// taps per sample: 4 per plane, 8 per plane for multiplane tri-planes (TRI)
+template <bool TRI> constexpr int kTaps = TRI ? 24 : 12;
+template <bool TRI> constexpr size_t kBwdSmemFloats = (size_t)kHidden * kC + kOut * kHidden + kHidden + 36 +
+                                                      (size_t)kT * (kXs + kHs + kHs + kDs + kHs + kXs) + kT * kTaps<TRI> * 2 + kT * 2 + kT;
 
 // texel indices (p*H*W + y*W + x, or -1) and bilinear weights of one plane, from the forward's dev::bilinear_footprint
 __device__ __forceinline__ void tap_texels(const Geom& g, int plane, float2 c, int2* out) {
@@ -170,8 +172,10 @@ __device__ __forceinline__ void tap_texels(const Geom& g, int plane, float2 c, i
     }
 }
 
-template <bool BF16>
+// TRI: multiplane tri-planes (g.D > 1): trilinear re-gather, 8 taps per plane scattered to the (N,3,D,H,W,C) gradient
+template <bool BF16, bool TRI>
 __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
+    constexpr int NT = kTaps<TRI>, PT = NT / 3;
     extern __shared__ float sm[];
     float* s_w1 = sm;                        // [64][32]  effective (gain folded)
     float* s_w2 = s_w1 + kHidden * kC;       // [33][64]
@@ -183,8 +187,8 @@ __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
     float* s_do = s_hs + kT * kHs;           // [128][36] d_logits
     float* s_dp = s_do + kT * kDs;           // [128][65] d_pre
     float* s_dx = s_dp + kT * kHs;           // [128][33] d_features (already / 3)
-    int2* s_tap = reinterpret_cast<int2*>(s_dx + kT * kXs);   // [128][12]
-    float* s_xz = reinterpret_cast<float*>(s_tap + kT * 12);  // [128][2]
+    int2* s_tap = reinterpret_cast<int2*>(s_dx + kT * kXs);   // [128][NT]
+    float* s_xz = reinterpret_cast<float*>(s_tap + kT * NT);  // [128][2]
     int* s_view = reinterpret_cast<int*>(s_xz + kT * 2);      // [128]
 
     const Geom& g = a.g;
@@ -216,14 +220,15 @@ __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
                     const float3 pt = ray_point(a.ro + ray * 3, a.rd + ray * 3, a.depth[gidx]);
                     px = pt.x; py = pt.y; pz = pt.z;
                 }
-                f = gather_features<BF16>(a.planes, g, view, px, py, pz, qd);
+                f = gather_features<BF16, TRI>(a.planes, g, view, px, py, pz, qd);
             }
             if (qd < 3) {                                         // lanes 0..2 of a sample record plane qd's taps
                 if (ok) {
-                    tap_texels(g, qd, plane_coords(g, qd, px, py, pz), s_tap + local * 12 + qd * 4);
+                    if constexpr (TRI) slab_texels(g, qd, plane_coords(g, qd, px, py, pz), plane_normal(g, qd, px, py, pz), s_tap + local * NT + qd * PT);
+                    else tap_texels(g, qd, plane_coords(g, qd, px, py, pz), s_tap + local * NT + qd * PT);
                 } else {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) s_tap[local * 12 + qd * 4 + k] = make_int2(-1, 0);
+                    for (int k = 0; k < PT; ++k) s_tap[local * NT + qd * PT + k] = make_int2(-1, 0);
                 }
             }
             float* dst = s_x + local * kXs + 4 * qd;
@@ -355,7 +360,7 @@ __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
     // ---- F) scatter d_features to the tri-plane gradient: 8 lanes x float4 per tap
     {
         const int sub = lane >> 3, qd = lane & 7;
-        const long long plane_elems = (long long)3 * g.H * g.W * kC;
+        const long long plane_elems = (long long)3 * (TRI ? g.D : 1) * g.H * g.W * kC;
         for (int round = 0; round < 8; ++round) {
             const int local = warp * 32 + round * 4 + sub;
             if (tile0 + local >= a.total) continue;
@@ -363,14 +368,25 @@ __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
             const float4 dv = make_float4(dxr[0], dxr[1], dxr[2], dxr[3]);
             float* base = a.d_planes + (long long)s_view[local] * plane_elems + 4 * qd;
 #pragma unroll
-            for (int k = 0; k < 12; ++k) {
-                const int2 tp = s_tap[local * 12 + k];
+            for (int k = 0; k < NT; ++k) {
+                const int2 tp = s_tap[local * NT + k];
                 if (tp.x < 0) continue;
                 const float wgt = __int_as_float(tp.y);
                 atomicAdd(reinterpret_cast<float4*>(base + (long long)tp.x * kC), make_float4(dv.x * wgt, dv.y * wgt, dv.z * wgt, dv.w * wgt));
             }
         }
     }
+}
+
+// the k_sample_backward instance for these planes and its dynamic shared memory (bytes)
+using SampleBwdKernel = void (*)(const SampleBwdArgs);
+SampleBwdKernel sample_backward_kernel(const Geom& g, const p3d_render_params* p, size_t* smem) {
+    if (g.D > 1) {
+        *smem = kBwdSmemFloats<true> * sizeof(float);
+        return p->planes_bf16 ? k_sample_backward<true, true> : k_sample_backward<false, true>;
+    }
+    *smem = kBwdSmemFloats<false> * sizeof(float);
+    return p->planes_bf16 ? k_sample_backward<true, false> : k_sample_backward<false, false>;
 }
 
 }  // namespace
@@ -395,8 +411,8 @@ int render_backward_v1(const Geom& g, const p3d_render_params* p, const void* pl
     if (smem_ray > 48 * 1024) P3D_CUDA_TRY(cudaFuncSetAttribute(k_ray_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ray));
     k_ray_backward<<<(unsigned)((R + 3) / 4), 128, smem_ray, stream>>>(ra);
     P3D_LAUNCH_CHECK();
-    const size_t smem = kBwdSmemFloats * sizeof(float);
-    auto kern = p->planes_bf16 ? k_sample_backward<true> : k_sample_backward<false>;
+    size_t smem;
+    auto kern = sample_backward_kernel(g, p, &smem);
     P3D_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     for (int pass = 0; pass < 2; ++pass) {
         const int per_ray = pass == 0 ? g.S : g.Sf;
@@ -417,8 +433,8 @@ int decode_points_backward_v1(const Geom& g, const p3d_render_params* p, const v
                               const float* w2, const float* b2, const float* coords, long long n_pts, const float* g_rgb,
                               const float* g_sigma, float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2,
                               cudaStream_t stream) {
-    const size_t smem = kBwdSmemFloats * sizeof(float);
-    auto kern = p->planes_bf16 ? k_sample_backward<true> : k_sample_backward<false>;
+    size_t smem;
+    auto kern = sample_backward_kernel(g, p, &smem);
     P3D_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     SampleBwdArgs sa{};
     sa.g = g; sa.planes = planes; sa.w1 = w1; sa.b1 = b1; sa.w2 = w2; sa.b2 = b2;

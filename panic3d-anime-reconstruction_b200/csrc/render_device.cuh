@@ -148,8 +148,106 @@ __device__ __forceinline__ Tap4 plane_taps(const Geom& g, long long base, float2
     return t;
 }
 
+// -------------------------------------------------------------------------------------------
+// Multiplane tri-planes (triplane_depth D > 1).  renderer.py:84-94: each plane is a stack of D slabs sampled by a 5-D
+// grid_sample (trilinear, zero padding, align_corners=False).  project_onto_planes keeps all three components of
+// coordinates @ inv(plane_axes); the third indexes the slabs.  Slab d of plane p of a view starts at
+// p * stride_plane + d * H * stride_row.  The forward taps (plane_taps3) and the backward's texels (slab_texels) live side
+// by side here and come from one footprint, so the gradients land on exactly the texels and weights the forward read.
+// -------------------------------------------------------------------------------------------
+// The slab (normal-axis) coordinate of plane p: z, y, then x for P3D_PLANES_PANIC3D or y otherwise.
+__device__ __forceinline__ float plane_normal(const Geom& g, int p, float x, float y, float z) {
+    const bool pm = g.plane_mode == P3D_PLANES_PANIC3D;
+    return p == 0 ? z : (p == 1 ? y : (pm ? x : y));
+}
+
+// grid_sample's trilinear footprint: the bilinear one in the plane, and along the normal the first slab z0 with the weights
+// of slabs z0 and z0 + 1.  Slabs outside [0, D) contribute zero; a NaN or far-away normal coordinate gets z0 = -4.
+struct Footprint3 {
+    Footprint f;
+    int z0;
+    float wz0, wz1;
+};
+__device__ __forceinline__ Footprint3 trilinear_footprint(const Geom& g, float ca, float cb, float cn) {
+    Footprint3 t;
+    t.f = bilinear_footprint(g, ca, cb);
+    const float gz = __fmul_rn(cn, g.coord_scale);
+    const float fz = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)g.D), 1.f), 0.5f);
+    const bool sane = (fz > -2.f) && (fz < (float)g.D + 1.f);
+    const float z0f = floorf(fz);
+    t.wz1 = fz - z0f;
+    t.wz0 = 1.f - t.wz1;
+    t.z0 = sane ? (int)z0f : -4;
+    return t;
+}
+
+// the 8 taps of one plane: k & 3 is the bilinear tap of plane_taps, k >> 2 the slab (z0, then z0 + 1)
+struct Tap8 {
+    long long off[8];
+    float w[8];
+};
+__device__ __forceinline__ Tap8 plane_taps3(const Geom& g, long long base, float2 c, float cn) {
+    const Footprint3 t = trilinear_footprint(g, c.x, c.y, cn);
+    const long long slab = (long long)g.H * g.stride_row;
+    Tap8 r;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int xi = t.f.x0 + (k & 1), yi = t.f.y0 + ((k >> 1) & 1), zi = t.z0 + (k >> 2);
+        const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H) && (zi >= 0) && (zi < g.D);
+        const float wgt = ((k & 1) ? t.f.wx1 : t.f.wx0) * (((k >> 1) & 1) ? t.f.wy1 : t.f.wy0) * ((k >> 2) ? t.wz1 : t.wz0);
+        r.w[k] = ok ? wgt : 0.f;
+        r.off[k] = base + (ok ? (long long)zi * slab + (long long)yi * g.stride_row + (long long)xi * g.stride_col : 0ll);
+    }
+    return r;
+}
+
+// texel indices ((p * D + z) * H + y) * W + x in the backward's (N,3,D,H,W,C) gradient (or -1) and weights of plane p's taps,
+// in plane_taps3's order
+__device__ __forceinline__ void slab_texels(const Geom& g, int plane, float2 c, float cn, int2* out) {
+    const Footprint3 t = trilinear_footprint(g, c.x, c.y, cn);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int xi = t.f.x0 + (k & 1), yi = t.f.y0 + ((k >> 1) & 1);
+        const int z = t.z0 + (k >> 2);
+        const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H) && (z >= 0) && (z < g.D);
+        const float wgt = ((k & 1) ? t.f.wx1 : t.f.wx0) * (((k >> 1) & 1) ? t.f.wy1 : t.f.wy0) * ((k >> 2) ? t.wz1 : t.wz0);
+        out[k] = make_int2(ok ? ((plane * g.D + z) * g.H + yi) * g.W + xi : -1, __float_as_int(ok ? wgt : 0.f));
+    }
+}
+
+// channels [4q, 4q+4) of the plane mean at (x, y, z), trilinear per plane
 template <bool BF16>
+__device__ __forceinline__ float4 gather_features3(const void* planes, const Geom& g, int view, float x, float y, float z, int q) {
+    const long long vbase = (long long)view * g.stride_view + 4 * q;
+    float4 f[3];
+#pragma unroll
+    for (int p = 0; p < 3; ++p) {
+        const Tap8 t = plane_taps3(g, vbase + p * g.stride_plane, plane_coords(g, p, x, y, z), plane_normal(g, p, x, y, z));
+        float4 v[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = load_quad<BF16>(planes, t.off[k]);
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            a.x = fmaf(v[k].x, t.w[k], a.x);
+            a.y = fmaf(v[k].y, t.w[k], a.y);
+            a.z = fmaf(v[k].z, t.w[k], a.z);
+            a.w = fmaf(v[k].w, t.w[k], a.w);
+        }
+        f[p] = a;
+    }
+    float4 r;
+    r.x = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].x, f[1].x), f[2].x), 3.f);
+    r.y = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].y, f[1].y), f[2].y), 3.f);
+    r.z = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].z, f[1].z), f[2].z), 3.f);
+    r.w = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].w, f[1].w), f[2].w), 3.f);
+    return r;
+}
+
+// TRI: multiplane planes (Geom::D > 1), gather_features3; otherwise one slab per plane
+template <bool BF16, bool TRI = false>
 __device__ __forceinline__ float4 gather_features(const void* planes, const Geom& g, int view, float x, float y, float z, int q) {
+    if constexpr (TRI) return gather_features3<BF16>(planes, g, view, x, y, z, q);
     const long long vbase = (long long)view * g.stride_view + 4 * q;
     Tap4 t0 = plane_taps(g, vbase, plane_coords(g, 0, x, y, z));
     Tap4 t1 = plane_taps(g, vbase + g.stride_plane, plane_coords(g, 1, x, y, z));

@@ -27,6 +27,8 @@ struct Geom {
     int crop_on, cull_on, binarize_on;
     int force_sigmoid;
     float w1_gain, b1_gain, w2_gain, b2_gain;
+    int D;                    // slabs per plane (plane_depth; 1 unless multiplane).  Fills the padding before seed, so the
+                              // struct keeps its size and every other field its offset
     unsigned long long seed;
 };
 

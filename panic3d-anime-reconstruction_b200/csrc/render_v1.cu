@@ -50,7 +50,8 @@ enum { MODE_COARSE = 0, MODE_FINE = 1, MODE_POINTS = 2, MODE_VOLUME = 3 };
 // -------------------------------------------------------------------------------------------
 // k_sample_decode
 // -------------------------------------------------------------------------------------------
-template <int MODE, bool BF16>
+// TRI: multiplane tri-planes (g.D > 1), trilinear gather
+template <int MODE, bool BF16, bool TRI>
 __global__ void __launch_bounds__(kTile) k_sample_decode(const SampleArgs a) {
     __shared__ __align__(16) float s_w1[kHidden * kC];          // [j][k], gain folded in
     __shared__ __align__(16) float s_w2t[kHidden * kW2Stride];  // [j][m], gain folded in
@@ -100,7 +101,7 @@ __global__ void __launch_bounds__(kTile) k_sample_decode(const SampleArgs a) {
                 const float3 pt = ray_point(a.ro + ray * 3, a.rd + ray * 3, t);
                 px = pt.x; py = pt.y; pz = pt.z;
             }
-            f = gather_features<BF16>(a.planes, g, view, px, py, pz, q);
+            f = gather_features<BF16, TRI>(a.planes, g, view, px, py, pz, q);
         }
         float* dst = s_feat + local * kFeatStride + 4 * q;
         dst[0] = f.x; dst[1] = f.y; dst[2] = f.z; dst[3] = f.w;
@@ -320,8 +321,13 @@ int launch_sample_decode(const SampleArgs& a, bool bf16, cudaStream_t stream) {
     const long long blocks = (a.total + kTile - 1) / kTile;
     P3D_REQUIRE(blocks < (1ll << 31), "too many samples for one launch (%lld)", a.total);
     ProfileScope prof(PROF_SAMPLE_DECODE, stream);
-    if (bf16) k_sample_decode<MODE, true><<<(unsigned)blocks, kTile, 0, stream>>>(a);
-    else k_sample_decode<MODE, false><<<(unsigned)blocks, kTile, 0, stream>>>(a);
+    if (a.g.D > 1) {
+        if (bf16) k_sample_decode<MODE, true, true><<<(unsigned)blocks, kTile, 0, stream>>>(a);
+        else k_sample_decode<MODE, false, true><<<(unsigned)blocks, kTile, 0, stream>>>(a);
+    } else {
+        if (bf16) k_sample_decode<MODE, true, false><<<(unsigned)blocks, kTile, 0, stream>>>(a);
+        else k_sample_decode<MODE, false, false><<<(unsigned)blocks, kTile, 0, stream>>>(a);
+    }
     P3D_LAUNCH_CHECK();
     return P3D_OK;
 }

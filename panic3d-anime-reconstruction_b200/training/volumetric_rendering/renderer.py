@@ -57,6 +57,25 @@ def _decoder_params(decoder):
             bool(getattr(decoder, 'force_sigmoid', False)))
 
 
+def _multiplane_texels(planes: torch.Tensor, depth: int) -> torch.Tensor:
+    """(N,3,C*D,H,W) -> (N,3,D,H,W,C) contiguous: channel c*D + d of the input is feature c of slab d (the reference's
+    view as (N*3,C,D,H,W), renderer.py:84-94), laid out as the D slabs of channels-last texels p3d_render_params'
+    plane_depth addresses."""
+    N, P, CD, H, W = planes.shape
+    return planes.view(N, P, CD // depth, depth, H, W).permute(0, 1, 3, 4, 5, 2).contiguous()
+
+
+def _check_depth(planes: torch.Tensor, depth: int) -> int:
+    if depth < 1 or planes.shape[2] % depth:
+        raise ValueError(f'triplane_depth {depth} does not divide the {planes.shape[2]} plane channels')
+    if depth > 1 and planes.shape[2] // depth != 32:
+        # the kernels are built for 32 features per texel (p3d_render_params.channels); a multiplane model with another
+        # width per slab (e.g. triplane_width 16 at triplane_depth 2) has no accelerated path
+        raise NotImplementedError(f'triplane_depth {depth} splits {planes.shape[2]} plane channels into {planes.shape[2] // depth} '
+                                  'features per slab; multiplane tri-planes are rendered with 32 features per slab only')
+    return depth
+
+
 class _PlaneCache:
     """Channels-last copy of the most recent tri-plane tensor (keyed on storage + version), so the
     16 views of one subject (generate.py:108-130) pay for the layout pre-pass once."""
@@ -66,16 +85,44 @@ class _PlaneCache:
         self.buf = None
         self.src = None        # strong ref: while cached, the source storage cannot be freed and its address reused
 
-    def get(self, planes: torch.Tensor, bf16: bool):
-        key = (planes.data_ptr(), planes._version, tuple(planes.shape), tuple(planes.stride()), planes.device, bf16)
+    def get(self, planes: torch.Tensor, bf16: bool, depth: int = 1):
+        key = (planes.data_ptr(), planes._version, tuple(planes.shape), tuple(planes.stride()), planes.device, bf16, depth)
         if key != self.key:
-            N, P, Cc, H, W = planes.shape
-            src = planes if planes.is_contiguous() else planes.contiguous()
-            buf = torch.empty((N, P, H, W, Cc), device=planes.device, dtype=torch.bfloat16 if bf16 else torch.float32)
-            _lib.check(_lib.lib().p3d_planes_to_channels_last(src.data_ptr(), buf.data_ptr(), N * P, Cc, H, W,
-                                                             1 if bf16 else 0, _lib.stream_ptr(planes.device)))
+            if depth > 1:
+                buf = _multiplane_texels(planes, depth).to(torch.bfloat16 if bf16 else torch.float32)
+            else:
+                N, P, Cc, H, W = planes.shape
+                src = planes if planes.is_contiguous() else planes.contiguous()
+                buf = torch.empty((N, P, H, W, Cc), device=planes.device, dtype=torch.bfloat16 if bf16 else torch.float32)
+                _lib.check(_lib.lib().p3d_planes_to_channels_last(src.data_ptr(), buf.data_ptr(), N * P, Cc, H, W,
+                                                                 1 if bf16 else 0, _lib.stream_ptr(planes.device)))
             self.key, self.buf, self.src = key, buf, planes
         return self.buf
+
+
+def _fp32_texels(planes: torch.Tensor, p) -> torch.Tensor:
+    """The training path's fp32 channels-last copy of the planes, (N,3,H,W,C) or (N,3,D,H,W,C) for multiplane planes; the
+    backward scatters into a buffer of the same layout.  Sets the plane strides of p."""
+    src = planes.detach().float()
+    if p.plane_depth > 1:
+        planes_cl = _multiplane_texels(src, p.plane_depth)
+        sv, sp, _, sr, sc, _ = planes_cl.stride()
+    else:
+        planes_cl = torch.empty((p.n_views, 3, p.plane_h, p.plane_w, p.channels), device=planes.device, dtype=torch.float32)
+        srcc = src if src.is_contiguous() else src.contiguous()
+        _lib.check(_lib.lib().p3d_planes_to_channels_last(srcc.data_ptr(), planes_cl.data_ptr(), p.n_views * 3, p.channels,
+                                                         p.plane_h, p.plane_w, 0, _lib.stream_ptr(planes.device)))
+        sv, sp, sr, sc, _ = planes_cl.stride()
+    p.stride_view, p.stride_plane, p.stride_row, p.stride_col, p.planes_bf16 = sv, sp, sr, sc, 0
+    return planes_cl
+
+
+def _planes_grad(d_planes: torch.Tensor, dtype) -> torch.Tensor:
+    """(N,3,H,W,C) or (N,3,D,H,W,C) gradient of the texels -> the (N,3,C[*D],H,W) indexing of the input planes."""
+    if d_planes.dim() == 6:
+        N, P, D, H, W, Cc = d_planes.shape
+        return d_planes.permute(0, 1, 5, 2, 3, 4).reshape(N, P, Cc * D, H, W).to(dtype)
+    return d_planes.permute(0, 1, 4, 2, 3).to(dtype)
 
 
 class _RenderFunction(torch.autograd.Function):
@@ -88,14 +135,8 @@ class _RenderFunction(torch.autograd.Function):
         dev = planes.device
         L = _lib.lib()
         N, M = p.n_views, p.n_rays
-        # the backward scatters into a canonical (N,3,H,W,C) buffer, so the forward reads the same layout
-        src = planes.detach().float()
-        planes_cl = torch.empty((N, 3, p.plane_h, p.plane_w, p.channels), device=dev, dtype=torch.float32)
-        srcc = src if src.is_contiguous() else src.contiguous()
-        _lib.check(L.p3d_planes_to_channels_last(srcc.data_ptr(), planes_cl.data_ptr(), N * 3, p.channels, p.plane_h, p.plane_w, 0,
-                                                 _lib.stream_ptr(dev)))
-        sv, sp, sr, sc, _ = planes_cl.stride()
-        p.stride_view, p.stride_plane, p.stride_row, p.stride_col, p.planes_bf16 = sv, sp, sr, sc, 0
+        # the backward scatters into a canonical (N,3,[D,]H,W,C) buffer, so the forward reads the same layout
+        planes_cl = _fp32_texels(planes, p)
         p.mlp_mode = _lib.P3D_MLP_FP32_SIMT
         wt = [t.detach().float().contiguous() for t in (w1, b1, w2, b2)]
         ro, rd = ro.detach().float().contiguous(), rd.detach().float().contiguous()
@@ -133,7 +174,7 @@ class _RenderFunction(torch.autograd.Function):
                                              scratch.data_ptr(), scratch.numel(), d_planes.data_ptr(), *[t.data_ptr() for t in d_w],
                                              _lib.stream_ptr(dev)))
         dts = ctx.in_dtypes
-        return (None, d_planes.permute(0, 1, 4, 2, 3).to(dts[0]), d_w[0].to(dts[1]), d_w[1].to(dts[2]), d_w[2].to(dts[3]),
+        return (None, _planes_grad(d_planes, dts[0]), d_w[0].to(dts[1]), d_w[1].to(dts[2]), d_w[2].to(dts[3]),
                 d_w[3].to(dts[4]), None, None, None, None)
 
 
@@ -148,13 +189,7 @@ class _PointsFunction(torch.autograd.Function):
         dev = planes.device
         L = _lib.lib()
         N, K = coords.shape[0], coords.shape[1]
-        src = planes.detach().float()
-        srcc = src if src.is_contiguous() else src.contiguous()
-        planes_cl = torch.empty((N, 3, p.plane_h, p.plane_w, p.channels), device=dev, dtype=torch.float32)
-        _lib.check(L.p3d_planes_to_channels_last(srcc.data_ptr(), planes_cl.data_ptr(), N * 3, p.channels, p.plane_h, p.plane_w, 0,
-                                                 _lib.stream_ptr(dev)))
-        sv, sp, sr, sc, _ = planes_cl.stride()
-        p.stride_view, p.stride_plane, p.stride_row, p.stride_col, p.planes_bf16 = sv, sp, sr, sc, 0
+        planes_cl = _fp32_texels(planes, p)
         wt = [t.detach().float().contiguous() for t in (w1, b1, w2, b2)]
         coords = coords.detach().float().contiguous()
         rgb = torch.empty((N, K, p.out_dim - 1), device=dev, dtype=torch.float32)
@@ -181,7 +216,7 @@ class _PointsFunction(torch.autograd.Function):
                                                     b2.data_ptr(), coords.data_ptr(), K, g_rgb.data_ptr(), g_sigma.data_ptr(),
                                                     d_planes.data_ptr(), *[t.data_ptr() for t in d_w], _lib.stream_ptr(dev)))
         dts = ctx.in_dtypes
-        return (d_planes.permute(0, 1, 4, 2, 3).to(dts[0]), d_w[0].to(dts[1]), d_w[1].to(dts[2]), d_w[2].to(dts[3]), d_w[3].to(dts[4]),
+        return (_planes_grad(d_planes, dts[0]), d_w[0].to(dts[1]), d_w[1].to(dts[2]), d_w[2].to(dts[3]), d_w[3].to(dts[4]),
                 None, None)
 
 
@@ -208,8 +243,6 @@ class ImportanceRenderer(torch.nn.Module):
 
     # ------------------------------------------------------------------ helpers
     def _params(self, planes_cl, N, M, opts, decoder, triplane_crop, cull_clouds, binarize_clouds, n_points=None):
-        if int(opts.get('triplane_depth', 1)) != 1:
-            raise NotImplementedError('triplane_depth > 1 (multiplane) is outside the accelerated path')
         if opts.get('density_noise', 0) > 0:
             raise NotImplementedError('density_noise > 0 is outside the accelerated path')
         if opts.get('clamp_mode', 'softplus') != 'softplus':
@@ -219,11 +252,17 @@ class ImportanceRenderer(torch.nn.Module):
         p.n_views, p.n_rays = N, M
         p.n_coarse = int(opts.get('depth_resolution', 2))
         p.n_fine = int(opts.get('depth_resolution_importance', 0) or 0)
-        _, _, H, W, Cc = planes_cl.shape
+        if planes_cl.dim() == 6:                         # multiplane (N,3,D,H,W,C): slab d at d * H * stride_row
+            _, _, D, H, W, Cc = planes_cl.shape
+            sv, sp, ss, sr, sc, s1 = planes_cl.stride()
+            assert ss == H * sr
+            p.plane_depth = D
+        else:
+            _, _, H, W, Cc = planes_cl.shape
+            sv, sp, sr, sc, s1 = planes_cl.stride()
+        assert s1 == 1
         p.channels, p.plane_h, p.plane_w = Cc, H, W
         p.hidden, p.out_dim = w1.shape[0], w2.shape[0]
-        sv, sp, sr, sc, s1 = planes_cl.stride()
-        assert s1 == 1
         p.stride_view, p.stride_plane, p.stride_row, p.stride_col = sv, sp, sr, sc
         p.planes_bf16 = 1 if planes_cl.dtype == torch.bfloat16 else 0
         p.box_warp = float(opts['box_warp'])
@@ -251,15 +290,26 @@ class ImportanceRenderer(torch.nn.Module):
         p.seed = int(torch.empty((), dtype=torch.int64).random_().item()) & 0xFFFFFFFFFFFFFFFF
         return p, (w1, b1, w2, b2)
 
-    def _planes_cl(self, planes: torch.Tensor) -> torch.Tensor:
+    def _planes_cl(self, planes: torch.Tensor, depth: int = 1) -> torch.Tensor:
+        """Channels-last texels of (N,3,C*depth,H,W) planes: (N,3,H,W,C), or (N,3,depth,H,W,C) for multiplane planes."""
         if planes.dim() != 5 or planes.shape[1] != 3:
             raise ValueError(f'planes must be (N,3,C,H,W), got {tuple(planes.shape)}')
+        depth = _check_depth(planes, depth)
         want = torch.bfloat16 if self.planes_bf16 else torch.float32
+        if depth > 1:
+            return self._planes.get(planes if planes.dtype == torch.float32 else planes.float(), self.planes_bf16, depth)
         if planes.stride(2) == 1 and planes.dtype == want:
             return planes.permute(0, 1, 3, 4, 2)            # already channels-last texels: zero-copy view
         if planes.dtype != torch.float32:
             planes = planes.float()
         return self._planes.get(planes, self.planes_bf16)
+
+    @staticmethod
+    def _shape_probe(planes: torch.Tensor, opts) -> torch.Tensor:
+        """A meta tensor with the shape of _planes_cl's result, for _params on the autograd paths."""
+        N, _, CD, H, W = planes.shape
+        D = _check_depth(planes, int(opts.get('triplane_depth', 1)))
+        return torch.empty((N, 3, D, H, W, CD // D) if D > 1 else (N, 3, H, W, CD), device='meta')
 
     @staticmethod
     def _require_cuda(*tensors):
@@ -285,7 +335,7 @@ class ImportanceRenderer(torch.nn.Module):
             return self._forward_autograd(planes, decoder, ray_origins, ray_directions, rendering_options, triplane_crop,
                                           cull_clouds, binarize_clouds)
         with torch.cuda.device(dev):
-            planes_cl = self._planes_cl(planes.detach())
+            planes_cl = self._planes_cl(planes.detach(), int(rendering_options.get('triplane_depth', 1)))
             p, (w1, b1, w2, b2) = self._params(planes_cl, N, M, rendering_options, decoder, triplane_crop, cull_clouds,
                                                binarize_clouds)
             ro = ray_origins.detach().float().contiguous()
@@ -341,7 +391,7 @@ class ImportanceRenderer(torch.nn.Module):
         if planes.dim() != 5 or planes.shape[1] != 3:
             raise ValueError(f'planes must be (N,3,C,H,W), got {tuple(planes.shape)}')
         with torch.cuda.device(dev):
-            shape_probe = torch.empty((N, 3, planes.shape[3], planes.shape[4], planes.shape[2]), device='meta')
+            shape_probe = self._shape_probe(planes, rendering_options)
             p, (w1, b1, w2, b2) = self._params(shape_probe, N, M, rendering_options, decoder, triplane_crop, cull_clouds, binarize_clouds)
             p.defer_depth_clamp = 1 if self.depth_bounds_reduce is not None else 0
             return _RenderFunction.apply(self, planes, w1, b1, w2, b2, ray_origins, ray_directions, p, self._noise(dev, N, M, p))
@@ -361,14 +411,14 @@ class ImportanceRenderer(torch.nn.Module):
             with torch.cuda.device(dev):
                 opts = dict(options)
                 opts.setdefault('depth_resolution', 2)
-                shape_probe = torch.empty((N, 3, planes.shape[3], planes.shape[4], planes.shape[2]), device='meta')
+                shape_probe = self._shape_probe(planes, opts)
                 p, (w1, b1, w2, b2) = self._params(shape_probe, N, 0, opts, decoder, None, None, None)
                 rgb, sigma = _PointsFunction.apply(planes, w1, b1, w2, b2, sample_coordinates, p)
             return {'rgb': rgb, 'sigma': sigma, 'xyz': sample_coordinates}
         with torch.cuda.device(dev):
-            planes_cl = self._planes_cl(planes.detach())
             opts = dict(options)
             opts.setdefault('depth_resolution', 2)
+            planes_cl = self._planes_cl(planes.detach(), int(opts.get('triplane_depth', 1)))
             p, (w1, b1, w2, b2) = self._params(planes_cl, N, 0, opts, decoder, None, None, None, n_points=N * K)
             coords = sample_coordinates.detach().float().contiguous()
             rgb = torch.empty((N, K, p.out_dim - 1), device=dev, dtype=torch.float32)

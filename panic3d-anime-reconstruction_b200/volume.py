@@ -60,7 +60,7 @@ def query_volume(planes, decoder, rendering_kwargs, resolution=256, triplane_cro
     dev = planes.device
     N, R = planes.shape[0], int(resolution)
     with torch.no_grad(), torch.cuda.device(dev):
-        planes_cl = r._planes_cl(planes.detach())
+        planes_cl = r._planes_cl(planes.detach(), int(rendering_kwargs.get('triplane_depth', 1)))
         opts = dict(rendering_kwargs)
         opts.setdefault('depth_resolution', 2)
         p, wts = r._params(planes_cl, N, 0, opts, decoder, None, None, None, n_points=N * int(resolution) ** 3)
