@@ -358,6 +358,22 @@ inline int sm_count(int* n) {
     *n = n_sm;
     return P3D_OK;
 }
+// cudaFuncAttributePreferredSharedMemoryCarveout for a kernel with `smem` bytes of dynamic shared memory: the share, in percent
+// of the SM's shared-memory maximum, that `smem` and the per-CTA reservation take, rounded down.  The driver rounds the hint
+// up to a carve-out that holds the CTA, so this selects the smallest one that does and leaves the rest of the SM's
+// 256 KB to L1, instead of leaving the split to the driver.
+inline int smem_carveout_percent(size_t smem, int* pct) {
+    static int max_sm = 0, reserved = 0;
+    if (!max_sm) {
+        int dev = 0;
+        P3D_CUDA_TRY(cudaGetDevice(&dev));
+        P3D_CUDA_TRY(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+        P3D_CUDA_TRY(cudaDeviceGetAttribute(&max_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+    }
+    const long long share = 100ll * ((long long)smem + reserved) / max_sm;
+    *pct = (int)(share < 1 ? 1 : (share > 100 ? 100 : share));
+    return P3D_OK;
+}
 // The texel stride the gather takes as a template argument (SCOL): kC (the layout pre-pass: one plane's texels contiguous),
 // 3 kC (a (N,96,H,W) channels_last backbone output consumed zero-copy) or 0 (any other stride, read at run time).
 // pick(std::integral_constant<int, SCOL>) returns the kernel instantiation.

@@ -36,14 +36,14 @@ using namespace fused;
 constexpr int kGW = 12, kEW = 8, kRW = 4, kTeams = 3;   // 24 warps = 6 warpgroups -> 80 registers per thread
 constexpr int kWarpsWS = kGW + kEW + kRW;
 constexpr int kThreadsWS = kWarpsWS * 32;        // 768
-constexpr int kNA = 4;                           // A1 ring depth
+constexpr int kNA = 3;                           // A1 ring depth: one stage per gather team
 // registers per thread by role (launched with 80 = 65536 / 768 rounded down to 8): the decoder warpgroups hold the layer-2
 // A operands and accumulators at once and take what the ray warpgroup does not need; 3 x 80 + 2 x kRegE + kRegR <= 6 x 80
 constexpr int kRegE = 88, kRegR = 64;
 static_assert(3 * 80 + 2 * kRegE + kRegR <= 6 * 80, "per-role registers exceed what the launch allocates");
 constexpr int kStates = 4;                       // per-group state ring
 constexpr int kRowsG = 384;                      // rows per pass per group
-constexpr int kColBufs = 3;                      // colour tiles of a group in shared memory at once (colours())
+constexpr int kColBufs = 2;                      // colour tiles of a group in shared memory at once (colours())
 constexpr int kHalfBytes = 64 * kRgb * 4;        // one decoder warpgroup's 64 rows of colour sigmoids: 8 KB
 
 
@@ -79,7 +79,12 @@ struct __align__(1024) WsSmem {
 // conflict-free.  The colour areas in global memory are byte copies of the tiles, so they hold the same layout.
 __device__ __forceinline__ int col_idx(int row, int c) { return row * kRgb + ((((c >> 2) ^ row) & 7) << 2) + (c & 3); }
 
-static_assert(sizeof(WsSmem) + 1024 <= 232448, "WsSmem + alignment slack exceeds the 227 KB a CTA can opt into");
+// Shared memory and L1 share 256 KB per SM.  At most 196 KB of shared memory (199,680 B for the CTA after the 1 KB the
+// system reserves) leaves 60 KB of L1 instead of the 28 KB of the largest carve-out: the gather's texel loads land in L1
+// while they are in flight, so L1 bounds how much of that traffic each SM keeps outstanding.  That is what the A1 ring
+// (one stage per team) and kColBufs (two colour tiles) are sized for.
+constexpr int kSmemWS = (int)sizeof(WsSmem) + 1024;                  // + alignment slack of the extern array
+static_assert(kSmemWS <= 199680, "WsSmem + alignment slack exceeds the 196 KB shared-memory carve-out");
 
 struct WsArgs {
     Geom g;
@@ -610,12 +615,15 @@ int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const vo
     }
     int n_sm;
     if ((rc = sm_count(&n_sm))) return rc;
-    const size_t smem = sizeof(WsSmem) + 1024;
+    const size_t smem = kSmemWS;
     void (*kern)(WsArgs) = with_texel_stride(g, [&](auto sc) -> void (*)(WsArgs) {
         if (g.S == 96) return p->planes_bf16 ? k_render_ws3<true, 96, sc.value> : k_render_ws3<false, 96, sc.value>;
         return p->planes_bf16 ? k_render_ws3<true, 48, sc.value> : k_render_ws3<false, 48, sc.value>;
     });
     P3D_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int carveout;
+    if ((rc = smem_carveout_percent(smem, &carveout))) return rc;
+    P3D_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
     const int grid = a.n_groups < n_sm ? a.n_groups : n_sm;
     {
         ProfileScope prof(PROF_FUSED, stream);
