@@ -4,7 +4,7 @@ fails it, as it must.  The tree is not modified.
 
     python tests/run_mutations.py TARGET [TARGET ...] [--files F ...] [--json out.json] [--build-only]
 
-TARGET is one of decode_tc, paste_front, render_backward, modconv, render_fused.  --files runs other GPU files against the same mutants
+TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane, modconv, render_fused.  --files runs other GPU files against the same mutants
 instead (to see which of them the rest of the suite catches); the exit code then only reports that the run completed.
 --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
 """
@@ -75,6 +75,14 @@ RENDER_BACKWARD = {
     'omega without its 1/2': ('om = 0.5f * (wl + wr);', 'om = (wl + wr);'),
 }
 
+# render_backward.cu, the multiplane (TRI) lines of k_sample_backward: value mutations that keep every access in bounds (the
+# view offset without D only shrinks it, the scatter bound only drops taps, the normal stays bounds-checked in slab_texels).
+RENDER_BACKWARD_MULTIPLANE = {
+    'per-view gradient offset without D': ('(long long)3 * (TRI ? g.D : 1) * g.H', '(long long)3 * g.H'),
+    'scatter stopped after the first 12 of 24 taps': ('for (int k = 0; k < NT; ++k) {', 'for (int k = 0; k < 12; ++k) {'),
+    'slab taps from the next plane\'s normal': ('plane_normal(g, qd, px, py, pz), s_tap', 'plane_normal(g, (qd + 1) % 3, px, py, pz), s_tap'),
+}
+
 # modconv.cu: every mutation keeps all memory accesses in bounds.
 MODCONV = {
     'demod epsilon dropped': ('block_reduce(ss, false, red) + 1e-8f', 'block_reduce(ss, false, red)'),
@@ -108,6 +116,7 @@ TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
     'paste_front': ('paste_front.cu', 'tests/test_paste_paths_gpu.py', PASTE_FRONT),
     'render_backward': ('render_backward.cu', 'tests/test_render_backward_paths_gpu.py', RENDER_BACKWARD),
+    'render_backward_multiplane': ('render_backward.cu', 'tests/test_multiplane_paths_gpu.py', RENDER_BACKWARD_MULTIPLANE),
     'modconv': ('modconv.cu', 'tests/test_modconv_gpu.py', MODCONV),
     'render_fused': ('render_fused_ws3.cu', 'tests/test_render_fused_paths_gpu.py', RENDER_FUSED),
 }

@@ -1,14 +1,16 @@
-"""Mutation check of tests/test_multiplane_gpu.py (needs an H100): build libp3d.so once per single-line value mutation of the
-multiplane section of csrc/render_device.cuh into a temporary directory, run the GPU test file against it (P3D_LIBP3D),
-and report whether the file fails it, as it must.  The tree is not modified.
+"""Mutation check of the multiplane GPU tests (needs an H100): build libp3d.so once per single-line value mutation of the
+multiplane section of csrc/render_device.cuh into a temporary directory, run tests/test_multiplane_paths_gpu.py against it
+(P3D_LIBP3D), and report whether the file fails it, as it must.  The tree is not modified.
 
-    python tests/run_mutations_multiplane.py [--json out.json] [--build-only]
+    python tests/run_mutations_multiplane.py [--files F ...] [--json out.json] [--build-only]
 
 The mutated code is a header, so each mutant recompiles every translation unit that includes it directly (render_v1.cu,
 render_backward.cu, marching_cubes.cu) from a copy next to the mutated header, where its #include "render_device.cuh"
 finds the mutant first.  The fused kernels reach the header through fused_common.cuh but call none of the multiplane
-functions, so their objects are the tree's.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs
-no GPU.  tests/run_mutations.py is the driver for the other kernel files.
+functions, so their objects are the tree's.  --files runs other GPU files against the same mutants instead (to see which
+of them tests/test_multiplane_gpu.py catches); the exit code then only reports that the run completed.  --build-only builds
+every mutant and stops; nvcc cross-compiles, so it needs no GPU.  tests/run_mutations.py is the driver for the other kernel
+files (its render_backward_multiplane target mutates the TRI lines of render_backward.cu).
 """
 import argparse
 import json
@@ -23,10 +25,11 @@ sys.path.insert(0, ROOT)
 from panic3d_b200 import _build  # noqa: E402
 
 HEADER = 'render_device.cuh'
-TEST_FILE = 'tests/test_multiplane_gpu.py'
+TEST_FILE = 'tests/test_multiplane_paths_gpu.py'
 
 # Value mutations; every index they produce is still checked against its bound before it addresses memory, except the slab
-# stride from W, which stays in bounds because every plane of the test file has H > W.
+# stride from W, which stays in bounds because every plane of both multiplane GPU files has H >= W.  No tap count, shared
+# memory size or tap-table stride is mutated: an unwritten s_tap entry would send the backward's atomics out of bounds.
 MUTATIONS = {
     'slab coordinate with align_corners=True': (
         'const float fz = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)g.D), 1.f), 0.5f);',
@@ -37,6 +40,11 @@ MUTATIONS = {
     'backward scatters to one slab only': ('const int z = t.z0 + (k >> 2);', 'const int z = t.z0;'),
     'slab offset from plane_w instead of plane_h': ('const long long slab = (long long)g.H * g.stride_row;',
                                                     'const long long slab = (long long)g.W * g.stride_row;'),
+    # the backward's weight of slab z0 + 1 (slab_texels; the same line in plane_taps3 is followed by `r.w[k]`)
+    'backward weight of slab z0 + 1 taken as z0\'s': ('t.wz1 : t.wz0);\n        out[k]', 't.wz0 : t.wz0);\n        out[k]'),
+    # the normal's zero-padding bands dropped: a point within a slab below slab 0 (or above slab D - 1) reads nothing
+    'zero-padding band below slab 0 dropped': ('(fz > -2.f) &&', '(fz >= 0.f) &&'),
+    'zero-padding band above slab D - 1 dropped': ('(fz < (float)g.D + 1.f)', '(fz < (float)(g.D - 1))'),
 }
 
 
@@ -73,6 +81,7 @@ def build_mutant(nvcc, d, name):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--files', nargs='+')
     ap.add_argument('--json')
     ap.add_argument('--build-only', action='store_true')
     args = ap.parse_args()
@@ -89,7 +98,7 @@ def main():
             return
         for name, lib in zip(names, libs):
             r = subprocess.run([sys.executable, '-m', 'pytest', '-q', '-x', '-m', 'gpu', '-p', 'no:cacheprovider',
-                                os.path.join(ROOT, TEST_FILE)], cwd=ROOT, env=dict(os.environ, P3D_LIBP3D=lib),
+                               ] + [os.path.join(ROOT, f) for f in args.files or [TEST_FILE]], cwd=ROOT, env=dict(os.environ, P3D_LIBP3D=lib),
                                stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
             failed = [ln for ln in r.stdout.splitlines() if ln.startswith('FAILED') or ln.startswith('ERROR')]
             results[name] = {'killed': r.returncode != 0, 'failures': failed, 'summary': r.stdout.strip().splitlines()[-1]}
@@ -98,7 +107,7 @@ def main():
                 print(f'    {ln[:160]}', flush=True)
     if args.json:
         json.dump(results, open(args.json, 'w'), indent=1)
-    sys.exit(0 if all(v['killed'] for v in results.values()) else 1)
+    sys.exit(0 if args.files or all(v['killed'] for v in results.values()) else 1)
 
 
 if __name__ == '__main__':

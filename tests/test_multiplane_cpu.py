@@ -197,6 +197,120 @@ def test_multiplane_mutation_table_applies_to_the_current_header():
     assert {os.path.basename(s) for s in including_units()} >= {'render_v1.cu', 'render_backward.cu'}
 
 
+# ------------------------------------------------------------------------------ the hand-written backward's multiplane taps
+BWD_FLAGS = {'crop_cull': dict(triplane_crop=0.1, cull_clouds=0.5), 'binarize': dict(triplane_crop=0.1, binarize_clouds=0.5)}
+
+
+def _bwd_inputs(D, use_triplane, seed=7, N=2, R=6, S=12, Sf=12, P=16):
+    """renderer_oracle.synth_inputs' decoder and rays, with planes of D slabs ((N, 3, 32*D, P, P); the same planes as
+    tests/test_render_backward_oracle_cpu.py at D = 1)."""
+    opts = dict(orc.DEFAULT_OPTS, depth_resolution=S, depth_resolution_importance=Sf, triplane_depth=D)
+    planes, dec, c2w, K, u_c, u_f = orc.synth_inputs(seed, N, R, S, Sf, P)
+    if D > 1:
+        planes = torch.from_numpy(np.random.default_rng(seed + 100).standard_normal((N, 3, 32 * D, P, P), dtype=np.float32))
+    dec = dict(dec, b2=dec['b2'].clone())
+    dec['b2'][0] += 1.0                        # sigma around the cull threshold
+    ro, rd = orc.ray_sampler(c2w, K, R)
+    rng = np.random.default_rng(seed + 1)
+    grads = [torch.from_numpy(rng.standard_normal(s)) for s in ((N, R * R, 32), (N, R * R, 1), (N, R * R, 1), (N, R * R, 3))]
+    return planes, dec, ro, rd, opts, u_c, u_f, grads
+
+
+def _oracle(D):
+    """The render oracle for planes of D slabs: at D = 1 the reference's one-slab lookup, not a 5-D grid_sample over one slab."""
+    return mo if D > 1 else orc
+
+
+def _dec64(dec, grad=False):
+    return {k: (v.double().requires_grad_(grad) if torch.is_tensor(v) else v) for k, v in dec.items()}
+
+
+@pytest.mark.parametrize('flags', sorted(BWD_FLAGS))
+@pytest.mark.parametrize('use_triplane', [True, False])
+@pytest.mark.parametrize('D', [1, 2, 3])
+def test_hand_written_backward_with_slabs_equals_fp64_autograd(D, use_triplane, flags):
+    """render_backward(depth=D) equals torch's fp64 autograd of multiplane_oracle.render fed the fp32 run's depths and
+    masks, to 1e-10 of each tensor's largest element, and its magnitude run bounds it."""
+    from oracle import render_backward_oracle as rbo
+    planes, dec, ro, rd, opts, u_c, u_f, grads = _bwd_inputs(D, use_triplane)
+    kw = dict(use_triplane=use_triplane, **BWD_FLAGS[flags])
+    _, smp = _oracle(D).render(planes, dec, ro, rd, opts, u_c, u_f, return_samples=True, **kw)
+    m = torch.cat([smp['masks'][0].reshape(-1), smp['masks'][1].reshape(-1)])
+    assert 0 < m.float().mean() < 1, 'the masks both keep and remove samples'
+    p64, d64 = planes.double().requires_grad_(True), _dec64(dec, True)
+    out = _oracle(D).render(p64, d64, ro, rd, opts, None, None, depths=smp['depths'], masks=smp['masks'], **kw)
+    ref = torch.autograd.grad(sum((o * g).sum() for o, g in zip(out, grads)), [p64] + [d64[k] for k in ('w1', 'b1', 'w2', 'b2')])
+    got = rbo.render_backward(planes.double(), _dec64(dec), ro, rd, opts, smp['depths'], smp['masks'], grads, depth=D, **kw)
+    A = rbo.render_backward(planes.double(), _dec64(dec), ro, rd, opts, smp['depths'], smp['masks'], grads, mag=True, c=1e30,
+                            depth=D, **kw)
+    for key, r in zip(('planes', 'w1', 'b1', 'w2', 'b2'), ref):
+        assert got[key].shape == r.shape, key
+        err = (got[key] - r).abs().max().item()
+        assert err <= 1e-10 * r.abs().max().item(), (key, err)
+        assert (r.abs() <= A[key] * (1 + 1e-12) + 1e-300).all(), key
+    assert (ref[0] != 0).any() and (ref[0] == 0).any()
+
+
+@pytest.mark.parametrize('use_triplane', [True, False])
+@pytest.mark.parametrize('D', [1, 2, 3])
+def test_points_backward_with_slabs_equals_fp64_autograd(D, use_triplane):
+    """points_backward(depth=D) is the gradient of multiplane_oracle.run_model's sigma, on points that include slab centres,
+    slab borders and points past the box along each normal; sigma_error_bound(depth=D) bounds the fp32 oracle's sigma."""
+    from oracle import render_backward_oracle as rbo
+    from tests.golden.cases_multiplane import slab_points
+    planes, dec, *_ = _bwd_inputs(D, use_triplane)
+    g = torch.Generator().manual_seed(3)
+    xyz = torch.cat([(torch.rand(2, 300, 3, generator=g) * 2 - 1) * 0.4,
+                     torch.from_numpy(slab_points(max(D, 2), use_triplane)).expand(2, -1, -1)], 1).contiguous()
+    g_sigma = torch.randn(2, xyz.shape[1], generator=g, dtype=torch.float64)
+    opts = dict(orc.DEFAULT_OPTS, triplane_depth=D)
+    p64, d64 = planes.double().requires_grad_(True), _dec64(dec, True)
+    ref = torch.autograd.grad((_oracle(D).run_model(p64, d64, xyz, opts, use_triplane)[1] * g_sigma[..., None]).sum(),
+                              [p64] + [d64[k] for k in ('w1', 'b1', 'w2', 'b2')])
+    bw = opts['box_warp']
+    got = rbo.points_backward(planes.double(), _dec64(dec), xyz, g_sigma, bw, use_triplane, depth=D)
+    A = rbo.points_backward(planes.double(), _dec64(dec), xyz, g_sigma, bw, use_triplane, mag=True, c=1e30, depth=D)
+    for key, r in zip(('planes', 'w1', 'b1', 'w2', 'b2'), ref):
+        assert (got[key] - r).abs().max().item() <= 1e-10 * r.abs().max().item(), key
+        assert (r.abs() <= A[key] * (1 + 1e-12) + 1e-300).all(), key
+    bound = rbo.sigma_error_bound(planes[0].double(), _dec64(dec), xyz[0], bw, use_triplane, depth=D)
+    s32 = _oracle(D).run_model(planes[:1], dec, xyz[:1], opts, use_triplane)[1]
+    s64 = _oracle(D).run_model(planes[:1].double(), _dec64(dec), xyz[:1], opts, use_triplane)[1]
+    assert ((s32.double() - s64)[0, :, 0].abs() <= bound).all(), 'the fp32 oracle is within the fp32 decode bound'
+
+
+@pytest.mark.parametrize('gather', ['manual', 'aten'])
+@pytest.mark.parametrize('use_triplane', [True, False])
+@pytest.mark.parametrize('D', [2, 3])
+def test_taps_weighted_sum_equals_sample_multiplane(D, use_triplane, gather):
+    """The 24 taps of render_backward_oracle.taps, summed with their weights over the texels of render_backward_oracle.texels,
+    are sample_multiplane's features; texel_counts counts exactly the in-bounds taps."""
+    from oracle import render_backward_oracle as rbo
+    from tests.golden.cases_multiplane import slab_points
+    planes, _, ro, rd, opts, u_c, _, _ = _bwd_inputs(D, use_triplane)
+    g = torch.Generator().manual_seed(11)
+    xyz = torch.cat([(torch.rand(1, 500, 3, generator=g) * 2 - 1) * 0.45,
+                     torch.from_numpy(slab_points(D, use_triplane))[None]], 1)
+    idx, wgt = rbo.taps(xyz[0], 16, 16, opts['box_warp'], use_triplane, D)
+    assert idx.shape == (xyz.shape[1], 24) and int(idx.max()) < 3 * D * 16 * 16
+    p64 = planes[:1].double()
+    got = rbo.gather(rbo.texels(p64[0], D), idx, wgt)                                     # (K,3,C)
+    # the manual gather takes the same fp32 footprint (fp64 sums); aten's grid_sample wants one dtype, so it runs in fp64
+    # from the fp32 points and differs by the footprint's fp32 rounding
+    xyz_g = xyz if gather == 'manual' else xyz.double()
+    want = mo.sample_multiplane(p64, xyz_g, opts['box_warp'], use_triplane, D, gather)[0]  # (3,K,C)
+    assert (got - want.permute(1, 0, 2)).abs().max().item() <= (1e-12 if gather == 'manual' else 1e-5)
+    # every slab is reached
+    z = (idx[idx >= 0] // (16 * 16)) % D
+    assert set(z.tolist()) == set(range(D))
+    d_c = orc.stratified_depths(u_c, opts['ray_start'], opts['ray_end'])
+    cnt = rbo.texel_counts(ro, rd, (d_c, None), 16, 16, opts['box_warp'], use_triplane, D)
+    assert cnt.shape == (2, 3, D, 16, 16)
+    for n in range(2):
+        xyz_n = (ro[n, :, None] + d_c[n, ..., 0, None] * rd[n, :, None]).reshape(-1, 3)
+        assert cnt[n].sum().item() == (rbo.taps(xyz_n, 16, 16, opts['box_warp'], use_triplane, D)[0] >= 0).sum().item()
+
+
 def test_oracle_sampling_is_scoped():
     """multiplane_oracle.sampling replaces the renderer oracle's plane lookup for its block only, also when it raises."""
     one_slab = orc.sample_planes
