@@ -47,6 +47,34 @@ constexpr int kColBufs = 2;                      // colour tiles of a group in s
 constexpr int kHalfBytes = 64 * kRgb * 4;        // one decoder warpgroup's 64 rows of colour sigmoids: 8 KB
 
 
+// Per-role cycle accounting, compiled in only with -DP3D_WS3_ROLE_CLOCKS (bench_roles.py): lane 0 of every warp adds
+// clock64() deltas into per-CTA counters [role][slot] in shared memory, which the CTA adds into WsArgs::role_clk
+// ([CTA][kRoles][kRcSlots], accumulated over launches) at its end.  RC_* slots 1-7 are mbarrier waits, the rest phases of work;
+// a role's remainder (RC_TOTAL minus the slots it uses) is untimed bookkeeping.  The default build has no clock reads.
+enum RoleClk {
+    RC_TOTAL, RC_A1_FULL, RC_A1_EMPTY, RC_STATE_FREE, RC_FINE_READY, RC_SIG_READY, RC_OMEGA_READY, RC_COL_FULL,
+    RC_COLOURS, RC_L1, RC_HIDDEN, RC_L2, RC_EPILOGUE,         // decoder phases (colours() includes its omega / col_full waits)
+    RC_TAPS, RC_GATHER,                                       // gather phases: tap table, loads + lerp into the A1 stage
+    RC_IMPORTANCE,                                            // ray phases: importance sampling (composite = the rest)
+    kRcSlots
+};
+#ifdef P3D_WS3_ROLE_CLOCKS
+constexpr int kRoles = 3;                                     // 0 gather, 1 decoder, 2 ray
+#define RC_BEGIN(v) const long long v = clock64()
+#define RC_END(role, slot, v) do { if (lane == 0) atomicAdd(&sm.rclk[role][slot], (unsigned long long)(clock64() - (v))); } while (0)
+// ties register values computed by plain arithmetic to the clock read after them (the compiler may otherwise sink them)
+__device__ __forceinline__ void rc_fence_regs(uint32_t (&x)[16], uint32_t (&y)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) asm volatile("" : "+r"(x[i]), "+r"(y[i])::"memory");
+}
+#define RC_FENCE_REGS(x, y) rc_fence_regs(x, y)
+#else
+#define RC_BEGIN(v) do {} while (0)
+#define RC_END(role, slot, v) do {} while (0)
+#define RC_FENCE_REGS(x, y) do {} while (0)
+#endif
+#define RC_WAIT(role, slot, bar, par) do { RC_BEGIN(rc_t_); mbar_wait(bar, par); RC_END(role, slot, rc_t_); } while (0)
+
 struct GroupState {                               // written by G (t_c, crop), E (sg_*), R (t_f)
     float t_c[kRowsG], sg_c[kRowsG], t_f[kRowsG], sg_f[kRowsG];
     unsigned char crop[2][kRowsG];
@@ -72,6 +100,9 @@ struct __align__(1024) WsSmem {
     unsigned long long fine_ready[kStates], state_free[kStates];
     unsigned long long sigc_ready[kStates], sigf_ready[kStates], omega_ready[2];   // E -> R (sigma in smem), R -> E (omega)
     unsigned long long col_full[kColBufs];        // both warpgroups' halves of a col_buf tile have landed (complete_tx)
+#ifdef P3D_WS3_ROLE_CLOCKS
+    unsigned long long rclk[kRoles][kRcSlots];
+#endif
 };
 
 // Float index of colour (row, c) in a staged / loaded colour tile: 128 B rows, 16-byte chunk (c / 4) XOR (row % 8).  The
@@ -99,6 +130,9 @@ struct WsArgs {
     int n_groups, single_pass;
     int srow, scol, splane;
     float sigma_cull;
+#ifdef P3D_WS3_ROLE_CLOCKS
+    unsigned long long* role_clk;    // [gridDim.x][kRoles][kRcSlots]
+#endif
 };
 
 // pass j of a CTA with N groups:  C(0) C(1) | F(0) C(2) | F(1) C(3) | ... | F(N-2) F(N-1)   (N == 1: C(0) F(0))
@@ -145,11 +179,15 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
     }
     stage_w1_biases(g, a.w1, a.b1, a.b2, sm.w1, sm.b1, sm.b2c, sm.b2s, tid, kThreadsWS);
     stage_w2(g, a.w2, sm.w2, kD2Cols, kLBO_W2, w2_row_n48, tid, kThreadsWS);
+#ifdef P3D_WS3_ROLE_CLOCKS
+    if (tid < kRoles * kRcSlots) (&sm.rclk[0][0])[tid] = 0ull;
+#endif
     fence_proxy_async();
     __syncthreads();
 
     if (warp < kGW) {
         // =========================================================================== GATHER
+        RC_BEGIN(rc_role);
         const int gw = warp, team = gw >> 2, wt = gw & 3;
         constexpr int kEsz = BF16 ? 2 : 4;
         const long long scolB = (long long)a.scol * kEsz, srowB = (long long)a.srow * kEsz;
@@ -167,10 +205,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             const int grp = (int)blockIdx.x + td.n * (int)gridDim.x;
             const long long ray0 = (long long)grp * GR;
             GroupState& st = sm.st[td.n & 3];
-            if (td.pass == 0) mbar_wait(&sm.state_free[td.n & 3], ((td.n >> 2) & 1) ^ 1);
-            else mbar_wait(&sm.fine_ready[td.n & 3], (td.n >> 2) & 1);
+            if (td.pass == 0) RC_WAIT(0, RC_STATE_FREE, &sm.state_free[td.n & 3], ((td.n >> 2) & 1) ^ 1);
+            else RC_WAIT(0, RC_FINE_READY, &sm.fine_ready[td.n & 3], (td.n >> 2) & 1);
             const int view = (int)(ray0 / g.M);
             // ---- tap table of this warp's 32 rows: lane = row
+            RC_BEGIN(rc_taps);
             {
                 const int trow = wt * 32 + lane;
                 const int rl = trow / RPT, s = td.k * RPT + (trow - rl * RPT);
@@ -195,17 +234,22 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 st.crop[td.pass][srow] = (g.crop_on && !((fabsf(pt.x) <= g.crop_limit) && (fabsf(pt.z) <= g.crop_limit))) ? 1 : 0;
             }
             __syncwarp();
+            RC_END(0, RC_TAPS, rc_taps);
             const int stage = my_it % kNA;
-            mbar_wait(&sm.a1_empty[stage], ((my_it / kNA) & 1) ^ 1);
+            RC_WAIT(0, RC_A1_EMPTY, &sm.a1_empty[stage], ((my_it / kNA) & 1) ^ 1);
+            RC_BEGIN(rc_gather);
             gather_a1<BF16, SCOL>(tab, reinterpret_cast<const char*>(a.planes) + (long long)view * g.stride_view * kEsz, 0 /* one view */, srowB,
                                   scolB, v, sm.a1[stage][0], sm.a1[stage][1], wt, lane);
             fence_proxy_async();
             __syncwarp();                                                   // also: the tap table is rewritten by the next tile
+            RC_END(0, RC_GATHER, rc_gather);
             if (lane == 0) mbar_arrive(&sm.a1_full[stage]);
         }
+        RC_END(0, RC_TOTAL, rc_role);
     } else if (warp < kGW + kEW) {
         // =========================================================================== DECODER
         setmaxnreg_inc<kRegE>();
+        RC_BEGIN(rc_role);
         const int e = warp - kGW, quarter = e & 3, chunk = e >> 2;      // chunk = warpgroup = 64-row half of a tile
         const int etid = tid - kGW * 32;                                  // 0..255 inside the decoder group
         const bool elect = (etid & 127) == 0;                             // the warpgroup's bulk-copy thread
@@ -241,10 +285,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             loaded = n;
         };
         auto colours = [&](int n) {                                        // sum_j omega_j * rgb_j for group n
+            RC_BEGIN(rc_col);
             if (loaded < n) first_loads(n);
             const int slot_i = n & 1;
             SlotState& sl = sm.slot[slot_i];
-            mbar_wait(&sm.omega_ready[slot_i], (n >> 1) & 1);              // omega / pos / back of group n (ray warps)
+            RC_WAIT(1, RC_OMEGA_READY, &sm.omega_ready[slot_i], (n >> 1) & 1);   // omega / pos / back of group n (ray warps)
             const int grp = (int)blockIdx.x + n * (int)gridDim.x;
             const long long ray0 = (long long)grp * GR;
             // Warp e sums rows [16 e, 16 e + 16) of each of the six tiles - always one ray, rl - with lane = channel, in a fixed
@@ -257,13 +302,18 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
 #pragma unroll 1
             for (int t = 0; t < 6; ++t) {
                 const int pass = t / 3, k = t - 3 * pass, b = t % kColBufs;
-                mbar_wait(&sm.col_full[b], ((6 * n + t) / kColBufs) & 1);
-                const float* buf = sm.col_buf[b];
                 const unsigned short* pos = sl.pos + pass * kRowsG + rl * S + k * RPT - rl * RPT;   // pos[trow]: the row's merged position
-#pragma unroll 4
+                // The omega of the tile's 16 rows is read before the wait for its colours (omega is ready, the tile may still
+                // be landing), and both loops are unrolled, so every load is issued before the first add of the fixed-order sum.
+                float omj[16];
+#pragma unroll
+                for (int j = 0; j < 16; ++j) omj[j] = live ? sl.om[rl * L + pos[16 * e + j]] : 0.f;
+                RC_WAIT(1, RC_COL_FULL, &sm.col_full[b], ((6 * n + t) / kColBufs) & 1);
+                const float* buf = sm.col_buf[b];
+#pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     const int trow = 16 * e + j;
-                    const float om = live ? sl.om[rl * L + pos[trow]] : 0.f;
+                    const float om = omj[j];
                     const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
                     part += fmaf(buf[col_idx(trow, lane)], ca, cb);
                 }
@@ -281,6 +331,7 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             }
             ebar();
             if (etid == 0) mbar_arrive(&sm.state_free[n & 3]);
+            RC_END(1, RC_COLOURS, rc_col);
         };
 
         // colours(n) needs omega from the ray warps; it runs at the top of the first tile of F(n+1) - three tiles (C(n+2))
@@ -291,18 +342,26 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             const TileDesc td = tile_at(it, n_my);
             if (td.pass == 1 && td.k == 0 && td.n >= 1) colours(td.n - 1);
             const int stage = it % kNA;
-            mbar_wait(&sm.a1_full[stage], (it / kNA) & 1);
+            RC_WAIT(1, RC_A1_FULL, &sm.a1_full[stage], (it / kNA) & 1);
+            RC_BEGIN(rc_l1);
             float d1[32];
             decoder_layer1(d1, smem_u32(sm.a1[stage][0]), smem_u32(sm.a1[stage][1]), kLBO_A1, w1h, w1l, kLBO_W1, chunk, a.single_pass);
             __syncwarp();
             if (lane == 0) mbar_arrive(&sm.a1_empty[stage]);
+            RC_END(1, RC_L1, rc_l1);
+            RC_BEGIN(rc_hid);
             uint32_t ah[16], al[16];
             decoder_hidden(d1, sm.b1, lane, ah, al);
+            RC_FENCE_REGS(ah, al);
+            RC_END(1, RC_HIDDEN, rc_hid);
+            RC_BEGIN(rc_l2);
             float d2[kD2Cols / 2];
             decoder_layer2_issue<kD2Cols>(d2, ah, al, w2h, w2l, kLBO_W2, a.single_pass);
             wgmma_commit();
             wgmma_wait_all();
             fence_operands(d2);
+            RC_END(1, RC_L2, rc_l2);
+            RC_BEGIN(rc_epi);
             // the staging half is free once the bulk store of the previous tile has read it
             if (stored > loaded) first_loads(stored);
             else if (elect) bulk_wait_read();
@@ -334,6 +393,7 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 bulk_store(colour_area(td.n, td.pass) + (td.k * 128 + 64 * chunk) * kRgb, smem_u32(stage_tile), kHalfBytes);
                 bulk_commit();
             }
+            RC_END(1, RC_EPILOGUE, rc_epi);
             if (td.k == 2) {                                              // the group's pass is complete: hand its sigma to the ray warps
                 if (td.pass == 1) stored = td.n;
                 __syncwarp();
@@ -341,9 +401,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             }
         }
         colours(n_my - 1);
+        RC_END(1, RC_TOTAL, rc_role);
     } else if (warp < kGW + kEW + kRW) {
         // =========================================================================== RAY (one warp per ray)
         setmaxnreg_dec<kRegR>();
+        RC_BEGIN(rc_role);
         const int rw = warp - kGW - kEW;
         float* scr = sm.rscratch[rw];
         constexpr int NC = (S + 31) / 32, nb = S - 3;
@@ -564,20 +626,59 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             const int n = pd.n, si = n & 3;
             const uint32_t par = (n >> 2) & 1;
             if (pd.pass == 0) {
-                mbar_wait(&sm.sigc_ready[si], par);
+                RC_WAIT(2, RC_SIG_READY, &sm.sigc_ready[si], par);
+                RC_BEGIN(rc_imp);
                 for (int rl = rw; rl < GR; rl += kRW) importance_ray(n, rl);
+                RC_END(2, RC_IMPORTANCE, rc_imp);
                 if (lane == 0) mbar_arrive(&sm.fine_ready[si]);
             } else {
-                mbar_wait(&sm.sigf_ready[si], par);
-                if (n >= 2) mbar_wait(&sm.state_free[(n - 2) & 3], ((n - 2) >> 2) & 1);       // colours(n-2) has released the omega slot
+                RC_WAIT(2, RC_SIG_READY, &sm.sigf_ready[si], par);
+                if (n >= 2) RC_WAIT(2, RC_STATE_FREE, &sm.state_free[(n - 2) & 3], ((n - 2) >> 2) & 1);   // colours(n-2) has released the omega slot
                 for (int rl = rw; rl < GR; rl += kRW) composite_ray(n, rl);
                 if (lane == 0) mbar_arrive(&sm.omega_ready[n & 1]);
             }
         }
+        RC_END(2, RC_TOTAL, rc_role);
     }
+#ifdef P3D_WS3_ROLE_CLOCKS
+    __syncthreads();
+    if (tid < kRoles * kRcSlots) atomicAdd(a.role_clk + (long long)blockIdx.x * (kRoles * kRcSlots) + tid, (&sm.rclk[0][0])[tid]);
+#endif
 }
 
+#ifdef P3D_WS3_ROLE_CLOCKS
+// the role counters of every CTA slot (one per SM), zeroed when first allocated, accumulated by every launch
+unsigned long long* g_role_clk = nullptr;
+int g_role_clk_ctas = 0;
+int role_clocks_buffer(int n_sm, unsigned long long** out) {
+    if (!g_role_clk) {
+        const size_t bytes = (size_t)n_sm * kRoles * kRcSlots * sizeof(unsigned long long);
+        P3D_CUDA_TRY(cudaMalloc(&g_role_clk, bytes));
+        P3D_CUDA_TRY(cudaMemset(g_role_clk, 0, bytes));
+        g_role_clk_ctas = n_sm;
+    }
+    *out = g_role_clk;
+    return P3D_OK;
+}
+#endif
+
 }  // namespace
+
+#ifdef P3D_WS3_ROLE_CLOCKS
+// Copies the accumulated role counters ([CTA][kRoles][kRcSlots] cycles, at most `cap` values) to `host` after a device
+// synchronise and zeroes them when `reset`.  Returns the number of values, or a (negative) P3D error.
+extern "C" long long p3d_ws3_role_clocks(unsigned long long* host, long long cap, int reset) {
+    int n_sm;
+    unsigned long long* buf;
+    if (int rc = sm_count(&n_sm)) return rc;
+    if (int rc = role_clocks_buffer(n_sm, &buf)) return rc;
+    const long long n = (long long)g_role_clk_ctas * kRoles * kRcSlots;
+    if (cudaDeviceSynchronize() != cudaSuccess) return P3D_ECUDA;
+    if (host && cap >= n && cudaMemcpy(host, buf, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) return P3D_ECUDA;
+    if (reset && cudaMemset(buf, 0, n * sizeof(unsigned long long)) != cudaSuccess) return P3D_ECUDA;
+    return n;
+}
+#endif
 
 bool fused_ws3_supported(const Geom& g) {
     if (!((g.S == 96 || g.S == 48) && (g.Sf == g.S) && ((long long)g.M % (384 / g.S) == 0))) return false;
@@ -615,6 +716,9 @@ int render_forward_fused_ws3(const Geom& g, const p3d_render_params* p, const vo
     }
     int n_sm;
     if ((rc = sm_count(&n_sm))) return rc;
+#ifdef P3D_WS3_ROLE_CLOCKS
+    if ((rc = role_clocks_buffer(n_sm, &a.role_clk))) return rc;
+#endif
     const size_t smem = kSmemWS;
     void (*kern)(WsArgs) = with_texel_stride(g, [&](auto sc) -> void (*)(WsArgs) {
         if (g.S == 96) return p->planes_bf16 ? k_render_ws3<true, 96, sc.value> : k_render_ws3<false, 96, sc.value>;
