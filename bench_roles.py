@@ -25,16 +25,16 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 SLOTS = ['total', 'wait a1_full', 'wait a1_empty', 'wait state_free', 'wait fine_ready', 'wait sigc/sigf_ready',
-         'wait omega_ready', 'wait col_full', 'colours()', 'layer 1', 'hidden', 'layer 2', 'epilogue + store', 'tap table',
+         'wait col_stored', 'wait col_full', 'colours()', 'layer 1', 'hidden', 'layer 2', 'epilogue + store', 'tap table',
          'gather loads + lerp', 'importance']
 ROLES = [('gather', 12, ['wait state_free', 'wait fine_ready', 'wait a1_empty', 'tap table', 'gather loads + lerp']),
-         # colours() includes its omega_ready / col_full waits, which are also listed on their own
-         ('decoder', 8, ['wait a1_full', 'colours()', 'wait omega_ready', 'wait col_full', 'layer 1', 'hidden', 'layer 2',
-                         'epilogue + store']),
-         ('ray', 4, ['wait sigc/sigf_ready', 'wait state_free', 'importance'])]
+         # the epilogue includes the state_free wait before a colour area is rewritten, which is also listed on its own
+         ('decoder', 8, ['wait a1_full', 'wait state_free', 'layer 1', 'hidden', 'layer 2', 'epilogue + store']),
+         # colours() includes its col_stored / col_full waits, which are also listed on their own
+         ('ray', 4, ['wait sigc/sigf_ready', 'colours()', 'wait col_stored', 'wait col_full', 'importance'])]
 EXCLUSIVE = {'gather': ['wait state_free', 'wait fine_ready', 'wait a1_empty', 'tap table', 'gather loads + lerp'],
-             'decoder': ['wait a1_full', 'colours()', 'layer 1', 'hidden', 'layer 2', 'epilogue + store'],
-             'ray': ['wait sigc/sigf_ready', 'wait state_free', 'importance']}
+             'decoder': ['wait a1_full', 'layer 1', 'hidden', 'layer 2', 'epilogue + store'],
+             'ray': ['wait sigc/sigf_ready', 'colours()', 'importance']}
 
 
 def build_roles_lib(out_dir):

@@ -3,27 +3,26 @@
 //   passes C(0) C(1) | F(0) C(2) | F(1) C(3) | ... | F(N-2) F(N-1)          (C = 3 coarse tiles, F = 3 importance tiles)
 //
 // A tile's colour sigmoids wait for the group's compositing weights (omega), which exist only after its fine pass.  They are
-// staged in global memory, in this CTA's own slice of the workspace colour buffers (see colour_area: coarse areas
-// CA[n % 3] and one fine area FA, 4 x 48 KB per CTA, ~25 MB on 132 SMs).  The areas are rewritten every few groups, so
+// staged in global memory, in this CTA's own slices of the workspace colour buffers (see colour_area: coarse areas
+// CA[n % 3] and fine areas FA[n & 1], 5 x 48 KB per CTA, ~32 MB on 132 SMs).  The areas are rewritten every few groups, so
 // their footprint fits the 50 MB L2, but they share it with the streamed tri-plane gather; how much of the round trip is
-// served by L2 rather than HBM has not been measured.  Both directions are bulk copies of whole 8 KB tile halves: the
-// epilogue stages them in shared memory for one cp.async.bulk store, and a group's tiles come back into shared memory
-// buffers (mbarrier complete_tx) while the decoder runs C(n+2), so colours(n) reduces from shared memory.  Only
-// the COARSE colours of a group have to wait through a whole fine pass; the fine ones are consumed right after the group's
-// merge, so all groups share one fine area.  With F(n) followed by C(n+2):
+// served by L2 rather than HBM has not been measured.  The decoder's epilogue stages each 8 KB tile half in shared memory
+// for one cp.async.bulk store; once a group's fine pass is stored, the ray warps bulk-load their own rays' rows back into
+// shared memory (mbarrier complete_tx) and reduce them there (colours(n)), off the decoder's critical path.  With F(n)
+// followed by C(n+2):
 //   * importance(n) has two passes of slack (F(n-1), C(n+1)) before the gather of F(n) needs its depths;
-//   * merge(n) + omega(n) run on the RAY warps while the decoder handles the three tiles of C(n+2); colours(n) runs at the
-//     top of F(n+1)'s first tile - the last point before F(n+1) overwrites the fine area (C(n+3), which reuses
-//     CA[n % 3], comes later still);
-//   * the per-group state ring stays 4 deep (groups n .. n+3 alive), the omega slot 2 deep.
+//   * merge(n) + omega(n) run on the RAY warps while the decoder handles the three tiles of C(n+2); colours(n) follows on
+//     the same warps once the decoder signals that F(n)'s stores completed (col_stored, in C(n+2)'s first epilogue);
+//   * the decoder stores into an area only after its previous group's colours are done (state_free): C(m) into CA[m % 3]
+//     after group m - 3, F(m) into FA[m & 1] after group m - 2, each with several tiles of slack;
+//   * the per-group state ring stays 4 deep (groups n .. n+3 alive).
 //
 //   warps  0-11  GATHER    three teams of four warps; team j takes tiles j, j+3, ... of the tile sequence
 //   warps 12-19  DECODER   two warpgroups, one per 64-row half of every tile: layer 1 (wgmma, A1 and W1 from shared memory)
 //                          -> softplus2 in registers -> layer 2 (one m64n48 wgmma, A from the registers): colour sigmoids ->
-//                          staging tile -> bulk store to the colour area, sigma -> group state; bulk loads of a group's
-//                          colours and their reduction once its omega is ready
+//                          staging tile -> bulk store to the colour area, sigma -> group state
 //   warps 20-23  RAY       a warp per ray: importance sampling after a group's coarse pass, merge / transmittance /
-//                          omega and the per-ray outputs after its fine pass
+//                          omega, the per-ray outputs and the colour reduction of its own rays after its fine pass
 #include "fused_common.cuh"
 
 namespace p3d {
@@ -45,6 +44,7 @@ constexpr int kStates = 4;                       // per-group state ring
 constexpr int kRowsG = 384;                      // rows per pass per group
 constexpr int kColBufs = 2;                      // colour tiles of a group in shared memory at once (colours())
 constexpr int kHalfBytes = 64 * kRgb * 4;        // one decoder warpgroup's 64 rows of colour sigmoids: 8 KB
+constexpr int kRowBytes = kRgb * 4;              // one row of colour sigmoids: 128 B
 
 
 // Per-role cycle accounting, compiled in only with -DP3D_WS3_ROLE_CLOCKS (bench_roles.py): lane 0 of every warp adds
@@ -52,10 +52,11 @@ constexpr int kHalfBytes = 64 * kRgb * 4;        // one decoder warpgroup's 64 r
 // ([CTA][kRoles][kRcSlots], accumulated over launches) at its end.  RC_* slots 1-7 are mbarrier waits, the rest phases of work;
 // a role's remainder (RC_TOTAL minus the slots it uses) is untimed bookkeeping.  The default build has no clock reads.
 enum RoleClk {
-    RC_TOTAL, RC_A1_FULL, RC_A1_EMPTY, RC_STATE_FREE, RC_FINE_READY, RC_SIG_READY, RC_OMEGA_READY, RC_COL_FULL,
-    RC_COLOURS, RC_L1, RC_HIDDEN, RC_L2, RC_EPILOGUE,         // decoder phases (colours() includes its omega / col_full waits)
+    RC_TOTAL, RC_A1_FULL, RC_A1_EMPTY, RC_STATE_FREE, RC_FINE_READY, RC_SIG_READY, RC_COL_STORED, RC_COL_FULL,
+    RC_COLOURS, RC_L1, RC_HIDDEN, RC_L2, RC_EPILOGUE,         // decoder phases (the epilogue includes its state_free wait)
     RC_TAPS, RC_GATHER,                                       // gather phases: tap table, loads + lerp into the A1 stage
-    RC_IMPORTANCE,                                            // ray phases: importance sampling (composite = the rest)
+    RC_IMPORTANCE,                                            // ray phases: importance sampling, colours() (which includes its
+                                                              // col_stored / col_full waits); composite = the rest
     kRcSlots
 };
 #ifdef P3D_WS3_ROLE_CLOCKS
@@ -79,27 +80,27 @@ struct GroupState {                               // written by G (t_c, crop), E
     float t_c[kRowsG], sg_c[kRowsG], t_f[kRowsG], sg_f[kRowsG];
     unsigned char crop[2][kRowsG];
 };
-struct SlotState {                                // written by R (composite), read by E (colours)
+struct SlotState {                                // written by composite_ray, read by colours() of the same ray warp
     float om[2 * kRowsG];                         // omega per merged position, [ray][2S]
     unsigned short pos[2 * kRowsG];                          // merged position of coarse rows [0,384) and fine rows [384,768)
-    float acc[8][kRgb];
-    float back[8];
 };
 
 struct __align__(1024) WsSmem {
     unsigned char a1[kNA][2][4 * kLBO_A1];
     float col_stage[2][64 * kRgb];                // per decoder warpgroup: its half of the tile being stored (col_idx layout)
-    float col_buf[kColBufs][128 * kRgb];          // colour tiles loaded back for colours(), same layout
+    float col_buf[kColBufs][128 * kRgb];          // colour tiles loaded back for colours(), same layout; each ray warp
+                                                  // loads and reads only its own rays' rows
     unsigned char w1[2][4096], w2[2][kD2Cols * 128];
     float b1[kHidden], b2c[kRgb], b2s, pad0[3];
     uint4 tab[kGW][32][4];                        // tap table of a gather warp's 32 rows (see "gather" below)
     GroupState st[kStates];
-    SlotState slot[2];
+    SlotState slot;
     float rscratch[kRW][768];                      // private scratch of each ray warp (importance / merge)
     unsigned long long a1_full[kNA], a1_empty[kNA];
     unsigned long long fine_ready[kStates], state_free[kStates];
-    unsigned long long sigc_ready[kStates], sigf_ready[kStates], omega_ready[2];   // E -> R (sigma in smem), R -> E (omega)
-    unsigned long long col_full[kColBufs];        // both warpgroups' halves of a col_buf tile have landed (complete_tx)
+    unsigned long long sigc_ready[kStates], sigf_ready[kStates];   // E -> R (sigma in smem)
+    unsigned long long col_stored[2];             // E -> R: both warpgroups' bulk stores of a group's fine pass completed
+    unsigned long long col_full[kRW][kColBufs];   // a ray warp's rows of a col_buf tile have landed (complete_tx)
 #ifdef P3D_WS3_ROLE_CLOCKS
     unsigned long long rclk[kRoles][kRcSlots];
 #endif
@@ -165,16 +166,24 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // provably warp-uniform
     const int n_my = (a.n_groups - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // groups of this CTA
     const int T = 6 * n_my;
+    // this CTA's colour area of (group n, pass): 384 rows x 32 sigmoids, row = 128 k + row of tile k, each tile in the
+    // col_idx layout (a byte copy of the staged tile).  CA[j] = slice j of the coarse workspace buffer, FA[i] = slice i of
+    // the fine one, where slice s is the one of this CTA's group s: they exist whenever they are used (n % 3, n & 1 < n_my).
+    auto colour_area = [&](int n, int pass) -> float* {
+        const int s = pass == 0 ? n % 3 : n & 1;
+        return (pass == 0 ? a.col_c : a.col_f) + ((long long)blockIdx.x + (long long)s * gridDim.x) * (kRowsG * kRgb);
+    };
 
     // ---------------- setup
     if (tid == 0) {
         for (int i = 0; i < kNA; ++i) { mbar_init(&sm.a1_full[i], 4); mbar_init(&sm.a1_empty[i], kEW); }
         for (int i = 0; i < kStates; ++i) {
-            mbar_init(&sm.fine_ready[i], kRW); mbar_init(&sm.state_free[i], 1);
+            mbar_init(&sm.fine_ready[i], kRW); mbar_init(&sm.state_free[i], kRW);
             mbar_init(&sm.sigc_ready[i], kEW); mbar_init(&sm.sigf_ready[i], kEW);
         }
-        mbar_init(&sm.omega_ready[0], kRW); mbar_init(&sm.omega_ready[1], kRW);
-        for (int i = 0; i < kColBufs; ++i) mbar_init(&sm.col_full[i], 2);
+        mbar_init(&sm.col_stored[0], 2); mbar_init(&sm.col_stored[1], 2);
+        for (int w = 0; w < kRW; ++w)
+            for (int i = 0; i < kColBufs; ++i) mbar_init(&sm.col_full[w][i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     stage_w1_biases(g, a.w1, a.b1, a.b2, sm.w1, sm.b1, sm.b2c, sm.b2s, tid, kThreadsWS);
@@ -253,94 +262,32 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         const int e = warp - kGW, quarter = e & 3, chunk = e >> 2;      // chunk = warpgroup = 64-row half of a tile
         const int etid = tid - kGW * 32;                                  // 0..255 inside the decoder group
         const bool elect = (etid & 127) == 0;                             // the warpgroup's bulk-copy thread
-        // this CTA's colour area of (group n, pass): 384 rows x 32 sigmoids, row = 128 k + row of tile k, each tile in the
-        // col_idx layout (a byte copy of the staged tile).  Areas are slices of the workspace colour buffers that belong to this
-        // CTA's own first two groups (coarse and fine buffer each), so they exist whenever they are used: CA[0..2] = slices
-        // 0..2, FA = slice 3 (slice 1 when the CTA has a single group)
-        auto colour_area = [&](int n, int pass) -> float* {
-            const int j = pass == 0 ? n % 3 : (n_my >= 2 ? 3 : 1);
-            return ((j & 1) ? a.col_f : a.col_c) + ((long long)blockIdx.x + (long long)(j >> 1) * gridDim.x) * (kRowsG * kRgb);
-        };
-        auto ebar = [] { asm volatile("bar.sync 1, 256;" ::: "memory"); };   // the eight decoder warps
         auto wgbar = [chunk] { asm volatile("bar.sync %0, 128;" ::"r"(2 + chunk) : "memory"); };   // this warpgroup's four warps
-        // Colour tile t of a group (t = 0..2: coarse tile t, 3..5: fine tile t - 3) is loaded into col_buf[t % kColBufs].  Each
-        // warpgroup loads back the half it stored itself, so the only stores a load depends on are the issuing thread's own.
-        auto load_tile = [&](int n, int t) {                             // elected thread only
-            const int pass = t / 3, b = t % kColBufs;
-            mbar_arrive_expect_tx(&sm.col_full[b], kHalfBytes);
-            bulk_load(smem_u32(sm.col_buf[b]) + chunk * kHalfBytes, colour_area(n, pass) + ((t - 3 * pass) * 128 + 64 * chunk) * kRgb,
-                      kHalfBytes, &sm.col_full[b]);
-        };
-        // The first kColBufs tiles of group n are requested once its fine pass is stored: in the epilogue of the next tile,
-        // C(n+2)'s first, so they arrive while the decoder runs C(n+2) - or at the top of colours(n) where no C(n+2) exists.
-        // A full wait_group (the stores are written, not just read) and the proxy fence make the area readable by the loads.
-        int stored = -1, loaded = -1;                                     // last group whose fine pass was stored / first tiles requested
-        auto first_loads = [&](int n) {
+        // The ray warps read a group's colours back once both warpgroups' stores of its fine pass have COMPLETED, not just
+        // read their staging tiles: in the epilogue of the next tile (C(n+2)'s first, or F(n+1)'s), and after the tile loop
+        // for the last group, the elected thread of each warpgroup waits for all its bulk groups and arrives on
+        // col_stored[n & 1].  The chain from these bulk stores to another thread's bulk loads of the same bytes, by the PTX
+        // ISA's memory consistency model and its proxy rules:
+        //   cp.async.bulk.wait_group 0     the stores (async proxy) are complete: their writes to global memory are performed;
+        //   fence.proxy.async.global       orders them before this thread's later generic-proxy operations;
+        //   mbarrier.arrive                release.cta by default; the ray warp's mbarrier.try_wait (acquire.cta) that
+        //                                  observes the completed phase synchronises with it (colours(), ray warps);
+        //   fence.proxy.async.global       on the loading thread: what it acquired is ordered before its own later
+        //                                  async-proxy operations;
+        //   cp.async.bulk (load)           reads the stored colours.
+        int stored = -1, signalled = -1;                                  // last group whose fine pass was stored / signalled
+        auto signal_stored = [&] {
             if (elect) {
                 bulk_wait_all();
                 fence_proxy_async_global();
-#pragma unroll 1
-                for (int t = 0; t < kColBufs; ++t) load_tile(n, t);
+                mbar_arrive(&sm.col_stored[stored & 1]);
             }
-            loaded = n;
+            signalled = stored;
         };
-        auto colours = [&](int n) {                                        // sum_j omega_j * rgb_j for group n
-            RC_BEGIN(rc_col);
-            if (loaded < n) first_loads(n);
-            const int slot_i = n & 1;
-            SlotState& sl = sm.slot[slot_i];
-            RC_WAIT(1, RC_OMEGA_READY, &sm.omega_ready[slot_i], (n >> 1) & 1);   // omega / pos / back of group n (ray warps)
-            const int grp = (int)blockIdx.x + n * (int)gridDim.x;
-            const long long ray0 = (long long)grp * GR;
-            // Warp e sums rows [16 e, 16 e + 16) of each of the six tiles - always one ray, rl - with lane = channel, in a fixed
-            // order.  The partial sums of a ray meet in sl.acc as one (S = 48) or two (S = 96: warps 2 rl, 2 rl + 1)
-            // shared-memory adds onto 0, whose order cannot change the rounded sum: the kernel is bit-reproducible run to run
-            // and independent of how the rays are batched.
-            const int rl = 16 * e / RPT;
-            const bool live = ray0 + rl < a.R;
-            float part = 0.f;
-#pragma unroll 1
-            for (int t = 0; t < 6; ++t) {
-                const int pass = t / 3, k = t - 3 * pass, b = t % kColBufs;
-                const unsigned short* pos = sl.pos + pass * kRowsG + rl * S + k * RPT - rl * RPT;   // pos[trow]: the row's merged position
-                // The omega of the tile's 16 rows is read before the wait for its colours (omega is ready, the tile may still
-                // be landing), and both loops are unrolled, so every load is issued before the first add of the fixed-order sum.
-                float omj[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) omj[j] = live ? sl.om[rl * L + pos[16 * e + j]] : 0.f;
-                RC_WAIT(1, RC_COL_FULL, &sm.col_full[b], ((6 * n + t) / kColBufs) & 1);
-                const float* buf = sm.col_buf[b];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int trow = 16 * e + j;
-                    const float om = omj[j];
-                    const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
-                    part += fmaf(buf[col_idx(trow, lane)], ca, cb);
-                }
-                if (t + kColBufs < 6) {
-                    wgbar();                                               // this warpgroup's half of col_buf[b] is read
-                    if (elect) load_tile(n, t + kColBufs);
-                }
-            }
-            atomicAdd(&sl.acc[rl][lane], part);
-            ebar();                                                        // all eight decoder warps (also: the buffers are read)
-            if (etid < GR * kRgb) {
-                const int rl = etid >> 5, c = etid & 31;
-                const long long ray = ray0 + rl;
-                if (ray < a.R) a.out_rgb[ray * kRgb + c] = __fsub_rn(__fmul_rn(__fadd_rn(sl.acc[rl][c], sl.back[rl]), 2.f), 1.f);
-            }
-            ebar();
-            if (etid == 0) mbar_arrive(&sm.state_free[n & 3]);
-            RC_END(1, RC_COLOURS, rc_col);
-        };
-
-        // colours(n) needs omega from the ray warps; it runs at the top of the first tile of F(n+1) - three tiles (C(n+2))
-        // after the group's last sigma - which is also the last point before F(n+1) overwrites the fine area.
         const uint32_t w1h = smem_u32(sm.w1[0]), w1l = smem_u32(sm.w1[1]), w2h = smem_u32(sm.w2[0]), w2l = smem_u32(sm.w2[1]);
         float* stage_tile = sm.col_stage[chunk];
         for (int it = 0; it < T; ++it) {
             const TileDesc td = tile_at(it, n_my);
-            if (td.pass == 1 && td.k == 0 && td.n >= 1) colours(td.n - 1);
             const int stage = it % kNA;
             RC_WAIT(1, RC_A1_FULL, &sm.a1_full[stage], (it / kNA) & 1);
             RC_BEGIN(rc_l1);
@@ -362,8 +309,8 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             fence_operands(d2);
             RC_END(1, RC_L2, rc_l2);
             RC_BEGIN(rc_epi);
-            // the staging half is free once the bulk store of the previous tile has read it
-            if (stored > loaded) first_loads(stored);
+            // the staging half is free once the bulk store of the previous tile has read it (wait_group 0 includes that)
+            if (stored > signalled) signal_stored();
             else if (elect) bulk_wait_read();
             wgbar();
             GroupState& st = sm.st[td.n & 3];
@@ -390,6 +337,10 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             fence_proxy_async();                                          // the staging writes, seen by the bulk store
             wgbar();
             if (elect) {
+                // The area was last read by the ray warps' loads for group n - 3 (CA[n % 3]) or n - 2 (FA[n & 1]).  Their
+                // colours() have waited for every load to land before arriving on that group's state_free.
+                const int prev = td.n - (td.pass == 0 ? 3 : 2);
+                if (td.k == 0 && prev >= 0) RC_WAIT(1, RC_STATE_FREE, &sm.state_free[prev & 3], (prev >> 2) & 1);
                 bulk_store(colour_area(td.n, td.pass) + (td.k * 128 + 64 * chunk) * kRgb, smem_u32(stage_tile), kHalfBytes);
                 bulk_commit();
             }
@@ -400,7 +351,7 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 if (lane == 0) mbar_arrive(td.pass == 0 ? &sm.sigc_ready[td.n & 3] : &sm.sigf_ready[td.n & 3]);
             }
         }
-        colours(n_my - 1);
+        signal_stored();                                                  // the last group's fine pass
         RC_END(1, RC_TOTAL, rc_role);
     } else if (warp < kGW + kEW + kRW) {
         // =========================================================================== RAY (one warp per ray)
@@ -541,7 +492,7 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         // ---- merge + transmittance + omega + per-ray outputs of ray rl of group n (renderer.py:289-301, ray_marcher.py:25-57)
         auto composite_ray = [&](int n, int rl) {
             GroupState& st = sm.st[n & 3];
-            SlotState& sl = sm.slot[n & 1];
+            SlotState& sl = sm.slot;
             const long long ray = (long long)((int)blockIdx.x + n * (int)gridDim.x) * GR + rl;
             const float* tc = st.t_c + rl * S;
             const float* tf = st.t_f + rl * Sf;
@@ -550,7 +501,6 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             const bool rev = tc[0] > tc[S - 1];
             const float* tca = rev ? tc + (S - 1) : tc;     // ascending view of the coarse depths: tca[m * dir]
             const int dir = rev ? -1 : 1;
-            sl.acc[rl][lane] = 0.f;
 #pragma unroll
             for (int c = 0; c < L / 32; ++c) {    // merge by rank: position = own index + count of the other list before it
                 const int r = c * 32 + lane;
@@ -617,10 +567,82 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                     atomicMax(&a.bounds[1], float_to_ordered(m_t[L - 1]));
                 }
             }
-            if (lane == 0) sl.back[rl] = back;
-            __syncwarp();
+            __syncwarp();                         // om / pos are read by the other lanes in colours()
+            return back;                          // warp-uniform (warp_sum is a butterfly)
         };
-        // tasks follow the pass schedule: importance(n) after C(n), merge(n) after F(n)
+        // ---- colours of this warp's rays of group n: sum_j omega_j * rgb_j over the group's six colour tiles (t = 0..2:
+        // coarse tile t, 3..5: fine tile t - 3).  The warp's rows of tile t - a ray's RPT rows of a tile are contiguous in the
+        // colour area - are bulk-loaded into the same rows of col_buf[t % kColBufs], which the warp reloads with tile
+        // t + kColBufs as soon as all its lanes have read it.
+        constexpr int RW = GR / kRW;              // rays of this warp: rw + kRW i, i < RW (1 at S = 96, 2 at S = 48)
+        auto load_tile = [&](int n, int t) {      // lane 0 only
+            const int pass = t / 3, k = t - 3 * pass, b = t % kColBufs;
+            const float* area = colour_area(n, pass) + k * 128 * kRgb;
+            mbar_arrive_expect_tx(&sm.col_full[rw][b], RW * RPT * kRowBytes);
+#pragma unroll
+            for (int i = 0; i < RW; ++i) {
+                const int row = (rw + kRW * i) * RPT;
+                bulk_load(smem_u32(sm.col_buf[b] + row * kRgb), area + row * kRgb, RPT * kRowBytes, &sm.col_full[rw][b]);
+            }
+        };
+        auto colours = [&](int n, const float (&back)[RW]) {
+            RC_BEGIN(rc_col);
+            // the decoder's elected threads arrive once their stores of F(n) are complete; the acquire here and the proxy
+            // fence below close the chain from those bulk stores to these bulk loads (argued at signal_stored)
+            RC_WAIT(2, RC_COL_STORED, &sm.col_stored[n & 1], (n >> 1) & 1);
+            if (lane == 0) {
+                fence_proxy_async_global();
+#pragma unroll 1
+                for (int t = 0; t < kColBufs; ++t) load_tile(n, t);
+            }
+            const SlotState& sl = sm.slot;
+            const long long ray0 = (long long)((int)blockIdx.x + n * (int)gridDim.x) * GR;
+            // Two chains of 16 rows per tile, lane = channel, each summed over tiles 0..5 in a fixed order: rows [0, 16) and
+            // [16, 32) of ray rw at S = 96, rows [0, 16) of rays rw and rw + 4 at S = 48.  The chains of a ray meet on 0
+            // (0 + a + b at S = 96), so the result is bit-reproducible run to run and independent of how rays are batched.
+            float acc[2] = {0.f, 0.f};
+#pragma unroll 1
+            for (int t = 0; t < 6; ++t) {
+                const int pass = t / 3, k = t - 3 * pass, b = t % kColBufs;
+                // The omega of the tile's 32 rows is read before the wait for its colours (the tile may still be landing), and
+                // the loops are unrolled, so every load is issued before the first add of the fixed-order sums.
+                float omj[2][16];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int rl = rw + kRW * (16 * h / RPT), r0 = 16 * h % RPT;          // chain h: rows r0 .. r0 + 15 of ray rl
+                    const bool live = ray0 + rl < a.R;
+                    const unsigned short* pos = sl.pos + pass * kRowsG + rl * S + k * RPT;   // pos[r]: merged position of row r
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) omj[h][j] = live ? sl.om[rl * L + pos[r0 + j]] : 0.f;
+                }
+                RC_WAIT(2, RC_COL_FULL, &sm.col_full[rw][b], ((6 * n + t) / kColBufs) & 1);
+                const float* buf = sm.col_buf[b];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int rl = rw + kRW * (16 * h / RPT), r0 = 16 * h % RPT;
+                    float& part = acc[h];
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int trow = rl * RPT + r0 + j;
+                        const float om = omj[h][j];
+                        const float ca = g.force_sigmoid ? om : 1.002f * om, cb = g.force_sigmoid ? 0.f : -0.001f * om;
+                        part += fmaf(buf[col_idx(trow, lane)], ca, cb);
+                    }
+                }
+                if (t + kColBufs < 6) {
+                    __syncwarp();                 // every lane has read the warp's rows of col_buf[b]
+                    if (lane == 0) load_tile(n, t + kColBufs);
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < RW; ++i) {
+                const long long ray = ray0 + rw + kRW * i;
+                const float sum = RW == 1 ? __fadd_rn(__fadd_rn(0.f, acc[0]), acc[1]) : __fadd_rn(0.f, acc[i]);
+                if (ray < a.R) a.out_rgb[ray * kRgb + lane] = __fsub_rn(__fmul_rn(__fadd_rn(sum, back[i]), 2.f), 1.f);
+            }
+            RC_END(2, RC_COLOURS, rc_col);
+        };
+        // tasks follow the pass schedule: importance(n) after C(n), merge(n) and colours(n) after F(n)
         for (int j = 0; j < 2 * n_my; ++j) {
             const PassDesc pd = pass_at(j, n_my);
             const int n = pd.n, si = n & 3;
@@ -633,9 +655,11 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                 if (lane == 0) mbar_arrive(&sm.fine_ready[si]);
             } else {
                 RC_WAIT(2, RC_SIG_READY, &sm.sigf_ready[si], par);
-                if (n >= 2) RC_WAIT(2, RC_STATE_FREE, &sm.state_free[(n - 2) & 3], ((n - 2) >> 2) & 1);   // colours(n-2) has released the omega slot
-                for (int rl = rw; rl < GR; rl += kRW) composite_ray(n, rl);
-                if (lane == 0) mbar_arrive(&sm.omega_ready[n & 1]);
+                float back[RW];
+#pragma unroll
+                for (int i = 0; i < RW; ++i) back[i] = composite_ray(n, rw + kRW * i);
+                colours(n, back);
+                if (lane == 0) mbar_arrive(&sm.state_free[si]);       // group state, and the colour areas' loads have landed
             }
         }
         RC_END(2, RC_TOTAL, rc_role);
