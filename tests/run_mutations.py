@@ -4,13 +4,18 @@ fails it, as it must.  The tree is not modified.
 
     python tests/run_mutations.py TARGET [TARGET ...] [--files F ...] [--json out.json] [--build-only]
 
-TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane, modconv, render_fused.  --files runs other GPU files against the same mutants
-instead (to see which of them the rest of the suite catches); the exit code then only reports that the run completed.
---build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
+TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane (the TRI lines of
+render_backward.cu), modconv, render_fused and multiplane (the multiplane section of the header render_device.cuh).  Each
+mutant recompiles every translation unit that includes its source, directly or through other headers.  --files runs other
+GPU files against the same mutants instead (to see which of them the rest of the suite catches); the exit code then only
+reports that the run completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
+--json writes {target: {mutation: result}}.
 """
 import argparse
 import json
 import os
+import re
+import shutil
 import subprocess
 import sys
 import tempfile
@@ -111,6 +116,27 @@ RENDER_FUSED = {
     'fine depths stored in descending order': ('if (f < Sf) st.t_f[rl * Sf + f] = us[c];', 'if (f < Sf) st.t_f[rl * Sf + Sf - 1 - f] = us[c];'),
 }
 
+# render_device.cuh, its multiplane section: every index these mutations produce is still checked against its bound before
+# it addresses memory, except the slab stride from W, which stays in bounds because every plane of both multiplane GPU files
+# has H >= W.  No tap count, shared memory size or tap-table stride is mutated: an unwritten s_tap entry would send the
+# backward's atomics out of bounds.
+MULTIPLANE = {
+    'slab coordinate with align_corners=True': (
+        'const float fz = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)g.D), 1.f), 0.5f);',
+        'const float fz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)(g.D - 1)), 0.5f);'),
+    'slab index off by one': ('t.z0 = sane ? (int)z0f : -4;', 't.z0 = sane ? (int)z0f + 1 : -4;'),
+    'EG3D plane 2 normal taken as x': ('(pm ? x : y));', '(pm ? x : x));'),
+    'depth axis clamped instead of zero-padded': (', zi = t.z0 + (k >> 2);', ', zi = min(max(t.z0 + (k >> 2), 0), g.D - 1);'),
+    'backward scatters to one slab only': ('const int z = t.z0 + (k >> 2);', 'const int z = t.z0;'),
+    'slab offset from plane_w instead of plane_h': ('const long long slab = (long long)g.H * g.stride_row;',
+                                                    'const long long slab = (long long)g.W * g.stride_row;'),
+    # the backward's weight of slab z0 + 1 (slab_texels; the same line in plane_taps3 is followed by `r.w[k]`)
+    'backward weight of slab z0 + 1 taken as z0\'s': ('t.wz1 : t.wz0);\n        out[k]', 't.wz0 : t.wz0);\n        out[k]'),
+    # the normal's zero-padding bands dropped: a point within a slab below slab 0 (or above slab D - 1) reads nothing
+    'zero-padding band below slab 0 dropped': ('(fz > -2.f) &&', '(fz >= 0.f) &&'),
+    'zero-padding band above slab D - 1 dropped': ('(fz < (float)g.D + 1.f)', '(fz < (float)(g.D - 1))'),
+}
+
 # target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
 TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
@@ -119,22 +145,41 @@ TARGETS = {
     'render_backward_multiplane': ('render_backward.cu', 'tests/test_multiplane_paths_gpu.py', RENDER_BACKWARD_MULTIPLANE),
     'modconv': ('modconv.cu', 'tests/test_modconv_gpu.py', MODCONV),
     'render_fused': ('render_fused_ws3.cu', 'tests/test_render_fused_paths_gpu.py', RENDER_FUSED),
+    'multiplane': ('render_device.cuh', 'tests/test_multiplane_paths_gpu.py', MULTIPLANE),
 }
 
 
-def build_mutant(nvcc, d, target, name):
-    """Compile the mutated source into d and link it with the tree's other objects; returns the library's path."""
-    src_name, _, mutations = TARGETS[target]
+def _include_closure(path, seen):
+    """path and every file it reaches through #include "..." lines, added to seen."""
+    if path not in seen and os.path.isfile(path):
+        seen.add(path)
+        for inc in re.findall(r'^\s*#include "([^"]+)"', open(path).read(), re.M):
+            _include_closure(os.path.normpath(os.path.join(os.path.dirname(path), inc)), seen)
+    return seen
+
+
+def units_including(src_name):
+    """The translation units under csrc/ whose #include closure contains csrc/<src_name>; for a .cu source, itself."""
     src = os.path.join(_build.CSRC, src_name)
-    text = open(src).read()
+    return [s for s in _build.sources() if src in _include_closure(s, set())]
+
+
+def build_mutant(nvcc, d, target, name):
+    """Copy csrc/ into d and apply the mutation there, compile every unit that includes the mutated file and link them with
+    the tree's objects for the rest; returns the library's path."""
+    src_name, _, mutations = TARGETS[target]
     old, new = mutations[name]
+    csrc = os.path.join(d, 'csrc')
+    shutil.copytree(_build.CSRC, csrc)
+    path = os.path.join(csrc, src_name)
+    text = open(path).read()
     assert text.count(old) == 1, f'{target}: {name}'
-    os.makedirs(d)
-    cu, obj, lib = os.path.join(d, src_name), os.path.join(d, src_name[:-3] + '.o'), os.path.join(d, 'libp3d.so')
-    open(cu, 'w').write(text.replace(old, new))
-    objs = [obj if s == src else _build.object_path(s) for s in _build.sources()]
-    # -I csrc: the copy finds csrc's headers, and its "../../include/..." resolves from csrc to the repository's include/
-    for cmd in (_build.compile_cmd(nvcc, cu, obj, ['-I', _build.CSRC]), _build.link_cmd(nvcc, lib, objs)):
+    open(path, 'w').write(text.replace(old, new))
+    objs = {s: os.path.join(d, os.path.basename(s)[:-3] + '.o') for s in units_including(src_name)}
+    lib = os.path.join(d, 'libp3d.so')
+    # Each copy's includes find the copied headers first; -I csrc resolves "../../include/..." to the repository's include/.
+    cmds = [_build.compile_cmd(nvcc, os.path.join(csrc, os.path.basename(s)), o, ['-I', _build.CSRC]) for s, o in objs.items()]
+    for cmd in cmds + [_build.link_cmd(nvcc, lib, [objs.get(s, _build.object_path(s)) for s in _build.sources()])]:
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode:
             raise RuntimeError(f'{target}: {name}: nvcc failed\n{r.stdout}')

@@ -1,29 +1,63 @@
-"""CPU: discrete-event simulation of the mbarrier and bulk-copy protocol of the fused renderer (csrc/render_fused_ws3.cu):
-its pass schedule and the hand-off between its 24 warps - 12 gather, 8 decoder (two wgmma warpgroups), 4 ray.  Every role's
-control flow is transcribed from the CUDA source (same loops, same barriers, parities and arrival counts, the same
-placement of colours(n) and its named barriers, the elected threads' bulk groups with their .read and full waits); work
-items get random durations and the runnable warps are stepped in random order, over many seeds and group counts.  Bulk
-copies run asynchronously with random read / write / landing delays, each with a tail longer than a tile, so that a check
-fires whenever the wait guarding it is missing (the negative controls at the end).  Asserted:
+"""CPU: discrete-event simulation of the mbarrier and bulk-copy protocol of the fused renderer (csrc/render_fused_ws3.cu)
+as it is built: its pass schedule and the hand-off between its 24 warps - 12 gather, 8 decoder (two wgmma warpgroups), 4 ray.
+Every role's control flow is transcribed from the CUDA source (same loops, barriers, parities and arrival counts, the
+decoder's elected threads with their bulk stores, .read and full waits, each ray warp's colours() with its own bulk loads);
+the ring sizes and arrival counts are read from the source, so a change there fails here until the model follows.  Work
+items get random durations and the runnable warps are stepped in random order, over many seeds and group counts, at S = 96
+and 48.  Bulk copies run asynchronously with random read / write / landing delays, each with a tail longer than a tile, so
+that a check fires whenever the wait guarding it is missing (the negative controls at the end).  Rows of the colour path
+are tracked in 16-row blocks: warpgroup h stores blocks 4h .. 4h + 3 of a tile, ray warp rw loads blocks 2rw, 2rw + 1
+(S = 96) or rw, rw + 4 (S = 48).  Asserted:
   * no deadlock and no lost mbarrier phase (a waiter that a barrier overtakes by two phases blocks forever), and every
-    group's colours run once;
+    group's colours are reduced by all four ray warps;
   * A1 ring: the gather rewrites a stage only after all eight decoder warps have read its previous tile, and a decoder warp
     reads a stage only once all four warps of the team have written it;
   * shared-memory hazards: the ray warps read a pass's sigma only after every decoder warp wrote its rows, a per-group state
-    slot is not rewritten by the gather before its previous group is finished, the omega slot not before its previous
-    group's colours are done, fine depths are read only after importance;
-  * colour path: a warpgroup's staging tile is not rewritten before its last bulk store has read it; no load of a colour
-    area half is issued before the store that wrote it completed; colours(n) reads a col_buf half only after its load
-    landed (complete_tx), and a load does not overwrite a half that colours() is still reading; CA[n % 3] and FA are not
-    rewritten before the loads of their previous group completed.
+    slot is not rewritten by the gather before its previous group is finished, fine depths are read only after importance;
+  * colour path: a warpgroup's staging tile is not rewritten before its last bulk store has read it; a ray warp loads a
+    group's rows only after col_stored fired for the group and the bulk stores of those rows completed; it reads a col_buf
+    tile only after its load landed and reloads it only after reading it; CA[n % 3] and FA[n & 1] blocks are not rewritten
+    before the previous group's loads of them landed.
 It mirrors the protocol, not the arithmetic; parity on hardware is what tests/test_render_gpu.py is for."""
 import heapq
+import os
 import random
+import re
 
 import pytest
 
-K_NA, K_EW, K_RW, K_TEAMS = 4, 8, 4, 3
-K_COL_BUFS = 3                                       # kColBufs
+from panic3d_b200 import _build
+
+with open(os.path.join(_build.CSRC, 'render_fused_ws3.cu')) as _f:
+    SRC = _f.read()
+
+
+def _kernel_constant(name):
+    m = re.search(r'\bconstexpr int (?:\w+ = \d+, )*%s = (\d+)[,;]' % name, SRC)
+    assert m, f'{name} not found in render_fused_ws3.cu'
+    return int(m.group(1))
+
+
+K_GW, K_EW, K_RW, K_TEAMS, K_NA, K_STATES, K_COL_BUFS = (
+    _kernel_constant(n) for n in ('kGW', 'kEW', 'kRW', 'kTeams', 'kNA', 'kStates', 'kColBufs'))
+
+# arrivals per phase of each mbarrier, as the roles below make them
+ARRIVALS = {
+    'a1_full': K_GW // K_TEAMS,                          # every warp of the gather team
+    'a1_empty': K_EW, 'sigc_ready': K_EW, 'sigf_ready': K_EW,          # every decoder warp
+    'fine_ready': K_RW, 'state_free': K_RW,              # every ray warp
+    'col_stored': K_EW // 4,                             # the elected thread of each decoder warpgroup
+    'col_full': 1,                                       # lane 0 of its ray warp, with the bytes of its bulk loads
+}
+
+
+def _mbar_init_counts():
+    """{barrier: arrival count} of the kernel's mbar_init(&sm.<barrier>..., <count>) lines."""
+    counts = {}
+    for name, count in re.findall(r'mbar_init\(&sm\.(\w+)(?:\[\w+\])*, (\w+)\)', SRC):
+        counts.setdefault(name, set()).add(int(count) if count.isdigit() else _kernel_constant(count))
+    assert all(len(c) == 1 for c in counts.values()), counts
+    return {name: c.pop() for name, c in counts.items()}
 
 
 def pass_at(j, N):                                   # render_fused_ws3.cu: pass_at
@@ -83,34 +117,42 @@ class TxBar(Bar):                                    # mbarrier with a transacti
 
 
 class Sim:
-    def __init__(self, N, seed, sig_count=K_EW, first_wait='all', staging_wait=True, colours_k=0):
+    def __init__(self, N, seed, S=96, sig_count=ARRIVALS['sigc_ready'], stored_wait='all', staging_wait=True,
+                 col_stored_wait=True, coarse_guard=True, fine_guard=True, fine_areas=2, reload_after_read=True):
         # The kernel's choices; the other values model bugs that the negative controls below must catch:
-        #   sig_count     arrivals of sigc_ready / sigf_ready (every decoder warp, K_EW)
-        #   first_wait    the bulk wait before a group's first loads: 'all' (wait_group 0) | 'read' (wait_group.read 0)
-        #   staging_wait  the .read wait before a warpgroup rewrites its staging tile
-        #   colours_k     colours(n) runs at the top of tile colours_k of F(n+1) (0: before F(n+1) stores to FA)
-        self.N, self.T, self.rng = N, 6 * N, random.Random(seed)
-        self.first_wait, self.staging_wait, self.colours_k = first_wait, staging_wait, colours_k
-        B = Bar
-        self.a1_full = [B(4) for _ in range(K_NA)]; self.a1_empty = [B(K_EW) for _ in range(K_NA)]
-        self.fine_ready = [B(K_RW) for _ in range(4)]; self.state_free = [B(1) for _ in range(4)]
-        self.sigc_ready = [B(sig_count) for _ in range(4)]; self.sigf_ready = [B(sig_count) for _ in range(4)]
-        self.omega_ready = [B(K_RW) for _ in range(2)]
-        self.col_full = [TxBar(2) for _ in range(K_COL_BUFS)]
+        #   sig_count          arrivals of sigc_ready / sigf_ready (every decoder warp)
+        #   stored_wait        the bulk wait before arriving on col_stored: 'all' (wait_group 0) | 'read' (wait_group.read 0)
+        #   staging_wait       the .read wait before a warpgroup rewrites its staging tile
+        #   col_stored_wait    the ray warps wait on col_stored before their first loads of a group
+        #   coarse_guard       the decoder waits for state_free of group m - 3 before its first store into CA[m % 3]
+        #   fine_guard         ... of group m - 2 before its first store into FA[m % fine_areas]
+        #   fine_areas         fine colour areas (2: FA[n & 1])
+        #   reload_after_read  a ray warp reloads a buffer after reading it (else right after its col_full wait)
+        self.N, self.T, self.S, self.rng = N, 6 * N, S, random.Random(seed)
+        self.stored_wait, self.staging_wait, self.col_stored_wait = stored_wait, staging_wait, col_stored_wait
+        self.coarse_guard, self.fine_guard, self.fine_areas = coarse_guard, fine_guard, fine_areas
+        self.reload_after_read = reload_after_read
+        A = ARRIVALS
+        self.a1_full = [Bar(A['a1_full']) for _ in range(K_NA)]; self.a1_empty = [Bar(A['a1_empty']) for _ in range(K_NA)]
+        self.fine_ready = [Bar(A['fine_ready']) for _ in range(K_STATES)]
+        self.state_free = [Bar(A['state_free']) for _ in range(K_STATES)]
+        self.sigc_ready = [Bar(sig_count) for _ in range(K_STATES)]; self.sigf_ready = [Bar(sig_count) for _ in range(K_STATES)]
+        self.col_stored = [Bar(A['col_stored']) for _ in range(2)]
+        self.col_full = [[TxBar(A['col_full']) for _ in range(K_COL_BUFS)] for _ in range(K_RW)]
         self.now, self.events, self.seq = 0.0, [], 0
         # hazard bookkeeping
         self.a1_tile, self.a1_written, self.a1_read = [None] * K_NA, [0] * K_NA, [0] * K_NA
         self.sigma_writes = {}                        # (group, pass) -> decoder warp-tiles that stored their sigma rows
-        self.colours_done, self.importance_done, self.composite_done = set(), set(), set()
-        self.state_owner = [None] * 4
-        self.slot_owner = [None] * 2
+        self.importance_done, self.colours_done = set(), set()
+        self.colours_warps = {}                       # group -> ray warps that finished its colours
+        self.state_owner = [None] * K_STATES
         self.bulk_groups = [[], []]                   # per warpgroup: its elected thread's bulk-store groups
-        self.area_content = {}                        # (area, half) -> (group, pass, k) whose store completed there
-        self.area_last = {}                           # (area, half) -> (group, pass, k) last stored there
-        self.load_done = set()                        # (group, t, half) whose load landed
-        self.buf = [[None, None] for _ in range(K_COL_BUFS)]      # [b][half] -> (group, t, landed?)
-        self.buf_reads = [[0, 0] for _ in range(K_COL_BUFS)]
-        self.ebar_count, self.ebar_gen = 0, 0
+        self.col_signalled = set()                    # groups whose col_stored phase completed
+        self.area_content = {}                        # (area, block) -> (group, tile) whose store completed there
+        self.area_last = {}                           # (area, block) -> (group, tile) last stored there
+        self.load_done = set()                        # (group, tile, block) whose load landed
+        self.buf = [[None] * K_COL_BUFS for _ in range(K_RW)]          # [warp][b] -> (group, tile, landed?)
+        self.buf_read = [[False] * K_COL_BUFS for _ in range(K_RW)]
         self.wg_count, self.wg_gen = [0, 0], [0, 0]
 
     def dur(self, lo, hi):
@@ -120,28 +162,33 @@ class Sim:
         self.seq += 1
         heapq.heappush(self.events, (self.now + dt, self.seq, fn))
 
-    @staticmethod
-    def area(n, p, k):
-        return ('CA', n % 3, k) if p == 0 else ('FA', k)
+    def area(self, n, p, k):
+        return ('CA', n % 3, k) if p == 0 else ('FA', n % self.fine_areas, k)
 
-    # ---------------------------------------------------------------- bulk copies of the elected thread of warpgroup h
-    def bulk_store(self, h, n, p, k):
-        key = (self.area(n, p, k), h)
-        prev = self.area_last.get(key)
-        if prev is not None:
-            m, pp, kk = prev
-            assert (m, 3 * pp + kk, h) in self.load_done, f'{key} of group {m} overwritten before its load completed'
-        self.area_last[key] = (n, p, k)
+    def blocks(self, rw):
+        return (2 * rw, 2 * rw + 1) if self.S == 96 else (rw, rw + K_RW)
+
+    # ---------------------------------------------------------------- bulk copies
+    def bulk_store(self, h, n, p, k):                # elected thread of warpgroup h: blocks 4h .. 4h + 3 of tile k
+        area = self.area(n, p, k)
+        kind = 'coarse' if p == 0 else 'fine'
+        for blk in range(4 * h, 4 * h + 4):
+            prev = self.area_last.get((area, blk))
+            if prev is not None:
+                m, t = prev
+                assert (m, t, blk) in self.load_done, f'{kind} area {area} block {blk} of group {m} overwritten before its load landed'
+            self.area_last[(area, blk)] = (n, 3 * p + k)
         rec = {'read': False, 'all': False}
         self.bulk_groups[h].append(rec)
         # Each delay of a bulk copy is usually short and now and then (a busy SM or a congested L2) much longer than a tile,
-        # so that every hazard check below can fire when the wait that guards it is missing.
+        # so that every hazard check can fire when the wait that guards it is missing.
         t_read = self.dur(0.05, 1.0) if self.rng.random() < 0.9 else self.dur(1.0, 20.0)
         self.later(t_read, lambda: rec.__setitem__('read', True))
 
         def written():
             rec['all'] = True
-            self.area_content[key] = (n, p, k)
+            for blk in range(4 * h, 4 * h + 4):
+                self.area_content[(area, blk)] = (n, 3 * p + k)
         self.later(t_read + (self.dur(0.05, 4.0) if self.rng.random() < 0.9 else self.dur(4.0, 40.0)), written)
 
     def bulk_wait(self, h, kind):                    # cp.async.bulk.wait_group{.read} 0
@@ -149,36 +196,41 @@ class Sim:
         if kind == 'all':
             self.bulk_groups[h] = []
 
-    def bulk_load(self, h, n, t):
+    def ray_load(self, rw, n, t):                    # lane 0 of ray warp rw: its blocks of tile t into col_buf[t % kColBufs]
         p, k = divmod(t, 3)
-        b, key = t % K_COL_BUFS, (self.area(n, p, k), h)
-        assert self.area_content.get(key) == (n, p, k), f'load of {key} for group {n} issued before its store completed'
-        assert self.buf[b][h] is None or self.buf_reads[b][h] == 4, f'col_buf[{b}] half {h} reloaded while colours() reads it'
-        self.col_full[b].arrive_expect_tx()
-        self.buf[b][h], self.buf_reads[b][h] = (n, t, False), 0
+        b, area = t % K_COL_BUFS, self.area(n, p, k)
+        blocks = self.blocks(rw)
+        assert n in self.col_signalled, f'load of {area} for group {n} (warp {rw}) issued before col_stored signalled the group'
+        assert all(self.area_content.get((area, blk)) == (n, t) for blk in blocks), \
+            f'load of {area} for group {n} (warp {rw}) issued before the bulk stores of its rows completed'
+        assert self.buf[rw][b] is None or self.buf_read[rw][b], f'col_buf[{b}] rows of warp {rw} reloaded before it read them'
+        self.col_full[rw][b].arrive_expect_tx()
+        self.buf[rw][b], self.buf_read[rw][b] = (n, t, False), False
 
         def landed():
-            self.buf[b][h] = (n, t, True)
-            self.load_done.add((n, t, h))
-            self.col_full[b].complete_tx()
+            self.buf[rw][b] = (n, t, True)
+            for blk in blocks:
+                self.load_done.add((n, t, blk))
+            self.col_full[rw][b].complete_tx()
         self.later(self.dur(0.2, 3.0) if self.rng.random() < 0.9 else self.dur(3.0, 30.0), landed)
 
     # ---------------------------------------------------------------- roles (generators yield ('wait', bar, parity) |
-    # ('until', predicate) | ('work', dt) | ('ebar',) | ('wgbar', warpgroup))
+    # ('until', predicate) | ('work', dt) | ('wgbar', warpgroup))
     def gather_warp(self, gw):
-        team, it = gw >> 2, 0
+        team, it = gw // (K_GW // K_TEAMS), 0
         for q in range(self.T):
             n, p, k = tile_at(q, self.N)
             my_it = it; it += 1
             if my_it % K_TEAMS != team:
                 continue
+            si, par = n % K_STATES, (n // K_STATES) & 1
             if p == 0:
-                yield ('wait', self.state_free[n & 3], ((n >> 2) & 1) ^ 1)
-                prev = self.state_owner[n & 3]
+                yield ('wait', self.state_free[si], par ^ 1)
+                prev = self.state_owner[si]
                 assert prev is None or prev == n or prev in self.colours_done, f'state slot of group {prev} rewritten for {n}'
-                self.state_owner[n & 3] = n
+                self.state_owner[si] = n
             else:
-                yield ('wait', self.fine_ready[n & 3], (n >> 2) & 1)
+                yield ('wait', self.fine_ready[si], par)
                 assert n in self.importance_done, f'fine gather of {n} before its importance sampling'
             stage = my_it % K_NA
             yield ('wait', self.a1_empty[stage], ((my_it // K_NA) & 1) ^ 1)
@@ -191,51 +243,30 @@ class Sim:
 
     def decoder_warp(self, e):
         h, elect = e >> 2, (e & 3) == 0
-        mark = {'stored': -1, 'loaded': -1}
+        mark = {'stored': -1, 'signalled': -1}       # last group whose fine pass was stored / signalled
 
-        def first_loads(n):
+        def signal_stored():
             if elect:
-                yield from self.bulk_wait(h, self.first_wait)
-                for t in range(K_COL_BUFS):
-                    self.bulk_load(h, n, t)
-            mark['loaded'] = n
-
-        def colours(n):
-            if mark['loaded'] < n:
-                yield from first_loads(n)
-            yield ('wait', self.omega_ready[n & 1], (n >> 1) & 1)
-            assert n in self.composite_done and self.slot_owner[n & 1] == n
-            for t in range(6):
-                b = t % K_COL_BUFS
-                yield ('wait', self.col_full[b], ((6 * n + t) // K_COL_BUFS) & 1)
-                assert self.buf[b][h] == (n, t, True), f'colours({n}) reads col_buf[{b}] before tile {t} landed'
-                yield ('work', self.dur(0.2, 1.5))
-                assert self.buf[b][h] == (n, t, True), f'col_buf[{b}] changed while colours({n}) read it'
-                self.buf_reads[b][h] += 1
-                if t + K_COL_BUFS < 6:
-                    yield ('wgbar', h)
-                    if elect:
-                        self.bulk_load(h, n, t + K_COL_BUFS)
-            yield ('ebar',)
-            yield ('work', self.dur(0.1, 0.5))
-            yield ('ebar',)
-            if e == 0:
-                self.colours_done.add(n)
-                self.state_free[n & 3].arrive()
+                yield from self.bulk_wait(h, self.stored_wait)
+                bar, n = self.col_stored[mark['stored'] & 1], mark['stored']
+                phase = bar.phase
+                bar.arrive()
+                if bar.phase != phase:
+                    self.col_signalled.add(n)
+            mark['signalled'] = mark['stored']
 
         for it in range(self.T):
             n, p, k = tile_at(it, self.N)
-            if p == 1 and k == self.colours_k and n >= 1:
-                yield from colours(n - 1)
             stage = it % K_NA
             yield ('wait', self.a1_full[stage], (it // K_NA) & 1)
-            assert self.a1_tile[stage] == it and self.a1_written[stage] == 4, f'decoder reads A1 stage {stage} before tile {it} is complete'
+            assert self.a1_tile[stage] == it and self.a1_written[stage] == ARRIVALS['a1_full'], \
+                f'decoder reads A1 stage {stage} before tile {it} is complete'
             yield ('work', self.dur(0.5, 2))          # layer 1 (wgmma from shared memory)
             self.a1_read[stage] += 1
             self.a1_empty[stage].arrive()
             yield ('work', self.dur(1, 4))            # softplus, layer 2 from registers
-            if mark['stored'] > mark['loaded']:
-                yield from first_loads(mark['stored'])
+            if mark['stored'] > mark['signalled']:
+                yield from signal_stored()
             elif elect and self.staging_wait:
                 yield from self.bulk_wait(h, 'read')
             yield ('wgbar', h)
@@ -244,17 +275,38 @@ class Sim:
             self.sigma_writes[(n, p)] = self.sigma_writes.get((n, p), 0) + 1
             yield ('wgbar', h)
             if elect:
+                prev = n - (3 if p == 0 else 2)
+                if k == 0 and prev >= 0 and (self.coarse_guard if p == 0 else self.fine_guard):
+                    yield ('wait', self.state_free[prev % K_STATES], (prev // K_STATES) & 1)
                 self.bulk_store(h, n, p, k)
             if k == 2:
                 if p == 1:
                     mark['stored'] = n
-                (self.sigc_ready if p == 0 else self.sigf_ready)[n & 3].arrive()
-        yield from colours(self.N - 1)
+                (self.sigc_ready if p == 0 else self.sigf_ready)[n % K_STATES].arrive()
+        yield from signal_stored()
+
+    def colours(self, rw, n):
+        if self.col_stored_wait:
+            yield ('wait', self.col_stored[n & 1], (n >> 1) & 1)
+        for t in range(K_COL_BUFS):
+            self.ray_load(rw, n, t)
+        for t in range(6):
+            b = t % K_COL_BUFS
+            yield ('wait', self.col_full[rw][b], ((6 * n + t) // K_COL_BUFS) & 1)
+            assert self.buf[rw][b] == (n, t, True), f'colours({n}) of warp {rw} reads col_buf[{b}] before tile {t} landed'
+            if not self.reload_after_read and t + K_COL_BUFS < 6:
+                self.ray_load(rw, n, t + K_COL_BUFS)
+            yield ('work', self.dur(0.2, 1.5))
+            assert self.buf[rw][b] == (n, t, True), f'col_buf[{b}] of warp {rw} changed while colours({n}) read it'
+            self.buf_read[rw][b] = True
+            if self.reload_after_read and t + K_COL_BUFS < 6:
+                self.ray_load(rw, n, t + K_COL_BUFS)
+        yield ('work', self.dur(0.1, 0.5))            # the warp's out_rgb rows
 
     def ray_warp(self, rw):
         for j in range(2 * self.N):
             n, p = pass_at(j, self.N)
-            si, par = n & 3, (n >> 2) & 1
+            si, par = n % K_STATES, (n // K_STATES) & 1
             if p == 0:
                 yield ('wait', self.sigc_ready[si], par)
                 assert self.sigma_writes.get((n, 0), 0) == 3 * K_EW, f'importance({n}) before every coarse sigma was stored'
@@ -265,25 +317,21 @@ class Sim:
             else:
                 yield ('wait', self.sigf_ready[si], par)
                 assert self.sigma_writes.get((n, 1), 0) == 3 * K_EW, f'composite({n}) before every fine sigma was stored'
-                if n >= 2:
-                    yield ('wait', self.state_free[(n - 2) & 3], ((n - 2) >> 2) & 1)
-                    assert (n - 2) in self.colours_done
-                prev = self.slot_owner[n & 1]
-                assert prev is None or prev == n or prev in self.colours_done, f'omega slot of group {prev} rewritten for {n}'
-                self.slot_owner[n & 1] = n
-                yield ('work', self.dur(2, 12))
-                if rw == 0:
-                    self.composite_done.add(n)
-                self.omega_ready[n & 1].arrive()
+                yield ('work', self.dur(2, 12))       # composite: omega / pos of the warp's own rays
+                yield from self.colours(rw, n)
+                self.colours_warps[n] = self.colours_warps.get(n, 0) + 1
+                if self.colours_warps[n] == K_RW:
+                    self.colours_done.add(n)
+                self.state_free[si].arrive()
 
     def procs(self):
-        return ([('G%d' % g, self.gather_warp(g)) for g in range(12)] + [('E%d' % e, self.decoder_warp(e)) for e in range(K_EW)] +
+        return ([('G%d' % g, self.gather_warp(g)) for g in range(K_GW)] + [('E%d' % e, self.decoder_warp(e)) for e in range(K_EW)] +
                 [('R%d' % r, self.ray_warp(r)) for r in range(K_RW)])
 
     # ---------------------------------------------------------------- scheduler
     def run(self):
         procs = self.procs()
-        state = {name: ('ready', None) for name, _ in procs}          # ready | wait | until | sleep | ebar | wgbar | done
+        state = {name: ('ready', None) for name, _ in procs}          # ready | wait | until | sleep | wgbar | done
         gens = dict(procs)
 
         def step(name):
@@ -297,23 +345,17 @@ class Sim:
             elif op[0] == 'work':
                 state[name] = ('sleep', None)
                 self.later(op[1], lambda name=name: state.__setitem__(name, ('ready', None)))
-            elif op[0] == 'wgbar':
+            else:                                    # bar.sync of the warpgroup's four warps
                 h = op[1]
                 self.wg_count[h] += 1
                 state[name] = ('wgbar', (h, self.wg_gen[h]))
                 if self.wg_count[h] == 4:
                     self.wg_count[h] = 0
                     self.wg_gen[h] += 1
-            else:
-                self.ebar_count += 1
-                state[name] = ('ebar', self.ebar_gen)
-                if self.ebar_count == K_EW:
-                    self.ebar_count = 0
-                    self.ebar_gen += 1
 
         def runnable(st, arg):
             return (st == 'ready' or (st == 'wait' and arg[0].passed(arg[1])) or (st == 'until' and arg[0]())
-                    or (st == 'ebar' and arg != self.ebar_gen) or (st == 'wgbar' and arg[1] != self.wg_gen[arg[0]]))
+                    or (st == 'wgbar' and arg[1] != self.wg_gen[arg[0]]))
         guard = 0
         while True:
             guard += 1
@@ -348,40 +390,41 @@ def test_pass_schedule_visits_every_group_once_in_a_valid_order():
                 assert pos[(n + 1, 0)] < pos[(n, 1)]                               # >= one pass of slack for importance(n)
 
 
+def test_model_sizes_and_arrival_counts_are_the_kernels():
+    assert (K_GW, K_EW, K_RW, K_TEAMS, K_NA, K_STATES, K_COL_BUFS) == (12, 8, 4, 3, 3, 4, 2)
+    assert 6 % K_COL_BUFS == 0          # colours() walks a group's six tiles through the buffers in whole rounds
+    assert _mbar_init_counts() == ARRIVALS
+
+
+@pytest.mark.parametrize('S', [96, 48])
 @pytest.mark.parametrize('N', [1, 2, 3, 4, 5, 7, 8, 13])
-def test_protocol_has_no_deadlock_or_hazard(N):
+def test_protocol_has_no_deadlock_or_hazard(N, S):
     # 24 distinct seeds (the two progressions share s = 0)
     for seed in [s * 101 + N for s in range(12)] + [s * 131 + N for s in range(1, 13)]:
-        Sim(N, seed).run()
+        Sim(N, seed, S=S).run()
 
 
-def test_simulation_catches_a_short_sigma_hand_off():
-    """The model is not vacuous: with half the decoder warps counted on sigc_ready / sigf_ready (the arrival count of the
-    earlier design, where four warps read sigma back) the ray warps start on sigma that is not all stored yet."""
-    with pytest.raises(AssertionError, match='sigma was stored'):
-        for seed in range(40):
-            Sim(4, seed, sig_count=4).run()
-
-
-def test_simulation_catches_a_read_only_wait_before_the_loads():
-    """With only a .read wait (the staging tile is free, the global writes may still be in flight) before a group's first
-    loads, a load starts on a colour area half that is not written yet."""
-    with pytest.raises(AssertionError, match='issued before its store completed'):
-        for seed in range(40):
-            Sim(4, seed, first_wait='read').run()
-
-
-def test_simulation_catches_a_missing_staging_wait():
-    """Without the .read wait before the epilogue, a warpgroup rewrites its staging tile while the bulk store of the
-    previous tile may still be reading it."""
-    with pytest.raises(AssertionError, match='rewritten before its bulk store read it'):
-        for seed in range(40):
-            Sim(4, seed, staging_wait=False).run()
-
-
-def test_simulation_catches_colours_after_the_fine_area_is_rewritten():
-    """With colours(n) one tile later (at the top of F(n+1)'s second tile), F(n+1)'s first tile is stored to the fine area
-    before colours(n) has loaded group n's copy of it."""
-    with pytest.raises(AssertionError, match='overwritten before its load completed'):
-        for seed in range(40):
-            Sim(4, seed, colours_k=1).run()
+@pytest.mark.parametrize('kw, match', [
+    # with four of the eight decoder warps counted on sigc_ready / sigf_ready, the ray warps start on sigma not all stored
+    pytest.param(dict(sig_count=4), r'before every (coarse|fine) sigma was stored', id='short_sigma_hand_off'),
+    # with only a .read wait before col_stored (the staging tile is free, the global writes may still be in flight), a ray
+    # warp loads colours whose stores have not completed
+    pytest.param(dict(stored_wait='read'), 'issued before the bulk stores of its rows completed', id='read_wait_before_col_stored'),
+    # without the .read wait before the epilogue, a warpgroup rewrites its staging tile while the previous tile's bulk store
+    # may still be reading it
+    pytest.param(dict(staging_wait=False), 'rewritten before its bulk store read it', id='no_staging_wait'),
+    # without the col_stored wait, a ray warp loads colours before the decoder signalled them
+    pytest.param(dict(col_stored_wait=False), 'issued before col_stored signalled the group', id='no_col_stored_wait'),
+    # without the coarse area's guard, C(m) overwrites CA[m % 3] while group m - 3's loads may be in flight
+    pytest.param(dict(coarse_guard=False), r'coarse area .* overwritten before its load landed', id='no_coarse_guard'),
+    # a reload issued right after the col_full wait overwrites rows the warp has not read
+    pytest.param(dict(reload_after_read=False), 'reloaded before it read them', id='reload_before_read'),
+    # with a single fine area and no guard, F(m + 1) overwrites it while group m's loads may be in flight
+    pytest.param(dict(fine_areas=1, fine_guard=False), r"fine area \('FA', 0, \d\) .* overwritten before its load landed", id='one_fine_area_unguarded'),
+])
+@pytest.mark.parametrize('S', [96, 48])
+def test_simulation_catches_each_protocol_bug(kw, match, S):
+    # the coarse areas have about five tiles of slack, so their hazard needs a long bulk-copy tail: up to 200 seeds
+    with pytest.raises(AssertionError, match=match):
+        for seed in range(200):
+            Sim(13, seed, S=S, **kw).run()

@@ -66,7 +66,7 @@ CASES = {
     'train_d3_cull': dict(TRAIN, D=3, flags=dict(triplane_crop=0.1, cull_clouds=0.5), centre_cull=0.5),
     # one spin12-like view and one from above, so that samples leave the box along every plane's normal
     'slabs_d4': dict(N=2, R=32, S=48, Sf=48, H=96, W=64, D=4, views=((0.0, 30.0), (75.0, 0.0))),
-    'contention_d2': dict(N=2, R=64, S=48, Sf=48, H=13, W=9, D=2),     # H >= W in every case (run_mutations_multiplane)
+    'contention_d2': dict(N=2, R=64, S=48, Sf=48, H=13, W=9, D=2),     # H >= W in every case (run_mutations.py multiplane)
     'auto_eg3d_d2': dict(N=2, R=32, S=48, Sf=48, H=64, W=64, D=2, opts=dict(ray_start='auto', ray_end='auto', white_back=False),
                          eg3d=True, lr_mul=0.5),
     'strided_d2': dict(N=2, R=32, S=48, Sf=48, H=64, W=48, D=2, strided=True),
