@@ -22,33 +22,24 @@ must be exactly one launch in profile slot 0.
 Reference: oracle/renderer_oracle.py (manual gather) and oracle/volume_oracle.py in float64 on the GPU, at most 2^19
 points at a time.  test_gpu_fp64_oracle_equals_cpu_oracle pins that run to the CPU fp32 oracle that the reference
 fixtures pin.  Bars: mode 1 (3-pass split bf16) 1e-4 abs, the project's bar for the decode; mode 2 per point, see
-`_single_pass_bars`.  Run with -s to see the worst error / bar of every comparison.
+`single_pass_bars` (tests/render_abi.py).  Run with -s to see the worst error / bar of every comparison.
 """
 import ctypes as C
 import functools
-import math
 
-import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import renderer_oracle as orc, volume_oracle as vo
-from tests.helpers import profiled
-from tests.test_render_gpu import make_decoder
+from tests import render_abi as ra
+from tests.render_abi import BAR, BW, DEV, PROF_SAMPLE_DECODE, Worst, dec64, decode_points, n_sm, single_pass_bars
 
 pytestmark = pytest.mark.gpu
-DEV = 'cuda:0'
-PROF_SAMPLE_DECODE = 0            # profile slot (csrc/p3d_common.cuh)
 N_TEAMS, N_STAGES = 3, 4          # decode_tc.cu:24 kTeams, :27 kNA
 TILE = 128
 CHUNK = 1 << 19                   # points per oracle call
-BAR = 1e-4                        # mode 1 vs the fp64 oracle
-BW = orc.DEFAULT_OPTS['box_warp']
 NV, H, W = 3, 64, 80              # views; plane size (H != W, W not a power of two)
 CROP, CULL = 0.1, 0.35
-U_BF16 = 2.0 ** -8                # unit roundoff of bf16 (8 significant bits, round to nearest)
-LOG2E, LN2 = 1.0 / math.log(2.0), math.log(2.0)
 DEPTH_K = (0, 1, 2, 3, 4, 8)
 # k -> (gather teams, ring stages, parity flips) that the deepest CTA reaches
 REACH = {0: (1, 1, 0), 1: (2, 2, 0), 2: (3, 3, 0), 3: (3, 4, 0), 4: (3, 4, 1), 8: (3, 4, 2)}
@@ -58,10 +49,6 @@ FP32_PIN = 2e-6                   # fp64 device oracle vs the CPU fp32 one: the 
 # further from the oracle than 3-pass's, so proportionally more points lie within its error of the cull threshold
 BORDER_SHARE = {1: 1e-3, 2: 1e-2}
 FREE_BYTES_256 = 12 << 30         # outputs of two 256^3 runs with rgb (2 x 2.5 GB) + oracle chunks, with margin
-
-
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def _schedule(n_tiles, sms):
@@ -87,18 +74,6 @@ def _volume_dest(n, R):
 
 
 # ------------------------------------------------------------------------------------------------- inputs
-@functools.lru_cache(maxsize=None)
-def _planes_and_decoder(seed, n=NV):
-    rng = np.random.default_rng(seed)
-    planes = torch.from_numpy(rng.standard_normal((n, 3, 32, H, W), dtype=np.float32))
-    _, dec, *_ = orc.synth_inputs(seed, 1, 1, 2, 0, 2)
-    return planes, dec
-
-
-def _dec64(dec):
-    return {k: (v.to(DEV, torch.float64) if torch.is_tensor(v) else v) for k, v in dec.items()}
-
-
 def _points(seed, n, k):
     """test_plane_variants_gpu._points scaled up: random points in and around the box, 1/16 of them on each face of the box
     (grid coordinate exactly +-1) and eight far outside, shuffled so every tile and lap gets some of each."""
@@ -144,77 +119,23 @@ def _centre_sigma_on_cull(planes, dec):
     """Shift the sigma bias so that the median sigma of a 33^3 lattice sits at the cull threshold (the density of the
     density falls below 0.35 for sigma < ~0.52), so the cull mask both keeps and removes points."""
     pts = vo.create_samples(33, BW).to(DEV, torch.float64).expand(planes.shape[0], -1, -1)
-    _, sig = orc.run_model(planes.to(DEV, torch.float64), _dec64(dec), pts, orc.DEFAULT_OPTS, True)
+    _, sig = orc.run_model(planes.to(DEV, torch.float64), dec64(dec), pts, orc.DEFAULT_OPTS, True)
     dec = dict(dec, b2=dec['b2'].clone())
     dec['b2'][0] += 0.52 - sig.median().item()
     return dec
 
 
 # ------------------------------------------------------------------------------------------------- the kernel, through the C ABI
-def _renderer(bf16, mode):
-    from panic3d_b200.training.volumetric_rendering.renderer import ImportanceRenderer
-    r = ImportanceRenderer(use_triplane=True)
-    r.planes_bf16 = bf16
-    r.mlp_mode = mode
-    return r
-
-
-def _params(r, cl, decoder, n_points):
-    """p3d_render_params as run_model / query_volume make them; 'auto' must pick the tensor-core decode for them."""
-    from panic3d_b200 import _lib
-    mode, r.mlp_mode = r.mlp_mode, 'auto'
-    p, _ = r._params(cl, cl.shape[0], 0, dict(orc.DEFAULT_OPTS), decoder, None, None, None, n_points=n_points)
-    assert p.mlp_mode == _lib.P3D_MLP_TC_3XBF16
-    r.mlp_mode = mode
-    p, wts = r._params(cl, cl.shape[0], 0, dict(orc.DEFAULT_OPTS), decoder, None, None, None, n_points=n_points)
-    assert p.mlp_mode == mode
-    return p, [t.detach().float().contiguous() for t in wts]
-
-
-def _twice(call, outs):
-    """call() twice into NaN-prefilled `outs`: exactly one decode launch each, bit-identical results."""
-    runs = []
-    for _ in range(2):
-        for t in outs:
-            if t is not None:
-                t.fill_(float('nan'))
-        torch.cuda.synchronize()
-        _, prof = profiled(call)
-        assert prof[PROF_SAMPLE_DECODE] == 1, prof
-        runs.append([None if t is None else t.clone() for t in outs])
-    for a, b in zip(*runs):
-        assert (a is None and b is None) or torch.equal(a, b), 'two runs differ'
-    return runs[0]
-
-
-def _decode_points(x, dec, coords, mode, bf16=False):
-    """p3d_decode_points on planes `x` (device, any layout) -> rgb (N,K,32), sigma (N,K,1)."""
-    from panic3d_b200 import _lib
-    N, K, _ = coords.shape
-    r = _renderer(bf16, mode)
-    decoder = make_decoder(dec, DEV)
-    with torch.no_grad(), torch.cuda.device(DEV):
-        cl = r._planes_cl(x)
-        p, wt = _params(r, cl, decoder, N * K)
-        c = coords.to(DEV).contiguous()
-        rgb = torch.empty((N, K, 32), device=DEV)
-        sigma = torch.empty((N, K, 1), device=DEV)
-        call = lambda: _lib.check(_lib.lib().p3d_decode_points(
-            C.byref(p), cl.data_ptr(), *[t.data_ptr() for t in wt], c.data_ptr(), K, rgb.data_ptr(), sigma.data_ptr(),
-            _lib.stream_ptr(DEV)))
-        return _twice(call, [rgb, sigma])
-
-
 def _volume_query(planes, dec, R, crop, cull, mode, want_rgb=True):
     """p3d_volume_query -> sigma, rgb, density, coordinates as (N, R, R, R, c) buffers (element (a, b, c) = sample
     volume_dest(a R^2 + b R + c))."""
     from panic3d_b200 import _lib
     N = planes.shape[0]
-    r = _renderer(False, mode)
-    decoder = make_decoder(dec, DEV)
+    r = ra.renderer(False, mode)
+    decoder = ra.make_decoder(dec, DEV)
     with torch.no_grad(), torch.cuda.device(DEV):
         cl = r._planes_cl(planes.to(DEV))
-        p, wt = _params(r, cl, decoder, N * R ** 3)
+        p, wt = ra.decode_params(r, cl, decoder, N * R ** 3)
         sig, dens = (torch.empty((N, R, R, R, 1), device=DEV) for _ in range(2))
         rgb = torch.empty((N, R, R, R, 32), device=DEV) if want_rgb else None
         xyz = torch.empty((N, R, R, R, 3), device=DEV)
@@ -222,99 +143,10 @@ def _volume_query(planes, dec, R, crop, cull, mode, want_rgb=True):
             C.byref(p), cl.data_ptr(), *[t.data_ptr() for t in wt], R, float(BW), -1.0 if crop is None else float(crop),
             -1.0 if cull is None else float(cull), sig.data_ptr(), _lib.ptr(rgb), dens.data_ptr(), xyz.data_ptr(),
             _lib.stream_ptr(DEV)))
-        out = _twice(call, [sig, rgb, dens, xyz])
+        out = ra.twice(call, [sig, rgb, dens, xyz], PROF_SAMPLE_DECODE)[0]
     for t in out:
         assert t is None or not torch.isnan(t).any(), 'an output element was never written'
     return out
-
-
-# ------------------------------------------------------------------------------------------------- bars
-def _single_pass_bars(p64, d64, x64):
-    """Per-point bars (rgb (N,K,32), sigma (N,K,1)) for mlp_mode 2, from the roundings the kernel makes.
-
-    The kernel decodes in base 2 (fused_common.cuh stage_w1_biases / stage_w2): the A1 row a is the sum of the three
-    planes' bilinear features, W1' = W1 g1 log2(e) / 3, b1' = b1 g1' log2(e), x' = a W1'^T + b1', h' = softplus2(x') =
-    log2(1 + 2^x') = softplus(x) log2(e); sigma = h' . (W2_0 g2 ln 2) + b2_0, colour = rcp(1 + ex2(h' . (-W2_c g2) + b2c')).
-    Single pass multiplies only the bf16 `hi` halves (split2 / split1): a, W1', h' and W2' are each rounded to bf16, u =
-    2^-8 relative each, so a product of two rounded operands is off by at most e = 2u + u^2 of |product|:
-      layer 1:  |dx'_j| <= e (|a| . |W1'_j|)
-      hidden:   softplus2' = sigmoid <= 1, so |dh'_j| <= |dx'_j|; the rounded h'~ times rounded W2' is then off by
-                dh_j = e |h'_j| + (1 + e) |dx'_j| per unit |W2'|
-      sigma:    ln 2 * sum_j |W2_0j g2| dh_j
-      colour:   |d(1.002 s - 0.001) / d logit'| <= 1.002 ln 2 / 4, times sum_j |W2_cj g2| dh_j
-    plus the fp32 / MUFU term: everything mode 1 also does (fp32 gather and accumulation, ex2 / lg2 / rcp.approx, the
-    biases), which mode 1's bar of 1e-4 covers."""
-    C_ = d64['w1'].shape[1]
-    lr = d64.get('lr_mul', 1.0)
-    g1, g2 = lr / math.sqrt(C_), lr / math.sqrt(d64['w2'].shape[1])
-    a = orc.sample_planes(p64, x64, BW, True).sum(1)                          # (N,K,C)
-    w1p = d64['w1'] * (g1 * LOG2E / 3)
-    x2 = a @ w1p.t() + d64['b1'] * (lr * LOG2E)
-    h2 = F.softplus(x2 * LN2) * LOG2E
-    e = 2 * U_BF16 + U_BF16 ** 2
-    dh = e * h2.abs() + (1 + e) * e * (a.abs() @ w1p.abs().t())
-    w2 = (d64['w2'] * g2).abs()
-    return 1.002 * LN2 / 4 * (dh @ w2[1:].t()) + BAR, LN2 * (dh @ w2[:1].t()) + BAR
-
-
-U32 = 2.0 ** -24                  # unit roundoff of fp32
-MUFU_EX2, MUFU_LG2, MUFU_RCP = 2.0 ** -22, 2.0 ** -22, 2.0 ** -23
-
-
-def _three_pass_bars(p64, d64, x64, force_sigmoid=False, use_triplane=True):
-    """Per-point bars (rgb (N,K,32), sigma (N,K,1)) for mlp_mode 1 (3-pass split bf16), at exact fp32 point coordinates.
-    The error of the coordinates themselves (ray_point, the grid transform) is the caller's: it moves the point.
-
-    In the base-2 form of `_single_pass_bars`, with u = 2^-8 (bf16) and v = 2^-24 (fp32):
-      gather    A1 = sum over 3 planes x 4 taps of w t (one fp32 fma chain, weights from three roundings):
-                |dA1_c| <= 16 v sum |w| |t_c|
-      split     an operand x = hi + lo + r, |lo| <= u |x|, |r| <= u |lo| <= u^2 |x|; the kernel forms hi hi + hi lo + lo hi
-                and drops lo lo, r_a b and a r_b: e3 = 3 u^2 (+ O(u^3)) of |a| |b| per product
-      accumulation  fp32 in the wgmma, 3K products: <= 3K v of sum |a| |b| (K = 32 for layer 1, 64 for layer 2)
-      staging   W1' and the biases carry <= 3 roundings (v each) of their own magnitude, W2' <= 2
-      layer 1   |dx'_j| <= (e3 + 100 v) sum_c |A1_c| |W1'_jc| + sum_c |dA1_c| |W1'_jc| + 4 v (|b1'_j| + |x'_j|)
-      hidden    h' = max(x', 0) + lg2(1 + ex2(-|x'|)), slope <= 1: |dh'_j| <= |dx'_j| + (ex2 + 2 v) / ln 2 + lg2 + v |h'_j|
-                with the MUFU bounds of the PTX ISA (ex2.approx.f32: relative error 2^-22, lg2.approx.f32: absolute 2^-22,
-                rcp.approx.f32: 1 ulp = relative 2^-23)
-      layer 2   |dl_k| <= (e3 + 200 v) sum_j |h'_j| |W2'_kj| + sum_j |dh'_j| |W2'_kj| + 3 v (|b2'_k| + |l_k|)
-      sigma     dl_0 (the sigma row is the plain sum)
-      colour    s = rcp(1 + ex2(l')): |ds| <= s (1 - s) (ln 2 |dl| + ex2) + s (v + rcp), times 1.002 for the colour map
-    """
-    C_ = d64['w1'].shape[1]
-    lr = d64.get('lr_mul', 1.0)
-    g1, g2 = lr / math.sqrt(C_), lr / math.sqrt(d64['w2'].shape[1])
-    a = orc.sample_planes(p64, x64, BW, use_triplane).sum(1)                  # (N,K,C)
-    # sum over planes and taps of |w| |t|: the bilinear gather of |planes| (weights are non-negative)
-    a_abs = orc.sample_planes(p64.abs(), x64, BW, use_triplane).sum(1)
-    da = 16 * U32 * a_abs
-    e3 = 3 * U_BF16 ** 2
-    w1p = d64['w1'] * (g1 * LOG2E / 3)
-    b1p = d64['b1'] * (lr * LOG2E)
-    x2 = a @ w1p.t() + b1p
-    dx = (e3 + 100 * U32) * (a.abs() @ w1p.abs().t()) + da @ w1p.abs().t() + 4 * U32 * (b1p.abs() + x2.abs())
-    h2 = F.softplus(x2 * LN2) * LOG2E
-    dh = dx + (MUFU_EX2 + 2 * U32) / LN2 + MUFU_LG2 + U32 * h2.abs()
-    w2p = d64['w2'] * g2
-    w2p = torch.cat([w2p[:1] * LN2, -w2p[1:]], 0)                             # sigma row, then the colour rows
-    b2p = d64['b2'] * lr
-    b2p = torch.cat([b2p[:1], -b2p[1:] * LOG2E], 0)
-    lg = h2 @ w2p.t() + b2p
-    dl = (e3 + 200 * U32) * (h2.abs() @ w2p.abs().t()) + dh @ w2p.abs().t() + 3 * U32 * (b2p.abs() + lg.abs())
-    s = torch.sigmoid(-lg[..., 1:] * LN2)
-    ds = s * (1 - s) * (LN2 * dl[..., 1:] + MUFU_EX2) + s * (U32 + MUFU_RCP)
-    return (ds if force_sigmoid else 1.002 * ds), dl[..., :1]
-
-
-class Worst:
-    """Worst |got - want| and worst |got - want| / bar of one output over pieces; NaN counts as infinitely wrong."""
-
-    def __init__(self):
-        self.err = self.ratio = 0.0
-
-    def add(self, got, want, bar):
-        err = (got.double() - want).abs().nan_to_num(nan=float('inf'))
-        self.err = max(self.err, err.max().item())
-        self.ratio = max(self.ratio, (err / bar).max().item())
 
 
 # ------------------------------------------------------------------------------------------------- oracle pin
@@ -322,10 +154,10 @@ def test_gpu_fp64_oracle_equals_cpu_oracle():
     """The fp64 device run of the oracle (what every test below compares with) equals the CPU fp32 oracle that the
     reference fixtures pin (tests/test_oracle_golden.py, tests/test_volume_oracle_golden.py), within the fp32 run's rounding;
     the chunked volume equals the whole one."""
-    planes, dec = _planes_and_decoder(500, n=2)
+    planes, dec = ra.planes_and_decoder(500, 2, H, W)
     planes = planes[:, :, :, :20, :30].contiguous()
     xyz = _points(500, 2, 600)
-    p64, d64 = planes.to(DEV, torch.float64), _dec64(dec)
+    p64, d64 = planes.to(DEV, torch.float64), dec64(dec)
     for a, b in zip(orc.run_model(p64, d64, xyz.to(DEV, torch.float64), orc.DEFAULT_OPTS, True),
                     orc.run_model(planes, dec, xyz, orc.DEFAULT_OPTS, True)):
         assert a.dtype == torch.float64 and a.device == p64.device
@@ -357,13 +189,13 @@ def _points_case(k):
     assert s['n_my_max'] == k + 1 and s['n_my_min'] == max(k, 1)                    # every last lap is ragged
     assert (s['teams'], s['stages'], s['flips']) == REACH[k], (k, s)
     seed = 600 + k
-    planes, dec = _planes_and_decoder(seed)
+    planes, dec = ra.planes_and_decoder(seed, NV, H, W)
     coords = _points(seed, NV, K)
     return planes, dec, coords, s, _oracle_points(planes, dec, coords)
 
 
 def _oracle_points(planes, dec, coords):
-    p64, d64, x64 = planes.to(DEV, torch.float64), _dec64(dec), coords.to(DEV, torch.float64)
+    p64, d64, x64 = planes.to(DEV, torch.float64), dec64(dec), coords.to(DEV, torch.float64)
     step = CHUNK // coords.shape[0]
     outs = [orc.run_model(p64, d64, x64[:, i:i + step], orc.DEFAULT_OPTS, True) for i in range(0, coords.shape[1], step)]
     return torch.cat([o[0] for o in outs], 1), torch.cat([o[1] for o in outs], 1)
@@ -383,7 +215,7 @@ def _check_points(got, want, bars, tag):
 @pytest.mark.parametrize('k', DEPTH_K)
 def test_points_at_depth_match_fp64_oracle(k):
     planes, dec, coords, s, want = _points_case(k)
-    got = _decode_points(planes.to(DEV), dec, coords, 1)
+    got = decode_points(planes.to(DEV), dec, coords, 1)
     _check_points(got, want, (BAR, BAR), f'points k={k} ({coords.shape[1]} x {NV} points, {s["n_my_max"]} tiles on the '
                                          f'deepest of {s["grid"]} CTAs)')
 
@@ -394,7 +226,7 @@ def test_points_layouts_at_depth_are_bit_identical(bf16):
     buffer (SCOL = 0) give bit-identical outputs for one storage type; bf16 NCHW matches the oracle on the bf16-rounded
     planes."""
     planes, dec, coords, s, want = _points_case(8)
-    outs = {layout: _decode_points(_layout(planes, layout, bf16), dec, coords, 1, bf16=bf16) for layout in LAYOUTS}
+    outs = {layout: decode_points(_layout(planes, layout, bf16), dec, coords, 1, bf16=bf16) for layout in LAYOUTS}
     for layout in LAYOUTS[1:]:
         for a, b in zip(outs['nchw'], outs[layout]):
             assert torch.equal(a, b), f'{layout} differs from nchw (max {(a - b).abs().max().item()})'
@@ -406,10 +238,10 @@ def test_points_layouts_at_depth_are_bit_identical(bf16):
 def test_points_single_pass_at_depth():
     """mlp_mode 2 at k = 8 within its derived per-point bar, and at least 10x further from the oracle than mode 1."""
     planes, dec, coords, s, want = _points_case(8)
-    p64, d64, x64 = planes.to(DEV, torch.float64), _dec64(dec), coords.to(DEV, torch.float64)
-    bars = _single_pass_bars(p64, d64, x64)
-    two = _check_points(_decode_points(planes.to(DEV), dec, coords, 2), want, bars, 'points k=8 single pass')
-    one = _check_points(_decode_points(planes.to(DEV), dec, coords, 1), want, (BAR, BAR), 'points k=8 3-pass')
+    p64, d64, x64 = planes.to(DEV, torch.float64), dec64(dec), coords.to(DEV, torch.float64)
+    bars = single_pass_bars(p64, d64, x64)
+    two = _check_points(decode_points(planes.to(DEV), dec, coords, 2), want, bars, 'points k=8 single pass')
+    one = _check_points(decode_points(planes.to(DEV), dec, coords, 1), want, (BAR, BAR), 'points k=8 3-pass')
     for e2, e1 in zip(two, one):
         assert e2 >= 10 * e1, ('single pass is not reaching the kernel', e2, e1)
 
@@ -428,7 +260,7 @@ def _check_volume(out, planes, dec, R, crop, cull, mode, tag, n_lo=0, n_hi=None,
     sig_k, rgb_k, dens_k, xyz_k = out
     N = planes.shape[0]
     n_hi = R ** 3 if n_hi is None else n_hi
-    p64, d64 = planes.to(DEV, torch.float64), _dec64(dec)
+    p64, d64 = planes.to(DEV, torch.float64), dec64(dec)
     samples = vo.create_samples(R, BW)[:, n_lo:n_hi]
     lim = BW / 2 - crop if crop is not None else None
     ws, wr, wd = Worst(), Worst(), Worst()
@@ -439,7 +271,7 @@ def _check_volume(out, planes, dec, R, crop, cull, mode, tag, n_lo=0, n_hi=None,
             dest = _volume_dest(idx, R)
             assert torch.equal(xyz_k[v].reshape(-1, 3)[dest], x[0].float()), (tag, 'coordinates')
             if mode == 2:
-                bar_rgb, bar_sig = (b[0] for b in _single_pass_bars(p64[v:v + 1], d64, x))
+                bar_rgb, bar_sig = (b[0] for b in single_pass_bars(p64[v:v + 1], d64, x))
             else:
                 bar_rgb = bar_sig = BAR
             g_sig = sig_k[v].reshape(-1, 1)[dest]
@@ -482,7 +314,7 @@ def _check_volume(out, planes, dec, R, crop, cull, mode, tag, n_lo=0, n_hi=None,
 
 @functools.lru_cache(maxsize=None)
 def _volume97_inputs():
-    planes, dec = _planes_and_decoder(700)
+    planes, dec = ra.planes_and_decoder(700, NV, H, W)
     return planes, _centre_sigma_on_cull(planes, dec)
 
 
@@ -509,11 +341,9 @@ def test_volume_single_pass_at_depth():
 
 def test_volume_eval_shape_256():
     """The eval mesh's query: 256^3 x 1 subject (131072 tiles, ~993 per CTA), crop and cull, with colours."""
-    free, _ = torch.cuda.mem_get_info()
-    if free < FREE_BYTES_256:
-        pytest.skip(f'needs {FREE_BYTES_256 >> 30} GB of free device memory, {free >> 30} GB free')
+    ra.skip_unless_free(FREE_BYTES_256)
     R = 256
-    planes, dec = _planes_and_decoder(800, n=1)
+    planes, dec = ra.planes_and_decoder(800, 1, H, W)
     dec = _centre_sigma_on_cull(planes, dec)
     s = _schedule(R ** 3 // TILE, n_sm())
     assert s['n_my_max'] >= 900, s
@@ -531,7 +361,7 @@ def test_volume_lattice_past_2_24():
     from panic3d_b200 import _lib
     R = 257
     assert R ** 3 > 2 ** 24 and (R - 1) ** 3 <= 2 ** 24
-    planes, dec = _planes_and_decoder(900, n=1)
+    planes, dec = ra.planes_and_decoder(900, 1, H, W)
     dec = _centre_sigma_on_cull(planes, dec)
     sig, rgb, dens, xyz = _volume_query(planes, dec, R, None, CULL, 1, want_rgb=False)
     assert rgb is None

@@ -9,22 +9,13 @@ import pytest
 import torch
 
 from oracle import imageio_oracle as io_orc
+from tests.helpers import TinyG, synth_image
 
 
 @pytest.fixture(scope='module')
 def built():
     import __graft_entry__ as g
     g.build()
-
-
-def synth_image(seed, c, h, w):
-    """Smooth gradients + noise + out-of-range values, so every filter type wins on some row and the clamp matters."""
-    g = np.random.Generator(np.random.PCG64(seed))
-    yy, xx = np.meshgrid(np.linspace(0, 1, h), np.linspace(0, 1, w), indexing='ij')
-    img = np.stack([0.5 + 0.6 * np.sin(6 * xx + ch) * np.cos(5 * yy - ch) for ch in range(c)])
-    img[:, h // 3: h // 2] += g.normal(0, 0.3, (c, h // 2 - h // 3, w))
-    img[:, : h // 8] = np.round(img[:, : h // 8] * 4) / 4                 # flat runs
-    return torch.from_numpy(img.astype(np.float32))
 
 
 @pytest.mark.parametrize('c,h,w', [(3, 40, 37), (4, 33, 64), (1, 17, 5)])
@@ -94,24 +85,6 @@ def test_async_pickle_writer(tmp_path):
     w.pdump(obj, tmp_path / 'missing' / 'mc.pkl')
     with pytest.raises(OSError):
         w.flush()
-
-
-class TinyG(torch.nn.Module):
-    """Stand-in with the attributes load_eg3dc_model relies on (init_args / init_kwargs via persistence, eg3dc_v0.py:44-50)."""
-
-    def __init__(self, width, depth=2, rendering_kwargs=None):
-        super().__init__()
-        self.init_args, self.init_kwargs = (width,), {'depth': depth, 'rendering_kwargs': rendering_kwargs}
-        self.layers = torch.nn.ModuleList([torch.nn.Linear(width, width) for _ in range(depth)])
-        self.register_buffer('w_avg', torch.randn(width))
-        self.register_buffer('steps', torch.tensor(7, dtype=torch.int64))
-        self.half_w = torch.nn.Parameter(torch.randn(3, 5).half())
-        self.rendering_kwargs = rendering_kwargs or {}
-        self.neural_rendering_resolution = 64
-        self.force_sigmoid = False
-
-    def set_force_sigmoid(self, s):
-        self.force_sigmoid = s
 
 
 def test_weight_file_round_trip_is_bit_exact(tmp_path):

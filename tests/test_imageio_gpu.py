@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from oracle import imageio_oracle as io_orc
-from tests.test_imageio_cpu import synth_image, TinyG
+from tests.helpers import TinyG, synth_image
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'

@@ -7,7 +7,7 @@ import torch
 from oracle import mesh_oracle as mo
 from tests import mesh_fields as mf
 from tests.golden.cases import VOLUME_CASES, build_case_inputs
-from tests.test_render_gpu import make_decoder
+from tests.render_abi import make_decoder
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'

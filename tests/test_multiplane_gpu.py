@@ -14,6 +14,7 @@ import torch
 from oracle import multiplane_oracle as mo, renderer_oracle as orc
 from tests.golden.cases_multiplane import RENDER_CASES, POINT_CASES, build_inputs, point_coords, upstream
 from tests.helpers import profiled
+from tests.render_abi import decode_points_call, render_forward
 
 pytestmark = pytest.mark.gpu
 
@@ -229,16 +230,14 @@ def _abi_inputs(dev, D, N=1, M=384):
 
 def _abi_render(p, planes_cl, wt, ro, rd):
     from panic3d_b200 import _lib
-    L, dev = _lib.lib(), planes_cl.device
+    dev = planes_cl.device
     N, M = p.n_views, p.n_rays
     out = [torch.empty(sh, device=dev) for sh in ((N, M, 32), (N, M), (N, M), (N, M, 3))]
-    ws = torch.empty(int(L.p3d_render_workspace_bytes(C.byref(p))), dtype=torch.uint8, device=dev)
-    _lib.check(L.p3d_render_forward(C.byref(p), planes_cl.data_ptr(), *[t.data_ptr() for t in wt], ro.data_ptr(), rd.data_ptr(),
-                                    None, None, ws.data_ptr(), ws.numel(), *[o.data_ptr() for o in out], _lib.stream_ptr(dev)))
+    ws = torch.empty(int(_lib.lib().p3d_render_workspace_bytes(C.byref(p))), dtype=torch.uint8, device=dev)
+    render_forward(p, planes_cl, wt, ro, rd, None, None, ws, out)
     pts = ro[:, :200] + 0.9 * rd[:, :200]
     rgb, sig = torch.empty((N, 200, 32), device=dev), torch.empty((N, 200), device=dev)
-    _lib.check(L.p3d_decode_points(C.byref(p), planes_cl.data_ptr(), *[t.data_ptr() for t in wt], pts.contiguous().data_ptr(), 200,
-                                   rgb.data_ptr(), sig.data_ptr(), _lib.stream_ptr(dev)))
+    decode_points_call(p, planes_cl, wt, pts.contiguous(), rgb, sig)
     torch.cuda.synchronize()
     return out + [rgb, sig]
 

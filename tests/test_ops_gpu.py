@@ -8,6 +8,7 @@ import torch
 
 from oracle import ops_oracle as oo
 from tests.golden.cases_ops import BIAS_ACT_CASES, UPFIRDN_CASES, FLRELU_CASES, make_input, make_filter
+from tests.helpers import f32_scalars
 
 pytestmark = pytest.mark.gpu
 G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ops_golden.npz'))
@@ -17,18 +18,6 @@ DEV = 'cuda:0'
 def _ba():
     from panic3d_b200.torch_utils.ops import bias_act
     return bias_act
-
-
-def _f32_scalars(kw, act):
-    """alpha / gain / clamp cross the C ABI as fp32 (as in the reference plugin: bias_act.h:27-29); give the fp64
-    oracle the same rounded scalars so fp64 comparisons can be tight."""
-    _, def_alpha, def_gain = oo.ACTS[act]
-    out = dict(kw)
-    out['alpha'] = float(np.float32(def_alpha if kw.get('alpha') is None else kw['alpha']))
-    out['gain'] = float(np.float32(def_gain if kw.get('gain') is None else kw['gain']))
-    if kw.get('clamp') is not None:
-        out['clamp'] = float(np.float32(kw['clamp']))
-    return out
 
 
 # ------------------------------------------------------------------------------------------ bias_act
@@ -50,7 +39,7 @@ def test_bias_act_dtypes(name, dtype, tol):
     kw = dict(dim=c.get('dim', 1), act=c['act'], alpha=c.get('alpha'), gain=c.get('gain'), clamp=c.get('clamp'))
     xd, bd = x.to(dtype), b.to(dtype)
     y = _ba().bias_act(xd.to(DEV), bd.to(DEV), **kw)
-    ref = oo.bias_act(xd.double(), bd.double(), **_f32_scalars(kw, c['act']))
+    ref = oo.bias_act(xd.double(), bd.double(), **f32_scalars(kw, c['act']))
     assert y.dtype == dtype
     assert (y.cpu().double() - ref).abs().max().item() < tol * max(1.0, ref.abs().max().item())
 
@@ -94,7 +83,7 @@ def test_bias_act_gradients(name):
         g2 = torch.autograd.grad(s, ins, allow_unused=True) if s.requires_grad else [None] * len(ins)
         return [y] + list(g1) + [g for g in g2]
 
-    kw_gpu, kw = kw, _f32_scalars(kw, c['act'])
+    kw_gpu, kw = kw, f32_scalars(kw, c['act'])
     if c['act'] == 'linear' and kw.get('clamp') is not None:
         # quirk of the reference CUDA path that this op reproduces on purpose: 'linear' saves neither x nor y
         # (activation_funcs['linear'].ref == '', bias_act.py:24,153-156), so its backward kernel sees yref = 0 and

@@ -27,7 +27,8 @@ import pytest
 import torch
 
 from oracle import ops_oracle as oo
-from tests.test_ops_gpu import _f32_scalars
+from tests.helpers import f32_scalars
+from tests.render_abi import n_sm
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -38,10 +39,6 @@ EMIN = {F16: -14, BF16: -126, F32: -126, F64: -1022}
 EPS = {F32: 2.0 ** -24, F16: 2.0 ** -24, BF16: 2.0 ** -24, F64: 2.0 ** -53}   # unit roundoff of the accumulation type
 CTAS_PER_SM_MAX = 8       # 256-thread CTAs: 2048 resident threads per SM on H100
 CHUNK = 1 << 23           # elements per piece of a float64 comparison
-
-
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 def min_work():
@@ -158,7 +155,7 @@ def ba_near_kink(x, b, dim, act, kw):
     """Distance of each element from the nearest gate discontinuity minus the required margin (>= 0 is safe)."""
     if act != 'lrelu':
         return torch.ones_like(x, dtype=F64)
-    k = _f32_scalars(kw, act)
+    k = f32_scalars(kw, act)
     s = x.double() + b.double().reshape(_bshape(x.ndim, dim))
     d = s.abs() - 1e-3
     if k.get('clamp') is not None:
@@ -172,7 +169,7 @@ def ba_ref(x, b, dim, kw, act, sl, cdim):
     """fp64 oracle on one slice along cdim (!= dim)."""
     idx = [slice(None)] * x.ndim
     idx[cdim] = sl
-    return oo.bias_act(x[tuple(idx)].double(), b.double(), dim=dim, act=act, **_f32_scalars(kw, act)), tuple(idx)
+    return oo.bias_act(x[tuple(idx)].double(), b.double(), dim=dim, act=act, **f32_scalars(kw, act)), tuple(idx)
 
 
 def ba_compare(name, y, x, b, dim, act, kw, n_ulp=4):
@@ -233,7 +230,7 @@ def test_bias_act_channels_last_at_size(dtype):
 def ba_grad_ref(g, y, kw, act, order, dy=None):
     """The kernel's derivative formulas (ops_bias_act.cu:46-50, 82-85) in float64, gated on the op's own stored y.
     order 1: g * act'(s) * gain, zero where |y| >= clamp; order 2 (tanh): g * act''(s) * gain * dy."""
-    k = _f32_scalars(kw, act)
+    k = f32_scalars(kw, act)
     y = y.double()
     yy = y / k['gain']
     if act == 'lrelu':
@@ -272,7 +269,7 @@ def test_bias_act_row_mode_gradients(act, dtype):
     second = torch.autograd.grad(s, [dy, x, b] if act == 'tanh' else [dy])
     y, dx, db = y.detach(), dx.detach(), db.detach()
     if act == 'lrelu':                                      # the stored y gates like the fp64 pre-activation
-        k = _f32_scalars(kw, act)
+        k = f32_scalars(kw, act)
         s64 = x.detach().double() + b.detach().double().reshape(-1, 1, 1)
         want = (s64 > 0) & ((torch.where(s64 > 0, s64, s64 * k['alpha']) * k['gain']).abs() < k['clamp'])
         got = (y > 0) & (y.double().abs() < k['clamp'])

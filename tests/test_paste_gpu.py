@@ -8,6 +8,7 @@ import torch
 
 from oracle import paste_oracle as po
 from tests.golden.cases_paste import PASTE_CASES, OUT_KEYS, build_paste_inputs
+from tests.helpers import StandInG
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -16,22 +17,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 def load(name):
     return {k: torch.from_numpy(v) for k, v in np.load(os.path.join(HERE, 'golden', f'paste_{name}.npz')).items()}
-
-
-class StandInG:
-    """The same stand-in generator the golden script uses: f() returns the fixed results of the two extra renders."""
-
-    def __init__(self, inp, dev):
-        self.rendering_kwargs = {'ray_start': inp['ray_start'], 'box_warp': inp['box_warp']}
-        self.inp, self.dev, self.seen = inp, dev, {}
-
-    def f(self, xin, return_more=False):
-        if xin.get('force_rays') is not None:
-            assert xin['paste_params'] is None
-            self.seen['occ_ro'], self.seen['occ_rd'] = xin['force_rays']['ray_origins'], xin['force_rays']['ray_directions']
-            return {'image_weights': self.inp['occ'].to(self.dev)}
-        assert float(xin['fovs'][0]) == -1 and 'paste_params' not in xin
-        return {'image_weights': self.inp['frontw'].to(self.dev)}
 
 
 def run_dropin(case, inp):

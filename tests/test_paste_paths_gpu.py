@@ -565,7 +565,7 @@ def test_dropin_paste_front_equals_the_fused_call():
     """panic3d_b200.paste.paste_front(G, x, out, grad_sample=True, **EVAL) at the training size: gradients into
     out['image'] and out['image_xyz'] equal paste_front_fused's (d_xyz up to the order of its atomic sums)."""
     import panic3d_b200.paste as pp
-    from tests.test_paste_gpu import StandInG
+    from tests.helpers import StandInG
     c = CASES['train_agrad']
     inp = _inputs_cpu('train_agrad')
     d = _inputs('train_agrad')

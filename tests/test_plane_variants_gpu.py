@@ -11,14 +11,12 @@ exactly the values the kernels read.
 
 Planes are 20 x 30 texels (W not a multiple of 4, H != W), and the rays / points reach every edge of each plane and
 leave the box, so the clamped 2 x 2 footprints of the gathers are exercised in every layout."""
-import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import renderer_oracle as orc, volume_oracle as vo
 from tests.helpers import profiled
-from tests.test_render_gpu import make_decoder
+from tests.render_abi import box_rays, make_decoder, planes_and_decoder
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -26,22 +24,6 @@ N, H, W = 2, 20, 30
 LAYOUTS = ('nchw', 'channels_last', 'strided64')
 TEXEL_STRIDE = {'nchw': 32, 'channels_last': 96, 'strided64': 64}
 PROF_SAMPLE_DECODE, PROF_FUSED = 0, 5          # profile slots (csrc/p3d_common.cuh)
-
-
-def _planes_and_decoder(seed, n=N, h=H, w=W):
-    rng = np.random.default_rng(seed)
-    planes = torch.from_numpy(rng.standard_normal((n, 3, 32, h, w), dtype=np.float32))
-    _, dec, *_ = orc.synth_inputs(seed, 1, 1, 2, 0, 2)
-    return planes, dec
-
-
-def _rays(seed, n, m):
-    """Origins on the unit sphere aimed at random points of the box: with t in [0.5, 1.5] the samples cross the box and
-    leave it on the far side."""
-    g = torch.Generator().manual_seed(seed)
-    o = F.normalize(torch.randn(n, m, 3, generator=g), dim=-1)
-    target = (torch.rand(n, m, 3, generator=g) * 2 - 1) * 0.3
-    return o.contiguous(), F.normalize(target - o, dim=-1).contiguous()
 
 
 def _noise(seed, n, m, S):
@@ -109,7 +91,7 @@ def _consume(kind, r, x, dec, use_triplane, seed):
     if kind in RENDERERS:
         S = RENDERERS[kind][0]
         opts.update(depth_resolution=S, depth_resolution_importance=S)
-        ro, rd = _rays(seed, N, 64)
+        ro, rd = box_rays(seed, N, 64)
         r.injected_noise = _noise(seed, N, 64, S)
         fn = lambda: r(x, decoder, ro.to(DEV), rd.to(DEV), opts)
     elif kind == 'points':
@@ -127,7 +109,7 @@ def _oracle(kind, planes, dec, use_triplane, seed):
     if kind in RENDERERS:
         S = RENDERERS[kind][0]
         opts.update(depth_resolution=S, depth_resolution_importance=S)
-        ro, rd = _rays(seed, N, 64)
+        ro, rd = box_rays(seed, N, 64)
         u_c, u_f = _noise(seed, N, 64, S)
         return list(orc.render(planes, dec, ro, rd, opts, u_c, u_f, use_triplane=use_triplane))
     if kind == 'points':
@@ -165,7 +147,7 @@ def _assert_close(kind, got, want, tag):
 @pytest.mark.parametrize('kind', CONSUMERS)
 def test_plane_layouts_are_bit_identical_and_match_oracle(kind, bf16, use_triplane):
     seed = 300 + CONSUMERS.index(kind) * 4 + 2 * int(bf16) + int(use_triplane)
-    planes, dec = _planes_and_decoder(seed)
+    planes, dec = planes_and_decoder(seed, N, H, W)
     if kind == 'volume':
         dec = _centre_sigma_on_cull(planes, dec, use_triplane)
     mode = RENDERERS[kind][1] if kind in RENDERERS else 1
@@ -198,7 +180,7 @@ def test_texel_stride_the_fused_kernel_cannot_take(bf16):
     """A texel stride of 36 elements passes the library's 4-element alignment but not the fused renderer's 8-element one:
     mlp_mode 'auto' renders with the SIMT kernels (and still matches the oracle), a forced fused mode raises."""
     seed = 350 + int(bf16)
-    planes, dec = _planes_and_decoder(seed)
+    planes, dec = planes_and_decoder(seed, N, H, W)
     dt = torch.bfloat16 if bf16 else torch.float32
     buf = torch.full((N, 3, H, W, 36), float('nan'), device=DEV, dtype=dt)
     buf[..., :32] = planes.permute(0, 1, 3, 4, 2).to(DEV, dt)
@@ -229,8 +211,8 @@ def _depth_check(S, k, bf16=False, layout='nchw'):
     n_my = (groups + n_sm - 1) // n_sm
     assert n_my == k + 1 and (k == 0 or groups % n_sm != 0)
     seed = 400 + S + k + int(bf16)
-    planes, dec = _planes_and_decoder(seed, h=64, w=64)
-    ro, rd = _rays(seed, N, M)
+    planes, dec = planes_and_decoder(seed, N, 64, 64)
+    ro, rd = box_rays(seed, N, M)
     u_c, u_f = _noise(seed, N, M, S)
     opts = dict(orc.DEFAULT_OPTS, depth_resolution=S, depth_resolution_importance=S)
     x = _layout(planes, layout, bf16)

@@ -12,41 +12,15 @@ import torch
 
 from oracle import renderer_oracle as orc
 from tests.golden.cases import build_case_inputs
-from tests.helpers import case_rays
-from tests.test_render_gpu import make_decoder
+from tests.helpers import BWD_CASES, bwd_case, bwd_flags, bwd_incoming, case_rays
+from tests.render_abi import make_decoder
 
 pytestmark = pytest.mark.gpu
 TIGHT = 1e-4        # forward outputs of the fp32 SIMT path vs the oracle
 GRAD_REL = 2e-3     # gradients: max abs error < GRAD_REL * max(1e-3, max |reference|)
 
 
-def _case(seed, S, Sf, R=15, N=2, opts=None, cameras=None, **kw):
-    o = dict(orc.DEFAULT_OPTS, depth_resolution=S, depth_resolution_importance=Sf)
-    o.update(opts or {})
-    return dict(seed=seed, N=N, R=R, P=64, opts=o, cameras=cameras, **kw)
-
-
-# merged intervals per ray = S + Sf - 1
-BWD_CASES = {
-    'train48': _case(61, 48, 48),                                               # 95: the training setting, three chunks
-    # 191, eval flags: the bias puts the cull threshold (sigma = 1 for cull 0.5) inside the samples' sigma range
-    'eval96': _case(68, 96, 96, R=5, triplane_crop=0.1, cull_clouds=0.5, force_sigmoid=True, sigma_bias=1.04),
-    'ragged31_17': _case(63, 31, 17),                                           # 47: second chunk half full
-    'ragged40_26': _case(64, 40, 26),                                           # 65: third chunk has one live lane
-    'coarse40': _case(65, 40, 0),                                               # 39: coarse-only path crosses a chunk
-    'lrmul_black48': _case(66, 48, 48, lr_mul=0.5, opts=dict(white_back=False)),
-}
-
 PARAMS = ('planes', 'w1', 'b1', 'w2', 'b2')
-
-
-def _flags(case):
-    return dict(triplane_crop=case.get('triplane_crop'), cull_clouds=case.get('cull_clouds'), binarize_clouds=case.get('binarize_clouds'))
-
-
-def _incoming(seed, N, M):
-    rng = np.random.default_rng(seed)
-    return [torch.from_numpy(rng.standard_normal(s).astype(np.float32)) for s in ((N, M, 32), (N, M, 1), (N, M, 1), (N, M, 3))]
 
 
 def _loss(outs, gw):
@@ -96,11 +70,11 @@ def test_multi_chunk_backward_matches_oracle_autograd(name):
         for frac, margin in _cull_census(case, planes, dec, ro, rd, u_c, u_f, opts):
             print(f'{name}: cull removes {frac:.3f} of the uncropped samples; closest sigma {margin:.2e} from the threshold')
             assert 0.05 < frac < 0.95 and margin > 1e-4, (frac, margin)
-    gw = _incoming(case['seed'] + 5, N, M)
+    gw = bwd_incoming(case['seed'] + 5, N, M)
 
     pl = planes.clone().requires_grad_(True)
     dref = {k: (v.clone().requires_grad_(True) if isinstance(v, torch.Tensor) else v) for k, v in dec.items()}
-    out = orc.render(pl, dref, ro, rd, opts, u_c, u_f if Sf > 0 else None, use_triplane=True, **_flags(case))
+    out = orc.render(pl, dref, ro, rd, opts, u_c, u_f if Sf > 0 else None, use_triplane=True, **bwd_flags(case))
     ref = torch.autograd.grad(_loss(out, gw), [pl, dref['w1'], dref['b1'], dref['w2'], dref['b2']])
 
     dev = torch.device('cuda:0')
@@ -108,7 +82,7 @@ def test_multi_chunk_backward_matches_oracle_autograd(name):
     r.injected_noise = (u_c, u_f)
     d = make_decoder(dec, dev).requires_grad_(True)
     pg = planes.to(dev).requires_grad_(True)
-    got_out = r(pg, d, ro.to(dev), rd.to(dev), opts, **_flags(case))
+    got_out = r(pg, d, ro.to(dev), rd.to(dev), opts, **bwd_flags(case))
     for o, o_ref, key in zip(got_out, out, ('rgb', 'depth', 'wsum', 'xyz')):
         err = (o.detach().cpu() - o_ref.detach()).abs().max().item()
         assert err < TIGHT, f'{name}:{key} forward max abs err {err}'
@@ -128,11 +102,11 @@ def test_sharded_backward_sums_to_the_batch_backward():
     the rank-local bounds in the workspace while the forward clamps to the reduced ones; a ray's unclamped depth is a
     convex combination of its own interval midpoints, so it lies inside both and the gate agrees."""
     from panic3d_b200.training.volumetric_rendering.renderer import ImportanceRenderer
-    case = _case(67, 48, 48, N=3, cameras=[(0.0, -180.0, 1.0, 30.0), (0.0, 90.0, 1.0, 30.0), (60.0, -45.0, 1.2, 45.0)])
+    case = bwd_case(67, 48, 48, N=3, cameras=[(0.0, -180.0, 1.0, 30.0), (0.0, 90.0, 1.0, 30.0), (60.0, -45.0, 1.2, 45.0)])
     planes, dec, c2w, K, u_c, u_f, opts = build_case_inputs(case)
     ro, rd = case_rays(case, c2w, K)
     N, M = ro.shape[0], ro.shape[1]
-    gw = _incoming(case['seed'] + 5, N, M)
+    gw = bwd_incoming(case['seed'] + 5, N, M)
     dev = torch.device('cuda:0')
     r = ImportanceRenderer(use_triplane=True)
     d = make_decoder(dec, dev).requires_grad_(True)

@@ -33,8 +33,8 @@ with the batch's bounds afterwards).  test_gpu_fp64_oracle_equals_cpu_oracle pin
 config1 and mid_eval96 fixtures.
 
 Bars.  The kernel's error is bounded per sample and propagated to first order through the oracle:
-  * per sample: the decoder's sigma and colour bars (test_decode_tc_depth_gpu._three_pass_bars for mode 1,
-    _single_pass_bars for mode 2; test_three_pass_bars_hold_on_the_decode checks the first on p3d_decode_points at the
+  * per sample: the decoder's sigma and colour bars (tests/render_abi.py: three_pass_bars for mode 1,
+    single_pass_bars for mode 2; test_three_pass_bars_hold_on_the_decode checks the first on p3d_decode_points at the
     oracle's own sample positions), plus the point's fp32 rounding (ray_point, the grid transform: 4 v (|o| + |t d| + box)
     per coordinate, v = 2^-24) times the one-sided finite-difference slopes of sigma and colour;
   * per depth: coarse 16 v (|t| + |t0| + |t1|); fine 8 v (|t| + |t1 - t0|) for the lerp, and (2 S + 40) v on every cdf
@@ -76,15 +76,12 @@ import pytest
 import torch
 
 from oracle import renderer_oracle as orc
-from tests.helpers import profiled
-from tests.test_decode_tc_depth_gpu import U32, _decode_points, _single_pass_bars, _three_pass_bars
-from tests.test_render_backward_paths_gpu import _cull_sigma
-from tests.test_render_gpu import make_decoder
+from tests import render_abi as ra
+from tests.render_abi import (BW, DEV, OUTPUTS, U32, Worst, cull_sigma, dec64, decode_points, make_decoder, n_sm,
+                              single_pass_bars, three_pass_bars)
 
 pytestmark = pytest.mark.gpu
-DEV = 'cuda:0'
 PROF_FUSED = 5                    # profile slot of k_render_ws3 (csrc/p3d_common.cuh)
-BW = orc.DEFAULT_OPTS['box_warp']
 CHUNK = 1024                      # rays per oracle call
 BENCH_STRIDE = 16
 SIMT_BAR = 1e-4                   # the SIMT kernel against the oracle (tests/test_render_gpu.py)
@@ -95,8 +92,7 @@ EXCLUDE_SHARE_MASKS = {'eval_flags96': 0.95, 'binarize48': 0.35}
 PIN = 2e-6                        # fp64 device oracle vs the CPU fp32 one: the fp32 run's rounding (measured 7.6e-7)
 FREE_BYTES = 12 << 30             # the 512^2 cases: measured peak 8.1 GB (bench8), with margin
 MUFU = 2.0 ** -22
-OUT_NAMES = ['rgb'] * 32 + ['depth', 'wsum', 'xyz', 'xyz', 'xyz']
-OUTPUTS = ('rgb', 'depth', 'wsum', 'xyz')
+OUT_COLS = dict(rgb=slice(0, 32), depth=slice(32, 33), wsum=slice(33, 34), xyz=slice(34, 37))
 AUTO = dict(ray_start='auto', ray_end='auto')
 
 CASES = {
@@ -134,24 +130,14 @@ DESCENDING = ('all_miss48', 'all_miss96', 'all_miss_negpdf48', 'descending96')
 NEGATIVE_PDF = ('all_miss_negpdf48',)
 
 
-def n_sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def _per_cta(n_groups, sms):
     """render_fused_ws3.cu: grid = min(n_groups, n_sm), CTA b runs ceil((n_groups - b) / grid) groups."""
     grid = min(n_groups, sms)
     return [(n_groups - b + grid - 1) // grid for b in range(grid)]
 
 
-def _dec64(dec):
-    return {k: (v.to(DEV, torch.float64) if torch.is_tensor(v) else v) for k, v in dec.items()}
-
-
 # ------------------------------------------------------------------------------------------------- inputs
 def _rays(case, N, R):
-    from panic3d_b200 import cameras
-    from panic3d_b200.training.volumetric_rendering.ray_sampler import RaySampler
     kind = case.get('rays', 'spin')
     if kind == 'ortho':
         ro, rd = zip(*(orc.rays_ortho(20.0, -135.0 + 40 * n, 1.0, BW, R) for n in range(N)))
@@ -165,11 +151,7 @@ def _rays(case, N, R):
         ro = torch.stack([0.4 + 0.2 * a, 0.4 * b - 0.2, torch.full_like(a, 1.0)], -1)
         rd = torch.nn.functional.normalize(torch.stack([torch.zeros_like(a), 0.3 * (b - 0.5), torch.ones_like(a)], -1), dim=-1)
         return ro.to(DEV).contiguous(), rd.to(DEV).contiguous()
-    spin = cameras.cam60[cameras.camsubs['spin12']]
-    lab = torch.stack([cameras.camera_params_to_matrix(elev=float(spin[i][0]), azim=float(spin[i][1]), dist=case.get('dist', 1.0),
-                                                       fov=30.0)['camera_label'] for i in range(N)]).to(DEV)
-    ro, rd = RaySampler()(lab[:, :16].view(-1, 4, 4), lab[:, 16:25].view(-1, 3, 3), R)
-    return ro.float().contiguous(), rd.float().contiguous()
+    return ra.rays_at(ra.spin12(N), R, case.get('dist', 1.0))
 
 
 @functools.lru_cache(maxsize=None)
@@ -199,8 +181,8 @@ def _inputs(name):
     if case.get('centre_cull'):                     # median coarse sigma on the cull threshold
         d_c = orc.stratified_depths(u_c.to(DEV), opts['ray_start'], opts['ray_end'])
         xyz = (ro[:, :, None] + d_c * rd[:, :, None]).reshape(N, -1, 3)[:, ::7]
-        _, sig = orc.run_model(planes.to(DEV, torch.float64), _dec64(dec), xyz, opts, not case.get('eg3d'))
-        dec['b2'][0] += _cull_sigma(case['centre_cull']) - sig.quantile(case.get('quantile', 0.5)).item()
+        _, sig = orc.run_model(planes.to(DEV, torch.float64), dec64(dec), xyz, opts, not case.get('eg3d'))
+        dec['b2'][0] += cull_sigma(case['centre_cull']) - sig.quantile(case.get('quantile', 0.5)).item()
     return planes, dec, opts, ro, rd, u_c.to(DEV).contiguous(), u_f.to(DEV).contiguous()
 
 
@@ -208,7 +190,7 @@ def _inputs(name):
 def _kernel(name, mode=None, checks_later=False):
     """p3d_render_forward twice into NaN-filled outputs and workspace: one launch in slot 5 each, bit-identical, no NaN.
     Returns (rgb, depth, wsum, xyz), the workspace bounds words; with checks_later, the checks of the two runs are left to
-    the caller (_repeats), which makes them after comparing the values."""
+    the caller (ra.repeats), which makes them after comparing the values."""
     from panic3d_b200 import _lib
     from panic3d_b200.training.volumetric_rendering.renderer import ImportanceRenderer
     case = CASES[name]
@@ -232,30 +214,14 @@ def _kernel(name, mode=None, checks_later=False):
         assert p.mlp_mode == mode
         p.defer_depth_clamp = 0
         wt = [t.detach().float().contiguous() for t in wts]
-        L = _lib.lib()
-        nbytes = int(L.p3d_render_workspace_bytes(C.byref(p)))
-        runs = []
-        for _ in range(2):
-            ws = torch.full((nbytes,), 0xFF, dtype=torch.uint8, device=DEV)          # every float in it NaN
-            out = [torch.full(s, float('nan'), device=DEV) for s in ((N, M, 32), (N, M, 1), (N, M, 1), (N, M, 3))]
-            torch.cuda.synchronize()
-            _, prof = profiled(lambda: _lib.check(L.p3d_render_forward(
-                C.byref(p), cl.data_ptr(), *[t.data_ptr() for t in wt], ro.data_ptr(), rd.data_ptr(), u_c.data_ptr(),
-                u_f.data_ptr(), ws.data_ptr(), ws.numel(), *[o.data_ptr() for o in out], _lib.stream_ptr(DEV))))
-            torch.cuda.synchronize()
-            if mode != 0:
-                assert prof[PROF_FUSED] == 1, prof
-            runs.append((out, ws[:64].view(torch.int32).clone()))
+        ws = torch.empty(int(_lib.lib().p3d_render_workspace_bytes(C.byref(p))), dtype=torch.uint8, device=DEV)
+        out = [torch.empty(s, device=DEV) for s in ((N, M, 32), (N, M, 1), (N, M, 1), (N, M, 3))]
+        first, second = ra.twice(lambda: ra.render_forward(p, cl, wt, ro, rd, u_c, u_f, ws, out),
+                                 out + [ws[:64].view(torch.int32)], PROF_FUSED if mode != 0 else None, [ws], checks_later=True)
         if checks_later:
-            return runs[0][0], runs[0][1], runs[1][0]
-        _repeats(name, runs[0][0], runs[1][0])
-        return runs[0]
-
-
-def _repeats(name, first, second):
-    for key, a, b in zip(OUTPUTS, first, second):
-        assert not torch.isnan(a).any(), f'{name}: {key} has NaN (an element never written, or read before it landed)'
-        assert torch.equal(a, b), f'{name}: two runs differ in {key}'
+            return first[:4], first[4], second[:4]
+        ra.repeats(first[:4], second[:4], OUTPUTS, nan=True)
+        return first[:4], first[4]
 
 
 # ------------------------------------------------------------------------------------------------- oracle and bars
@@ -280,14 +246,14 @@ def _decoded(name, v, xyz, rd_s, mode):
     case = CASES[name]
     planes, dec, opts, *_ = _inputs(name)
     tri = not case.get('eg3d')
-    p64, d64 = planes[v:v + 1].to(DEV, torch.float64), _dec64(dec)
+    p64, d64 = planes[v:v + 1].to(DEV, torch.float64), dec64(dec)
     run = lambda x: orc.run_model(p64, d64, x, opts, tri)
     rgb, sig = run(xyz)
     if mode == 1:
-        b_rgb, b_sig = _three_pass_bars(p64, d64, xyz, force_sigmoid=dec['force_sigmoid'], use_triplane=tri)
+        b_rgb, b_sig = three_pass_bars(p64, d64, xyz, force_sigmoid=dec['force_sigmoid'], use_triplane=tri)
     else:
         assert tri and not dec['force_sigmoid']
-        b_rgb, b_sig = _single_pass_bars(p64, d64, xyz)
+        b_rgb, b_sig = single_pass_bars(p64, d64, xyz)
     h = 1e-7
     beta_x = 4 * U32 * (xyz.abs() + BW)
     g_sig, g_rgb = torch.zeros_like(sig), torch.zeros_like(rgb)
@@ -396,7 +362,7 @@ def _chunk(name, v, sl, mode, with_bars=True, controls=False):
     res = dict(o=o, t_max=mid['t_all'].max(), t_min=mid['t_all'].min(), illdef=illdef)
     if controls:
         # the colour map without its gain: s - 0.001 instead of 1.002 s - 0.001
-        dec_s = _dec64(dict(dec, force_sigmoid=True))
+        dec_s = dec64(dict(dec, force_sigmoid=True))
         p64 = planes[v:v + 1].to(DEV, torch.float64)
         rgb_s = lambda smp: orc.run_model(p64, dec_s, smp['xyz'].reshape(1, -1, 3), opts, not case.get('eg3d'))[0].reshape(m, -1, 32) - 0.001
         c0s, f0s = dict(c0, rgb=rgb_s(c0)), dict(f0, rgb=rgb_s(f0))
@@ -454,7 +420,7 @@ def _chunk(name, v, sl, mode, with_bars=True, controls=False):
     # rays with a sample within its bar of a jump
     near = torch.zeros(m, dtype=torch.bool, device=DEV)
     if fl.get('cull_clouds') or fl.get('binarize_clouds'):
-        thr = _cull_sigma(fl.get('cull_clouds') or fl.get('binarize_clouds'))
+        thr = cull_sigma(fl.get('cull_clouds') or fl.get('binarize_clouds'))
         for smp, move in ((c0, beta['t_c'][..., 0]), (f0, fine_move)):
             cropped = orc.crop_mask(smp['xyz'].reshape(1, -1, 3), fl['triplane_crop'], BW).reshape(m, -1) if fl.get('triplane_crop') \
                 else torch.zeros(m, S, dtype=torch.bool, device=DEV)
@@ -483,21 +449,6 @@ def _rays_of(name):
     return [(v, idx[i:i + CHUNK]) for v in range(case['N']) for i in range(0, idx.numel(), CHUNK)]
 
 
-class Worst:
-    def __init__(self):
-        self.err = {k: 0.0 for k in OUTPUTS}
-        self.ratio = {k: 0.0 for k in OUTPUTS}
-
-    def add(self, got, want, bar, keep):
-        err = (got.double() - want).abs().nan_to_num(nan=float('inf'))[keep]
-        r = (err / bar[keep])
-        for j, key in enumerate(OUTPUTS):
-            cols = [i for i, n in enumerate(OUT_NAMES) if n == key]
-            if err.shape[0]:
-                self.err[key] = max(self.err[key], err[:, cols].max().item())
-                self.ratio[key] = max(self.ratio[key], r[:, cols].max().item())
-
-
 def _flat(out, v, sl):
     rgb, depth, wsum, xyz = out
     return torch.cat([rgb[v, sl], depth[v, sl], wsum[v, sl], xyz[v, sl]], -1)
@@ -507,7 +458,7 @@ def _compare(name, out, mode, controls=()):
     """The kernel's outputs against the oracle's, ray by ray.  Returns the worst abs errors, ratios and control ratios."""
     res_all = [(v, sl, _chunk(name, v, sl, mode, controls=bool(controls))) for v, sl in _rays_of(name)]
     t_hi = max(r['t_max'].item() for *_, r in res_all)
-    worst = Worst()
+    worst = {key: Worst() for key in OUTPUTS}
     n_near = n_total = n_ill = 0
     ctl = {c: 0.0 for c in controls}
     cull = [0, 0]
@@ -519,7 +470,9 @@ def _compare(name, out, mode, controls=()):
         bar[dead, 32] = 64 * U32 * abs(t_hi)
         keep = ~r['near'] & ~r['illdef']
         n_ill += r['illdef'].sum().item()
-        worst.add(got, want, bar, keep)
+        if keep.any():
+            for key, cols in OUT_COLS.items():
+                worst[key].add(got[keep][:, cols], want[keep][:, cols], bar[keep][:, cols])
         n_near += r['near'].sum().item()
         n_total += r['near'].numel()
         for c in controls:
@@ -531,7 +484,7 @@ def _compare(name, out, mode, controls=()):
             cull[0] += r['cull_share'][0]
             cull[1] += r['cull_share'][1]
     for key in OUTPUTS:
-        print(f'{name} mode {mode} {key}: max abs err {worst.err[key]:.3e}, worst err / bar {worst.ratio[key]:.4f}')
+        print(f'{name} mode {mode} {key}: max abs err {worst[key].err:.3e}, worst err / bar {worst[key].ratio:.4f}')
     print(f'{name}: {n_near} of {n_total} rays excluded (a sample within its bar of a mask threshold), {n_ill} with a '
           f'non-positive importance pdf')
     if name in NEGATIVE_PDF:
@@ -556,7 +509,7 @@ def test_gpu_fp64_oracle_equals_cpu_oracle():
         fl = {k: case[k] for k in ('triplane_crop', 'cull_clouds', 'binarize_clouds') if case.get(k)}
         cpu, smp = orc.render(planes, dec, ro, rd, opts, u_c, u_f, return_samples=True, **fl)
         to = lambda t: None if t is None else t.to(DEV)
-        gpu = orc.render(planes.to(DEV, torch.float64), _dec64(dec), ro.to(DEV), rd.to(DEV), opts, None, None,
+        gpu = orc.render(planes.to(DEV, torch.float64), dec64(dec), ro.to(DEV), rd.to(DEV), opts, None, None,
                          depths=tuple(to(t) for t in smp['depths']), masks=tuple(to(t) for t in smp['masks']), **fl)
         for key, a, b in zip(OUTPUTS, gpu, cpu):
             assert a.dtype == torch.float64
@@ -577,7 +530,7 @@ def test_render_graph_is_the_oracle(name):
     n = M if opts['ray_start'] == 'auto' else min(256, M)
     views = range(N) if opts['ray_start'] == 'auto' else range(1)
     fl = case.get('flags', {})
-    want = orc.render(planes[:len(views)].to(DEV, torch.float64), _dec64(dec), ro[:len(views), :n].double(), rd[:len(views), :n].double(),
+    want = orc.render(planes[:len(views)].to(DEV, torch.float64), dec64(dec), ro[:len(views), :n].double(), rd[:len(views), :n].double(),
                       opts, u_c[:len(views), :n].double(), u_f.view(N, M, -1)[:len(views), :n].reshape(len(views) * n, -1).double(),
                       use_triplane=not case.get('eg3d'), **fl)
     worst = dict.fromkeys(OUTPUTS, 0.0)
@@ -596,20 +549,20 @@ def test_render_graph_is_the_oracle(name):
 
 
 def test_three_pass_bars_hold_on_the_decode():
-    """The per-sample mode 1 bar (_three_pass_bars) holds on p3d_decode_points (the same decoder code, fused_common.cuh) at
+    """The per-sample mode 1 bar (three_pass_bars) holds on p3d_decode_points (the same decoder code, fused_common.cuh) at
     the oracle's own coarse and fine sample positions of train48's first view."""
     name = 'train48'
     planes, dec, opts, ro, rd, u_c, u_f = _inputs(name)
     n = 1024
-    p64, d64 = planes[:1].to(DEV, torch.float64), _dec64(dec)
+    p64, d64 = planes[:1].to(DEV, torch.float64), dec64(dec)
     _, smp = orc.render(p64, d64, ro[:1, :n].double(), rd[:1, :n].double(), opts, u_c[:1, :n].double(), u_f[:n].double(),
                         return_samples=True)
     pts = [(ro[:1, :n, None].double() + d * rd[:1, :n, None].double()).reshape(1, -1, 3) for d in smp['depths']]
     xyz = torch.cat(pts, 1).float()
     x64 = xyz.double()
     rgb, sig = orc.run_model(p64, d64, x64, opts, True)
-    b_rgb, b_sig = _three_pass_bars(p64, d64, x64)
-    k_rgb, k_sig = _decode_points(planes[:1].to(DEV), dec, xyz, 1)
+    b_rgb, b_sig = three_pass_bars(p64, d64, x64)
+    k_rgb, k_sig = decode_points(planes[:1].to(DEV), dec, xyz, 1)
     for key, k, w, b in (('rgb', k_rgb, rgb, b_rgb), ('sigma', k_sig, sig, b_sig)):
         err = (k.double() - w).abs().nan_to_num(nan=float('inf'))
         print(f'decode at the render samples {key}: max abs err {err.max().item():.3e}, worst err / bar {(err / b).max().item():.4f}, '
@@ -677,8 +630,8 @@ def test_fused_matches_fp64_oracle(name):
         print(f'negative control "{CONTROLS[c]}" on {name}: worst err / bar {r:.1f}')
     print(f'{name}: {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GB')
     assert share <= EXCLUDE_SHARE_MASKS.get(name, EXCLUDE_SHARE[1]), share
-    assert max(worst.ratio.values()) <= 1.0, (name, worst.ratio)
-    _repeats(name, out, again)
+    assert max(w.ratio for w in worst.values()) <= 1.0, (name, {k: w.ratio for k, w in worst.items()})
+    ra.repeats(out, again, OUTPUTS, nan=True)
     for c, r in ctl.items():
         if CONTROL_CASES[c] == name:
             assert r >= CONTROL_MIN, (CONTROLS[c], r)
@@ -703,6 +656,6 @@ def test_single_pass_matches_fp64_oracle():
     w2, share2, *_ = _compare(name, two, 2)
     w1, share1, *_ = _compare(name, one, 1)
     assert share2 <= EXCLUDE_SHARE[2] and share1 <= EXCLUDE_SHARE[1]
-    assert max(w2.ratio.values()) <= 1.0 and max(w1.ratio.values()) <= 1.0
+    assert max(w.ratio for w in w2.values()) <= 1.0 and max(w.ratio for w in w1.values()) <= 1.0
     for key in ('rgb', 'wsum'):
-        assert w2.err[key] >= 10 * w1.err[key], ('single pass is not reaching the kernel', key, w2.err[key], w1.err[key])
+        assert w2[key].err >= 10 * w1[key].err, ('single pass is not reaching the kernel', key, w2[key].err, w1[key].err)

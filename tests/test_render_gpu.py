@@ -10,6 +10,7 @@ import torch
 from oracle import renderer_oracle as orc
 from tests.golden.cases import RENDER_CASES, POINT_CASES, build_case_inputs
 from tests.helpers import load_golden, oracle_render
+from tests.render_abi import make_decoder
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3          # the bar
@@ -18,16 +19,6 @@ TIGHT = 1e-4        # what the fp32 path should really reach (no cull discontinu
 
 def _dev():
     return torch.device('cuda:0')
-
-
-def make_decoder(dec, dev):
-    from panic3d_b200.training.triplane import OSGDecoder
-    d = OSGDecoder(dec['w1'].shape[1], {'decoder_lr_mul': dec['lr_mul'], 'decoder_output_dim': dec['w2'].shape[0] - 1})
-    with torch.no_grad():
-        d.net[0].weight.copy_(dec['w1']); d.net[0].bias.copy_(dec['b1'])
-        d.net[2].weight.copy_(dec['w2']); d.net[2].bias.copy_(dec['b2'])
-    d.set_force_sigmoid(bool(dec['force_sigmoid']))
-    return d.to(dev).requires_grad_(False)
 
 
 def gpu_rays(case, c2w, K, dev):

@@ -22,7 +22,7 @@ import torch
 from oracle import philox as ph, renderer_oracle as orc
 from tests.golden.cases import RENDER_CASES, build_case_inputs
 from tests.helpers import case_rays, profiled
-from tests.test_render_gpu import make_decoder
+from tests.render_abi import make_decoder
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0')
@@ -201,15 +201,15 @@ def test_fused_headline_config_draws_the_restated_uniforms():
 def test_fused_late_laps_draw_their_own_rays():
     """n_groups = 4 * n_sm + r at 48+48: every CTA runs 4 or 5 ray groups of its persistent loop, and a group of a late
     lap (grp = blockIdx.x + n * gridDim.x) must draw the uniforms of its own global rays."""
-    from tests.test_plane_variants_gpu import _planes_and_decoder, _rays
+    from tests.render_abi import box_rays, planes_and_decoder
     n_sm = torch.cuda.get_device_properties(0).multi_processor_count
     S, k, N = 48, 4, 2
     GR = 384 // S
     groups = k * n_sm + 18
     M = groups * GR // N
     assert groups % N == 0 and 18 < n_sm and (groups + n_sm - 1) // n_sm == k + 1
-    planes, dec = _planes_and_decoder(460, n=N, h=64, w=64)
-    ro, rd = _rays(460, N, M)
+    planes, dec = planes_and_decoder(460, N, 64, 64)
+    ro, rd = box_rays(460, N, M)
     opts = dict(orc.DEFAULT_OPTS, depth_resolution=S, depth_resolution_importance=S)
     got = _fused(planes, dec, ro, rd, opts, 461)
     want = _oracle(planes, dec, ro, rd, opts, {}, ph.render_uniforms(ph.drawn_seed(461), N, M, S, S))

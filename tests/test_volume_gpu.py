@@ -6,7 +6,7 @@ import torch
 from oracle import volume_oracle as vo
 from tests.golden.cases import VOLUME_CASES, build_case_inputs
 from tests.helpers import load_golden
-from tests.test_render_gpu import make_decoder
+from tests.render_abi import make_decoder
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
