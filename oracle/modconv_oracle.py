@@ -108,6 +108,31 @@ def transposed_prefilter(x, w):
     return y.reshape(n, o, *y.shape[2:])
 
 
+def oracle_conv(x, w, up, k, chunk=4096):
+    """The tensor p3d_modconv_forward computes before its epilogue, for per-sample weights w (N, O, I, k, k): the grouped
+    conv (up 1, padding k // 2) or transposed_prefilter (up 2).  Runs `chunk` samples per grouped call."""
+    if x.shape[0] > chunk:
+        return torch.cat([oracle_conv(x[i:i + chunk], w[i:i + chunk], up, k) for i in range(0, x.shape[0], chunk)])
+    n = x.shape[0]
+    if up == 2:
+        return transposed_prefilter(x, w)
+    y = F.conv2d(x.reshape(1, -1, *x.shape[2:]), w.reshape(-1, *w.shape[2:]), padding=k // 2, groups=n)
+    return y.reshape(n, -1, *y.shape[2:])
+
+
+def epilogue64(acc, bias=None, noise=None, act='linear', gain=1.0, clamp=None):
+    """The epilogue of p3d_modconv_forward on the accumulator `acc` (N, O, H, W): clamp(act(acc + noise + bias) * gain),
+    act lrelu (slope 0.2) or linear, clamp None for none.  `noise` broadcasts against acc ([N, 1, H, W] or [H, W]); `bias`
+    is given in the values the kernel reads (the layer dtype)."""
+    v = acc if noise is None else acc + noise.double()
+    if bias is not None:
+        v = v + bias.double().reshape(1, -1, 1, 1)
+    if act == 'lrelu':
+        v = torch.where(v > 0, v, v * 0.2)
+    v = v * gain
+    return v if clamp is None else v.clamp(-clamp, clamp)
+
+
 # ------------------------------------------------------------------------------------------ modulated_conv2d (fused branch)
 def modulated_conv2d(x, weight, styles, noise=None, up=1, down=1, padding=0, resample_filter=None, demodulate=True,
                      flip_weight=True, fused_modconv=True):

@@ -114,20 +114,26 @@ def conv(p, x, ws, bias=None, noise=None, act='linear', gain=1.0, clamp=None):
     return y
 
 
-def unpack_workspace(p, ws):
-    """The prepared operand as (N, Cout, Cin, k, k) fp32 (fp16 values widened): the weights the conv kernel multiplies."""
+def workspace_rows(p, ws):
+    """The whole workspace as (N, Cout padded to the N tile, slot, Cin padded to the K chunk), in the compute type (fp16
+    or tf32 as fp32): a view of its bytes, padding included."""
     f16 = p.dtype == P3D_F16
     es = 2 if f16 else 4
     kce = KB // es
     nchunks = -(-p.in_channels // kce)
     bn = 8 if p.out_channels <= 8 else 128
     nnb = -(-p.out_channels // bn)
-    slots = tap_slots(p)
-    vals = ws.view(torch.float16 if f16 else torch.float32).to(torch.float32)
+    nslots = len(tap_slots(p))
+    vals = ws.view(torch.float16 if f16 else torch.float32)
     # tile_byte(r, b) = (b >> 4) * (bn * 16) + (r >> 3) * 128 + (r & 7) * 16 + (b & 15): dims (kc, rg, r8, e) of one tile
-    vals = vals.view(p.batch, nnb, len(slots), nchunks, kce * es // 16, bn // 8, 8, 16 // es)
-    vals = vals.permute(0, 1, 5, 6, 2, 3, 4, 7).reshape(p.batch, nnb * bn, len(slots), nchunks * kce)
-    vals = vals[:, :p.out_channels, :, :p.in_channels]
+    vals = vals.view(p.batch, nnb, nslots, nchunks, kce * es // 16, bn // 8, 8, 16 // es)
+    return vals.permute(0, 1, 5, 6, 2, 3, 4, 7).reshape(p.batch, nnb * bn, nslots, nchunks * kce)
+
+
+def unpack_workspace(p, ws):
+    """The prepared operand as (N, Cout, Cin, k, k) fp32 (fp16 values widened): the weights the conv kernel multiplies."""
+    slots = tap_slots(p)
+    vals = workspace_rows(p, ws)[:, :p.out_channels, :, :p.in_channels].to(torch.float32)
     k = p.kernel_size
     out = torch.zeros(p.batch, p.out_channels, p.in_channels, k * k, dtype=torch.float32, device=ws.device)
     for s, t in enumerate(slots):

@@ -5,8 +5,8 @@ fails it, as it must.  The tree is not modified.
     python tests/run_mutations.py TARGET [TARGET ...] [--files F ...] [--json out.json] [--build-only]
 
 TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane (the TRI lines of
-render_backward.cu), modconv, render_fused and multiplane (the multiplane section of the header render_device.cuh).  Each
-mutant recompiles every translation unit that includes its source, directly or through other headers.  --files runs other
+render_backward.cu), modconv, modconv_paths (more modconv.cu mutations, against tests/test_modconv_paths_gpu.py),
+render_fused and multiplane (the multiplane section of the header render_device.cuh).  Each mutant recompiles every translation unit that includes its source, directly or through other headers.  --files runs other
 GPU files against the same mutants instead (to see which of them the rest of the suite catches); the exit code then only
 reports that the run completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
 --json writes {target: {mutation: result}}.
@@ -101,6 +101,30 @@ MODCONV = {
     'noise indexed per channel': ('(long long)oy * a.snh', '(long long)(co % a.H) * a.snh'),
 }
 
+# modconv.cu against tests/test_modconv_paths_gpu.py: every mutation keeps all memory accesses in bounds at every shape that
+# file runs (the reason is next to each entry).
+MODCONV_PATHS = {
+    # the epilogue writes phase (py, 0) on a grid of in_h + 1 columns: in bounds because every up-2 shape of the file has
+    # in_h <= in_w (its tall shapes run up 1 or kernel 1), so oy and ox stay inside the (2H+1) x (2W+1) output and the
+    # loads stay bounds-checked; columns it no longer reaches stay NaN.  Equal to the kernel on square shapes
+    'up-2 phase width from in_h': ('(px == 0 ? p->in_w + 1 : p->in_w)', '(px == 0 ? p->in_h + 1 : p->in_h)'),
+    # the prep writes kernel row 2 - 2j where row 2j belongs (and columns likewise); prep only: the conv reads the tap
+    # offsets, not the kernel taps, so an oracle on the weights read back through the same slots agrees with it
+    'up-2 prep kernel rows reversed': ('k = ph == 0 ? 2 * j : 1;', 'k = ph == 0 ? 2 - 2 * j : 1;'),
+    # an odd number of K-steps in a chunk (fp16 Cin % 64 = 16 or 48) drops its last step; fewer wgmmas on the same tiles
+    'K-steps of a chunk rounded down to even': ('const int ksteps = min(KCE, a.Cin - q * KCE) * ES / 32;',
+                                                'const int ksteps = min(KCE, a.Cin - q * KCE) * ES / 64 * 2;'),
+    # the im2col row of output pixel pix taken from the phase height: the gathered input pixel is still checked against
+    # H and W before it is read.  Equal to the kernel when the phase grid is square
+    'im2col pixel from the phase height': ('const int pa = prow ? pix / owp : 0, pb = prow ? pix % owp : 0;',
+                                           'const int pa = prow ? pix / tt.oh[ph] : 0, pb = prow ? pix % tt.oh[ph] : 0;'),
+    # every sample reads sample 0's noise: a smaller offset into the same tensor
+    'noise of sample 0 for every sample': ('(long long)n * a.snn + ', ''),
+    # the N tile's padding rows get row 0's weights (wrow already points at row 0 for them); the conv never stores those
+    # columns, so only the workspace check sees it
+    'N-tile padding rows not zeroed': ('(live && ci < a.Cin) ?', '(ci < a.Cin) ?'),
+}
+
 # render_fused_ws3.cu: value mutations only - no stage index, parity, arrival count or transaction size changes, and every
 # access stays in bounds (trow ^ 1 stays inside the 128-row tile), so none can hang.
 RENDER_FUSED = {
@@ -144,6 +168,7 @@ TARGETS = {
     'render_backward': ('render_backward.cu', 'tests/test_render_backward_paths_gpu.py', RENDER_BACKWARD),
     'render_backward_multiplane': ('render_backward.cu', 'tests/test_multiplane_paths_gpu.py', RENDER_BACKWARD_MULTIPLANE),
     'modconv': ('modconv.cu', 'tests/test_modconv_gpu.py', MODCONV),
+    'modconv_paths': ('modconv.cu', 'tests/test_modconv_paths_gpu.py', MODCONV_PATHS),
     'render_fused': ('render_fused_ws3.cu', 'tests/test_render_fused_paths_gpu.py', RENDER_FUSED),
     'multiplane': ('render_device.cuh', 'tests/test_multiplane_paths_gpu.py', MULTIPLANE),
 }

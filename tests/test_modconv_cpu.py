@@ -128,3 +128,57 @@ def test_modconv_symbols_are_declared_and_bound():
     oh, ow = C.c_int32(), C.c_int32()
     up2 = mc.make_params(x, torch.empty(64, 32, 3, 3), True, up=2)
     assert L.p3d_modconv_out_size(C.byref(up2), C.byref(oh), C.byref(ow)) == 0 and (oh.value, ow.value) == (17, 17)
+
+
+# ------------------------------------------------------------------------------------------ the supported envelope
+F32, F16 = 0, 1                 # P3D_F32 / P3D_F16 (include/p3d_ops.h)
+
+
+def _envelope(p):
+    """include/p3d_modconv.h restated: (supported, (out_h, out_w) or None, workspace bytes).  The workspace holds, per
+    sample and N tile (8 rows when Cout <= 8, else 128), one 128-byte-per-row B tile per tap slot and K chunk (64 fp16 /
+    32 fp32 channels); up 2 has 4 + 2 + 2 + 1 = 9 slots, like kernel 3."""
+    nph = 4 if p.up == 2 else 1
+    ok = ((p.kernel_size == 3 or (p.kernel_size == 1 and p.up == 1)) and p.up in (1, 2) and p.down == 1 and
+          (p.dtype == F16 or (p.dtype == F32 and p.allow_tf32)) and p.demodulate in (0, 1) and
+          0 < p.in_channels <= 65536 and p.in_channels % 16 == 0 and 1 <= p.out_channels <= 4096 and
+          1 <= p.batch and p.batch * nph <= 65535 and 1 <= p.in_h <= 4096 and 1 <= p.in_w <= 4096)
+    if not ok:
+        return False, None, 0
+    es = 2 if p.dtype == F16 else 4
+    bn = 8 if p.out_channels <= 8 else 128
+    nchunks = -(-p.in_channels * es // 128)
+    ntaps = 1 if p.kernel_size == 1 else 9
+    size = (2 * p.in_h + 1, 2 * p.in_w + 1) if p.up == 2 else (p.in_h, p.in_w)
+    return True, size, p.batch * -(-p.out_channels // bn) * ntaps * nchunks * bn * 128
+
+
+_BASE = dict(batch=2, in_channels=32, out_channels=64, in_h=8, in_w=8, kernel_size=3, up=1, down=1, dtype=F16,
+             demodulate=1, allow_tf32=1)
+# each boundary at, one below and one above; every row also runs in fp32, kernel 1 and up 2 (where those are supported)
+_EDGES = [('in_channels', v) for v in (0, 15, 16, 17, 31, 32, 48, 65520, 65535, 65536, 65537, 65552)] + \
+         [('out_channels', v) for v in (0, 1, 2, 7, 8, 9, 127, 128, 129, 4095, 4096, 4097)] + \
+         [('in_h', v) for v in (0, 1, 2, 4095, 4096, 4097)] + [('in_w', v) for v in (0, 1, 2, 4095, 4096, 4097)] + \
+         [('batch', v) for v in (0, 1, 16383, 16384, 65534, 65535, 65536)] + \
+         [('demodulate', v) for v in (-1, 0, 1, 2)] + [('down', v) for v in (0, 2)] + [('kernel_size', v) for v in (0, 2, 5)] + \
+         [('up', v) for v in (0, 3)] + [('dtype', v) for v in (2, 3, -1)] + [('allow_tf32', 0)]
+
+
+@pytest.mark.parametrize('field,value', _EDGES, ids=[f'{f}={v}' for f, v in _EDGES])
+def test_supported_out_size_and_workspace_at_each_boundary(field, value):
+    """p3d_modconv_supported / _out_size / _workspace_bytes against the restatement at every boundary of the envelope, +-1,
+    with a non-square input (in_h != in_w) so that a swapped out_size shows."""
+    import __graft_entry__ as g
+    g.build()
+    import panic3d_b200.modconv as mc
+    from panic3d_b200 import _lib
+    L = _lib.lib()
+    for variant in (dict(), dict(dtype=F32), dict(kernel_size=1, demodulate=0), dict(up=2),
+                    dict(in_h=5, in_w=37), dict(in_h=37, in_w=5, up=2), dict(dtype=F32, allow_tf32=0)):
+        p = mc.ModconvParams(**{**_BASE, **variant, field: value})
+        ok, size, nbytes = _envelope(p)
+        assert bool(L.p3d_modconv_supported(C.byref(p))) == ok, (variant, field, value)
+        assert int(L.p3d_modconv_workspace_bytes(C.byref(p))) == nbytes, (variant, field, value)
+        oh, ow = C.c_int32(-1), C.c_int32(-1)
+        rc = L.p3d_modconv_out_size(C.byref(p), C.byref(oh), C.byref(ow))
+        assert (rc == 0) == ok and (not ok or (oh.value, ow.value) == size), (variant, field, value, oh.value, ow.value)

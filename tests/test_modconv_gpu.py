@@ -17,7 +17,7 @@ import math
 import pytest
 import torch
 
-from oracle.modconv_oracle import EVAL_SHAPES
+from oracle.modconv_oracle import EVAL_SHAPES, epilogue64, oracle_conv
 
 pytestmark = pytest.mark.gpu
 
@@ -70,31 +70,6 @@ class _Slot7:
         self.count = int(cnt[7])
 
 
-def _epilogue64(acc, layer, noise, kind, gain, dtype):
-    if kind == 'torgb':
-        v = acc + layer.bias.to(dtype).double().reshape(1, -1, 1, 1)
-        return v.clamp(-layer.conv_clamp, layer.conv_clamp) if layer.conv_clamp is not None else v
-    if noise is not None:
-        v = acc + noise.double()
-    else:
-        v = acc
-    v = v + layer.bias.to(dtype).double().reshape(1, -1, 1, 1)
-    v = torch.where(v > 0, v, v * 0.2) * (layer.act_gain * gain)
-    if layer.conv_clamp is not None:
-        c = layer.conv_clamp * gain
-        v = v.clamp(-c, c)
-    return v
-
-
-def _oracle_conv(mo, x64, w64, up, k):
-    """fp64 grouped conv of per-sample weights w64 (N, O, I, k, k): the kernel's tensor before its epilogue."""
-    n = x64.shape[0]
-    if up == 2:
-        return mo.transposed_prefilter(x64, w64)
-    y = torch.nn.functional.conv2d(x64.reshape(1, -1, *x64.shape[2:]), w64.reshape(-1, *w64.shape[2:]), padding=k // 2, groups=n)
-    return y.reshape(n, -1, *y.shape[2:])
-
-
 def _check_layer(env, shape, n, channels_last, noise_mode='none', gain=1.0):
     mc, lib, mo = env
     name, cin, cout, res, up, kind, dtype, clamp = shape
@@ -118,9 +93,16 @@ def _check_layer(env, shape, n, channels_last, noise_mode='none', gain=1.0):
             g_eff = 1.0
         wk = mc.unpack_workspace(p, ws).double()
         x64 = mo.round_operand(x, dtype)
-        acc = _oracle_conv(mo, x64, wk, up, layer.weight.shape[-1])
-        s_abs = _oracle_conv(mo, x64.abs(), wk.abs(), up, layer.weight.shape[-1])
-        ref = acc if (kind == 'layer' and up == 2) else _epilogue64(acc, layer, noise, kind, gain, dtype)
+        acc = oracle_conv(x64, wk, up, layer.weight.shape[-1])
+        s_abs = oracle_conv(x64.abs(), wk.abs(), up, layer.weight.shape[-1])
+        bias = layer.bias.to(dtype)
+        if kind == 'torgb':
+            ref = epilogue64(acc, bias, clamp=layer.conv_clamp)
+        elif up == 1:
+            ref = epilogue64(acc, bias, noise, 'lrelu', layer.act_gain * gain,
+                             None if layer.conv_clamp is None else layer.conv_clamp * gain)
+        else:
+            ref = acc
         K = wk.shape[2] * wk.shape[3] * wk.shape[4]
         bar = abs(g_eff) * K * U32 * s_abs + (U16 if dtype == torch.float16 else U32) * ref.abs() + 2.0 ** -24
         err = (y.double() - ref).abs()
@@ -155,8 +137,8 @@ def test_gpu_oracle_equals_cpu_oracle(env):
     x = torch.randn(2, 32, 6, 6, dtype=torch.float64)
     w = torch.randn(2, 24, 32, 3, 3, dtype=torch.float64)
     for up in (1, 2):
-        a = _oracle_conv(mo, x, w, up, 3)
-        b = _oracle_conv(mo, x.cuda(), w.cuda(), up, 3).cpu()
+        a = oracle_conv(x, w, up, 3)
+        b = oracle_conv(x.cuda(), w.cuda(), up, 3).cpu()
         assert float((a - b).abs().max()) <= 1e-12 * float(a.abs().max())
 
 
@@ -192,7 +174,7 @@ def test_fp16_layers_stay_within_two_ulps_of_the_reference_order(env):
             # the fp64 reference-order value, to size the accumulation slack of the two routes
             p = mc.make_params(x, layer.weight, True)
             wk = mc.unpack_workspace(p, mc.prep(p, layer.weight, layer.affine(w))).double()
-            s_abs = _oracle_conv(mo, x.double().abs(), wk.abs(), 1, 3) * layer.act_gain
+            s_abs = oracle_conv(x.double().abs(), wk.abs(), 1, 3) * layer.act_gain
         K = wk[0, 0].numel()
         bar = 2 * U16 * ref.double().abs() + 2 * K * U32 * s_abs + 2.0 ** -24
         frac = float(((got.double() - ref.double()).abs() / bar).max())
@@ -213,7 +195,7 @@ def test_noise_draws_like_the_original_method(env, noise_mode):
         ref = mo.SynthesisLayer.forward(layer, x, w, noise_mode=noise_mode)
         p = mc.make_params(x, layer.weight, True)
         wk = mc.unpack_workspace(p, mc.prep(p, layer.weight, layer.affine(w))).double()
-        s_abs = _oracle_conv(mo, x.double().abs(), wk.abs(), 1, 3) * layer.act_gain
+        s_abs = oracle_conv(x.double().abs(), wk.abs(), 1, 3) * layer.act_gain
     err = (got.double() - ref.double()).abs()
     assert float((err / (s_abs * 2.0 ** -9 + 1e-5)).max()) <= 1.0          # TF32 on both routes
 
