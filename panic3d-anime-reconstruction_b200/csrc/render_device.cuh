@@ -31,12 +31,18 @@ __device__ __forceinline__ float coarse_depth(const Geom& g, int s, float u, flo
 // coarse_depth with the ray's 'auto' limits: a ray that misses the box takes the smallest and largest valid start of the
 // whole batch (bounds[2..3], when bounds[4] says there is one).  renderer.py:165-170.  A dead row (live == false) reads
 // no limits.
+// Deviation from the reference: a NaN limit (k_ray_limits: an axis-parallel ray starting on a box face) in a batch where no
+// ray hits the box takes the miss limits (-1, -2).  The reference renders NaN depths there; NaN depths would break the
+// rank merge (merge_by_rank's comparisons are all false), leaving merged slots whose colour row index is never written.
 __device__ __forceinline__ float coarse_sample_depth(const Geom& g, int s, float u, long long ray, bool live, const float* ray_t0,
                                                      const float* ray_t1, const unsigned int* bounds) {
     float t0 = 0.f, t1 = 0.f;
     if (g.ray_mode == P3D_RAYS_AUTOBOX && live) {
         t0 = ray_t0[ray]; t1 = ray_t1[ray];
-        if (!(t1 > t0) && bounds[4]) { t0 = ordered_to_float(bounds[2]); t1 = ordered_to_float(bounds[3]); }
+        if (!(t1 > t0)) {
+            if (bounds[4]) { t0 = ordered_to_float(bounds[2]); t1 = ordered_to_float(bounds[3]); }
+            else if (isnan(t0) || isnan(t1)) { t0 = -1.f; t1 = -2.f; }
+        }
     }
     return coarse_depth(g, s, u, t0, t1);
 }

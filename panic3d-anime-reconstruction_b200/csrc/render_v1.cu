@@ -180,7 +180,13 @@ __global__ void __launch_bounds__(kTile) k_sample_decode(const SampleArgs a) {
 
 // -------------------------------------------------------------------------------------------
 // k_ray_limits: math_utils.get_ray_limits_box (:46-98) + validity reduction (renderer.py:165-170)
+// An axis-parallel ray (a direction component of +-0, inv = +-inf) whose origin lies exactly on that axis's box face gets
+// 0 * inf = NaN there.  torch.max / torch.min propagate it, so the reference returns a NaN limit, fails t1 > t0 and
+// renders the ray with the batch's fallback limits; max_nan / min_nan keep that NaN where fmaxf / fminf would drop it.
 // -------------------------------------------------------------------------------------------
+__device__ __forceinline__ float max_nan(float a, float b) { return (isnan(a) || isnan(b)) ? __int_as_float(0x7fffffff) : fmaxf(a, b); }
+__device__ __forceinline__ float min_nan(float a, float b) { return (isnan(a) || isnan(b)) ? __int_as_float(0x7fffffff) : fminf(a, b); }
+
 __global__ void k_ray_limits(const float* ro, const float* rd, long long R, float h, float* t0o, float* t1o,
                              unsigned int* bounds) {
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -196,8 +202,8 @@ __global__ void k_ray_limits(const float* ro, const float* rd, long long R, floa
         if (ax == 0) { tmin = lo; tmax = hi; }
         else {
             if (tmin > hi || lo > tmax) valid = false;
-            tmin = fmaxf(tmin, lo);       // torch.max propagates NaN, fmaxf does not: NaN only for 0*inf rays
-            tmax = fminf(tmax, hi);
+            tmin = max_nan(tmin, lo);
+            tmax = min_nan(tmax, hi);
         }
     }
     if (!valid) { tmin = -1.f; tmax = -2.f; }

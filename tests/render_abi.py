@@ -22,6 +22,7 @@ TINY = 2.0 ** -126              # fp32 underflow: a step whose fp64 value is bel
 U_BF16 = 2.0 ** -8              # unit roundoff of bf16 (8 significant bits, round to nearest)
 LOG2E, LN2 = 1.0 / math.log(2.0), math.log(2.0)
 MUFU_EX2, MUFU_LG2, MUFU_RCP = 2.0 ** -22, 2.0 ** -22, 2.0 ** -23
+ULP2 = 2.0 ** -22               # expf and log1pf: 2 ulp (CUDA C++ Programming Guide, single-precision maximum ulp errors)
 BW = orc.DEFAULT_OPTS['box_warp']
 BAR = 1e-4                      # the tensor-core 3-pass decode (mlp_mode 1) vs the fp64 oracle
 FWD_BAR = 1e-4                  # fp32 SIMT forward vs the fp64 oracle (tests/test_render_backward_gpu.py TIGHT)
@@ -300,6 +301,278 @@ def three_pass_bars(p64, d64, x64, force_sigmoid=False, use_triplane=True):
     s = torch.sigmoid(-lg[..., 1:] * LN2)
     ds = s * (1 - s) * (LN2 * dl[..., 1:] + MUFU_EX2) + s * (U32 + MUFU_RCP)
     return (ds if force_sigmoid else 1.002 * ds), dl[..., :1]
+
+
+def simt_bars(p64, d64, x64, force_sigmoid=False, use_triplane=True):
+    """Per-point bars (rgb (N,K,32), sigma (N,K,1)) for mlp_mode 0 (k_sample_decode, all fp32), at exact fp32 point
+    coordinates (their rounding, and the grid transform's, are the caller's, as for `three_pass_bars`).  v = 2^-24:
+      gather    per plane 4 fmaf of taps and weights that carry <= 2 roundings each, then (f0 + f1 + f2) / 3 in 3 roundings:
+                |da_c| <= 12 v mean over planes of sum |w| |t_c|
+      layer 1   W1 g1 and b1 lr each rounded once, then 32 fmaf from the bias: |dx_j| <= 34 v (|a| . |W1'_j| + |b1'_j|) +
+                |da| . |W1'_j|
+      hidden    softplus_t = log1pf(expf(x)), slope <= 1; expf and log1pf 2 ulp each: |dh_j| <= |dx_j| + 2^-22 (1 + |h_j|)
+      layer 2   64 fmaf from the rounded bias: |do_k| <= 66 v (|h| . |W2'_k| + |b2'_k|) + |dh| . |W2'_k|
+      sigma     do_0
+      colour    s = 1 / (1 + expf(-o)) (the division and the add rounded): |ds| <= s (1 - s) (|do| + 2^-22) + 2 v s, then
+                1.002 s - 0.001 in two roundings: 1.002 |ds| + v (1.002 s + |colour|)"""
+    C_ = d64['w1'].shape[1]
+    lr = d64.get('lr_mul', 1.0)
+    g1, g2 = lr / math.sqrt(C_), lr / math.sqrt(d64['w2'].shape[1])
+    a = orc.sample_planes(p64, x64, BW, use_triplane).mean(1)                 # (N,K,C)
+    da = 12 * U32 * orc.sample_planes(p64.abs(), x64, BW, use_triplane).mean(1)
+    w1p, b1p = (d64['w1'] * g1).abs(), (d64['b1'] * lr).abs()
+    x = a @ (d64['w1'] * g1).t() + d64['b1'] * lr
+    dx = 34 * U32 * (a.abs() @ w1p.t() + b1p) + da @ w1p.t()
+    h = F.softplus(x)
+    dh = dx + ULP2 * (1 + h.abs())
+    w2p, b2p = (d64['w2'] * g2).abs(), (d64['b2'] * lr).abs()
+    o = h @ (d64['w2'] * g2).t() + d64['b2'] * lr
+    do = 66 * U32 * (h.abs() @ w2p.t() + b2p) + dh @ w2p.t()
+    s = torch.sigmoid(o[..., 1:])
+    ds = s * (1 - s) * (do[..., 1:] + ULP2) + 2 * U32 * s
+    if not force_sigmoid:
+        ds = 1.002 * ds + U32 * (1.002 * s + (1.002 * s - 0.001).abs())
+    return ds, do[..., :1]
+
+
+# ------------------------------------------------------------------------------------------------- per-ray bars of a render
+class Arith:
+    """The rounding model of one renderer kernel, for `ray_oracle`:
+      sample_bars(p64, d64, x64, force_sigmoid, use_triplane) -> per-sample (rgb, sigma) bars of the decoder;
+      alpha = (e_exp, e_sp_rel, e_sp_abs): alpha = 1 - exp(-softplus(smid) dt) with exp relative error e_exp and softplus
+              error e_sp_rel softplus + e_sp_abs (see `alpha_bar`);
+      cdf(S) -> the bar of every importance cdf entry of a ray with S coarse samples."""
+
+    def __init__(self, sample_bars, alpha, cdf):
+        self.sample_bars, self.alpha, self.cdf = sample_bars, alpha, cdf
+
+
+# the fused kernel, mode 1 / mode 2 (tests/test_render_fused_paths_gpu.py): ex2.approx / lg2.approx in the interval alpha
+# and the softplus, and (2 S + 40) v on every cdf entry (fp32 weights, their sum, the division and the scans)
+FUSED_ALPHA = (MUFU_EX2, 4 * MUFU_EX2, 2 * MUFU_EX2)
+FUSED_CDF = lambda S: (2 * S + 40) * U32
+FUSED_MODE1 = Arith(three_pass_bars, FUSED_ALPHA, FUSED_CDF)
+FUSED_MODE2 = Arith(lambda p64, d64, x64, force_sigmoid, use_triplane: single_pass_bars(p64, d64, x64), FUSED_ALPHA, FUSED_CDF)
+
+
+def simt_cdf(S):
+    """The fp32 SIMT importance cdf (render_device.cuh importance_ray), nb = S - 3 bins in nc = ceil(nb / 32) warp chunks:
+    the coarse weights carry ~(5 + nc) v of their transmittance scan, each pooled pdf value 3 v (pooled add, + 0.01,
+    + 1e-5), the total (nc + 5) v (8 lane adds, 5 butterflies), the division v: (2 nc + 14) v relative on every pdf,
+    so as much absolute on a cdf entry <= 1; the in-chunk scan adds <= 5 roundings and every chunk's carry one more, of
+    partial sums <= 1: 6 nc v.  Doubled for the orders this does not follow exactly."""
+    nc = -(-(S - 3) // 32)
+    return 2 * (8 * nc + 14) * U32
+
+
+# k_sample_decode / k_ray_importance / k_ray_composite: expf (2 ulp) and softplus_t = log1pf(expf(x)) (2 ulp each)
+SIMT = Arith(simt_bars, (ULP2, ULP2, ULP2), simt_cdf)
+
+
+def alpha_bar(sig, t, e_exp, e_sp_rel, e_sp_abs):
+    """Bound of a kernel's alpha error per interval, from the fp64 sigma and depths (..,L,1): the exp's relative error
+    on 1 - alpha, the rounding of 1 - exp, and, scaled by (1 - alpha) dt, the softplus error, the rounding of smid =
+    (s_a + s_b) / 2 - 1 through its slope sigmoid(smid), and 6 v of softplus dt for dt and the product."""
+    dt = t[..., 1:, :] - t[..., :-1, :]
+    smid = (sig[..., 1:, :] + sig[..., :-1, :]) / 2 - 1
+    sp = F.softplus(smid)
+    alpha = 1 - torch.exp(-sp * dt)
+    spread = sig[..., 1:, :].abs() + sig[..., :-1, :].abs() + 2
+    return (e_exp * (1 - alpha) + U32 * alpha +
+            (1 - alpha) * (dt.abs() * (e_sp_rel * sp + e_sp_abs + torch.sigmoid(smid) * U32 * spread) + 6 * U32 * sp * dt.abs()))
+
+
+def render_graph(ro, rd, d_c, u_f, c0, f0, white, leaves, importance=orc.importance_depths, left=False):
+    """The oracle's render of a chunk of rays as a function of zero-valued perturbation leaves.  c0 / f0: (sigma masked,
+    colour, slope of sigma, slope of colour, mask) of the coarse samples and of the fine samples at the unperturbed fine
+    depths f0['t'] (f0 None: no fine pass).  `importance(z, w, u, cdf_eps=)` draws the fine depths.  Returns the
+    outputs (m, 37) and the intermediate values the bars need."""
+    e = leaves
+    t_c = d_c + e['t_c']
+    s_c = c0['sig'] + torch.where(c0['mask'], 0, c0['g_sig']) * e['t_c'] + e['s_c']
+    col_c = c0['rgb'] + c0['g_rgb'] * e['t_c'] + e['c_c']
+    x_c = ro[:, None] + t_c * rd[:, None]
+    inf = torch.tensor(float('inf'), device=DEV, dtype=torch.float64)
+    if f0 is None:
+        out, depth, w = orc.march(torch.cat([col_c, x_c], -1)[None], s_c[None], t_c[None], white, -inf, inf,
+                                  alpha_eps=e['a'][None], left_colours=left)
+        o = torch.cat([out[0, :, :32], depth[0], w[0].sum(1), out[0, :, 32:]], -1)
+        return o, dict(t_all=t_c, sig=s_c, col=torch.cat([col_c, x_c], -1), w=w[0], t_f=None)
+    _, _, w = orc.march(torch.cat([col_c, x_c], -1)[None], s_c[None], t_c[None], white, alpha_eps=e['a_c'][None])
+    t_f = importance(t_c[..., 0], w[0, ..., 0], u_f, cdf_eps=e['cdf'])[..., None] + e['t_f']
+    dtf = t_f - f0['t']
+    s_f = f0['sig'] + torch.where(f0['mask'], 0, f0['g_sig']) * dtf + e['s_f']
+    col_f = f0['rgb'] + f0['g_rgb'] * dtf + e['c_f']
+    x_f = ro[:, None] + t_f * rd[:, None]
+    t_all = torch.cat([t_c, t_f], -2)
+    order = torch.sort(t_all.detach(), dim=-2, stable=True)[1]
+    t_all = torch.gather(t_all, -2, order)
+    col = torch.gather(torch.cat([torch.cat([col_c, x_c], -1), torch.cat([col_f, x_f], -1)], -2), -2,
+                       order.expand(-1, -1, 35))
+    sig = torch.gather(torch.cat([s_c, s_f], -2), -2, order)
+    out, depth, w = orc.march(col[None], sig[None], t_all[None], white, -inf, inf, alpha_eps=e['a'][None], left_colours=left)
+    o = torch.cat([out[0, :, :32], depth[0], w[0].sum(1), out[0, :, 32:]], -1)
+    return o, dict(t_all=t_all, sig=sig, col=col, w=w[0], t_f=t_f)
+
+
+def zero_leaves(m, S, Sf, grad=False):
+    """The perturbation leaves of `render_graph` for m rays of S coarse and Sf fine samples: coarse depth, sigma and
+    colour, coarse alpha, cdf, fine depth, sigma and colour, merged alpha."""
+    L = S + Sf
+    shapes = dict(t_c=(m, S, 1), s_c=(m, S, 1), c_c=(m, S, 32))
+    if Sf:
+        shapes.update(a_c=(m, S - 1, 1), cdf=(m, S - 2), t_f=(m, Sf, 1), s_f=(m, Sf, 1), c_f=(m, Sf, 32))
+    shapes['a'] = (m, L - 1, 1)
+    return {k: torch.zeros(s, device=DEV, dtype=torch.float64, requires_grad=grad) for k, s in shapes.items()}
+
+
+def decoded(arith, p64, d64, opts, use_triplane, xyz, rd_s, ray_point=True):
+    """sigma (1,K,1) and colour (1,K,32) in fp64 at points xyz (1,K,3) of one view's planes p64; their slopes along the
+    ray direction rd_s (central differences); their bars: the decoder's (arith) plus the points' fp32 rounding (ray_point
+    and the grid transform: 4 v (|x| + box) per coordinate) times one-sided slopes.  ray_point False: points given
+    exactly in fp32 (p3d_decode_points), so only the grid transform rounds.  bilinear_footprint forms
+    fx = ((x cs + 1) W - 1) / 2 with cs = 2 / box rounded: 2 v |gx| + v (|gx| + 1) before the factor W / 2 and
+    v (|gx| + 1) W after it, which is v (5 |x| + 2.5 box) in units of x: 5 v (|x| + box / 2)."""
+    run = lambda x: orc.run_model(p64, d64, x, opts, use_triplane)
+    rgb, sig = run(xyz)
+    b_rgb, b_sig = arith.sample_bars(p64, d64, xyz, bool(d64.get('force_sigmoid', False)), use_triplane)
+    h = 1e-7
+    beta_x = 4 * U32 * (xyz.abs() + BW) if ray_point else 5 * U32 * (xyz.abs() + BW / 2)
+    g_sig, g_rgb = torch.zeros_like(sig), torch.zeros_like(rgb)
+    for i in range(3):
+        e = torch.zeros_like(xyz)
+        e[..., i] = h
+        rp, sp = run(xyz + e)
+        rm, sm = run(xyz - e)
+        b_sig = b_sig + torch.maximum((sp - sig).abs(), (sig - sm).abs()) / h * beta_x[..., i:i + 1]
+        b_rgb = b_rgb + torch.maximum((rp - rgb).abs(), (rgb - rm).abs()) / h * beta_x[..., i:i + 1]
+        g_sig = g_sig + (sp - sm) / (2 * h) * rd_s[..., i:i + 1]
+        g_rgb = g_rgb + (rp - rm) / (2 * h) * rd_s[..., i:i + 1]
+    return sig, rgb, g_sig, g_rgb, b_sig, b_rgb
+
+
+def ray_oracle(arith, p64, d64, opts, flags, use_triplane, ro, rd, d_c, t0, t1, u_f, Sf, with_bars=True, fine_bars=False):
+    """The fp64 oracle's render of m rays of one view (ro, rd (m,3) fp64, coarse depths d_c (m,S,1), coarse limits t0, t1
+    (m,1), fine uniforms u_f (m,Sf)) with a bar per ray and output component for a kernel of rounding model `arith`.
+
+    The kernel's error is bounded per sample and propagated to first order through the oracle:
+      * per sample: arith.sample_bars plus the point's fp32 rounding times the sigma and colour slopes (`decoded`);
+      * per depth: coarse 16 v (|t| + |t0| + |t1|); fine 8 v (|t| + |t1 - t0|) for the lerp, and arith.cdf(S) on every
+        cdf entry;
+      * per interval alpha: `alpha_bar` with arith.alpha, in both marches.
+    The render is restated as a graph of these perturbations (zero-valued leaves, `render_graph`): the coarse sigma /
+    colour / depth perturbations move the coarse weights, the importance depths (kept differentiable) and, through each
+    fine sample's slope along its ray, the fine sigma and colour.  For each output component o_k of a ray (32 rgb, depth,
+    wsum, 3 xyz), one vector-Jacobian product per component over the chunk (rays are independent) gives
+        bar_k = 2 (sum over leaves |do_k / d leaf| beta_leaf) + floor_k
+    floor_k covers the roundings of the sums that form the output ((L + 8) v relative on each weight and on every partial
+    sum; L = S + Sf).  The factor 2 covers second-order terms.  A fine depth's own bar (`fine_move`, (m, Sf)) is the same
+    sum over the leaves that move it, doubled.
+    Masks: a cull, binarize or crop decision is a jump.  A ray is `near` when one of its samples' fp64 sigma lies within
+    its sigma bar (plus the rounding of the host's sigma_cull) of the threshold, or its |x| / |z| within the position bar
+    of the crop bound.
+
+    Returns (res, ctx): res has o (m,37), t_max, t_min, illdef (rays whose importance pdf is not positive: their cdf is not
+    monotone and searchsorted's result depends on its probe order) and, with_bars, bar (m,37), near (m,), cull_share,
+    fine_move; ctx has what mutated oracles need: samples(t), c0, f0, w (coarse weights), zero leaves, white."""
+    m, S = d_c.shape[:2]
+    white = bool(opts.get('white_back', False))
+
+    def samples(t):
+        xyz = (ro[:, None] + t * rd[:, None]).reshape(1, -1, 3)
+        rd_s = rd[:, None].expand(-1, t.shape[1], -1).reshape(1, -1, 3)
+        sig, rgb, g_sig, g_rgb, b_sig, b_rgb = decoded(arith, p64, d64, opts, use_triplane, xyz, rd_s)
+        sig_m = orc.apply_masks(sig, xyz, BW, flags.get('triplane_crop'), flags.get('cull_clouds'), flags.get('binarize_clouds'))
+        mask = sig_m != sig
+        r = lambda x: x.reshape(m, t.shape[1], -1)
+        return dict(sig=r(sig_m), raw=r(sig), rgb=r(rgb), g_sig=r(g_sig), g_rgb=r(g_rgb), b_sig=r(torch.where(mask, 0, b_sig)),
+                    b_sig_raw=r(b_sig), g_sig_raw=r(g_sig), b_rgb=r(b_rgb), mask=r(mask), xyz=r(xyz), t=t)
+
+    c0 = samples(d_c)
+    w = t_f0 = f0 = None
+    illdef = torch.zeros(m, dtype=torch.bool, device=DEV)
+    if Sf:
+        _, _, w = orc.march(torch.cat([c0['rgb'], c0['xyz']], -1)[None], c0['sig'][None], d_c[None], white)
+        w = w[0, ..., 0]
+        t_f0 = orc.importance_depths(d_c[..., 0], w, u_f)[..., None]
+        wp = F.avg_pool1d(F.max_pool1d(w[:, None], 2, 1, padding=1), 2, 1)[:, 0] + 0.01
+        illdef = (wp[:, 1:-1] + 1e-5).min(1).values <= 1e-6
+        f0 = samples(t_f0)
+    zero = zero_leaves(m, S, Sf)
+    o, mid = render_graph(ro, rd, d_c, u_f, c0, f0, white, zero)
+    res = dict(o=o, t_max=mid['t_all'].max(), t_min=mid['t_all'].min(), illdef=illdef, t_f=t_f0)
+    ctx = dict(samples=samples, c0=c0, f0=f0, w=w, zero=zero, white=white)
+    if not with_bars:
+        return res, ctx
+    leaves = zero_leaves(m, S, Sf, grad=True)
+    o, mid = render_graph(ro, rd, d_c, u_f, c0, f0, white, leaves)
+    # beta of every leaf
+    L = S + Sf
+    span = (t1 - t0).abs()[:, None]
+    beta = dict(t_c=16 * U32 * (d_c.abs() + t0.abs()[:, None] + t1.abs()[:, None]), s_c=c0['b_sig'], c_c=c0['b_rgb'],
+                a=alpha_bar(mid['sig'], mid['t_all'], *arith.alpha))
+    if Sf:
+        beta.update(a_c=alpha_bar(c0['sig'], d_c, *arith.alpha), cdf=torch.full((m, S - 2), arith.cdf(S), device=DEV, dtype=torch.float64),
+                    t_f=8 * U32 * (t_f0.abs() + span), s_f=f0['b_sig'], c_f=f0['b_rgb'])
+    names = list(leaves)
+    bar = torch.zeros(m, 37, device=DEV, dtype=torch.float64)
+    for k in range(37):
+        gs = torch.autograd.grad(o[:, k].sum(), [leaves[n] for n in names], retain_graph=True, allow_unused=True)
+        for n, gk in zip(names, gs):
+            if gk is not None:
+                bar[:, k] += (gk.abs() * beta[n]).reshape(m, -1).sum(1)
+    fine_move = None
+    if Sf and (flags or fine_bars):                 # the fine depths' own bars, for the mask borders and the depth check
+        fine_move = torch.zeros(m, Sf, device=DEV, dtype=torch.float64)
+        tf = mid['t_f'][..., 0]
+        moving = ('t_c', 's_c', 'a_c', 'cdf', 't_f')
+        for f in range(Sf):
+            gs = torch.autograd.grad(tf[:, f].sum(), [leaves[n] for n in moving], retain_graph=True, allow_unused=True)
+            for n, gk in zip(moving, gs):
+                if gk is not None:
+                    fine_move[:, f] += (gk.abs() * beta[n]).reshape(m, -1).sum(1)
+        fine_move = 2 * fine_move
+    res['fine_move'] = fine_move
+    # floors: the roundings of the sums that form each output
+    wts = mid['w'][..., 0].detach()
+    W = wts.sum(1)
+    tm = (mid['t_all'][:, 1:] + mid['t_all'][:, :-1])[..., 0] / 2
+    om = torch.cat([wts[:, :1] * 0, wts], 1) / 2 + torch.cat([wts, wts[:, :1] * 0], 1) / 2
+    rel = 2 * (L + 8) * U32
+    fW = rel * W
+    fD = rel * (wts * tm.abs()).sum(1)
+    floor = torch.zeros_like(bar)
+    floor[:, :32] = 2 * rel * (om[..., None] * (mid['col'][..., :32].detach().abs() + 0.002)).sum(1) + (2 * fW[:, None] if white else 0) + 8 * U32
+    dep = (wts * tm).sum(1) / W
+    floor[:, 32] = (fD + dep.abs() * fW) / W + U32 * dep.abs()
+    floor[:, 33] = fW
+    floor[:, 34:] = 2 * (ro.abs() * fW[:, None] + rd.abs() * fD[:, None] + 3 * U32 * (ro.abs() * W[:, None] + rd.abs() * (wts * tm).sum(1)[:, None])
+                         + (fW[:, None] if white else 0)) + 4 * U32
+    res['bar'] = 2 * bar + floor
+    # rays with a sample within its bar of a jump
+    near = torch.zeros(m, dtype=torch.bool, device=DEV)
+    smps = ((c0, beta['t_c'][..., 0]),) + (((f0, fine_move),) if Sf else ())
+    if flags.get('cull_clouds') or flags.get('binarize_clouds'):
+        thr = cull_sigma(flags.get('cull_clouds') or flags.get('binarize_clouds'))
+        for smp, move in smps:
+            cropped = orc.crop_mask(smp['xyz'].reshape(1, -1, 3), flags['triplane_crop'], BW).reshape(m, -1) if flags.get('triplane_crop') \
+                else torch.zeros(m, smp['t'].shape[1], dtype=torch.bool, device=DEV)
+            # the slope of the unmasked sigma along the ray, times how far the sample's depth may move
+            g_raw = smp['g_sig_raw'][..., 0].abs()
+            b = smp['b_sig_raw'][..., 0] + g_raw * move + 2 * U32 * abs(thr) + 1e-12
+            near |= (~cropped & ((smp['raw'][..., 0] - thr).abs() <= b)).any(1)
+    if flags.get('triplane_crop'):
+        lim = BW / 2 - flags['triplane_crop']
+        for smp, move in smps:
+            bx = 4 * U32 * (smp['xyz'].abs() + BW) + rd.abs()[:, None] * move[..., None] + 2 * U32 * lim
+            near |= ((smp['xyz'][..., [0, 2]].abs() - lim).abs() <= bx[..., [0, 2]]).any(-1).any(1)
+    res['near'] = near
+    res['cull_share'] = None
+    if flags.get('cull_clouds'):
+        unc = ~orc.crop_mask(c0['xyz'].reshape(1, -1, 3), flags['triplane_crop'], BW).reshape(m, -1) if flags.get('triplane_crop') else \
+            torch.ones(m, S, dtype=torch.bool, device=DEV)
+        res['cull_share'] = ((c0['mask'][..., 0] & unc).sum().item(), unc.sum().item())
+    return res, ctx
 
 
 # ------------------------------------------------------------------------------------------------- the training path

@@ -6,7 +6,9 @@ fails it, as it must.  The tree is not modified.
 
 TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane (the TRI lines of
 render_backward.cu), modconv, modconv_paths (more modconv.cu mutations, against tests/test_modconv_paths_gpu.py),
-render_fused and multiplane (the multiplane section of the header render_device.cuh).  Each mutant recompiles every translation unit that includes its source, directly or through other headers.  --files runs other
+render_fused, multiplane (the multiplane section of the header render_device.cuh), render_simt (render_v1.cu, against
+tests/test_render_simt_paths_gpu.py) and render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same
+file).  Each mutant recompiles every translation unit that includes its source, directly or through other headers.  --files runs other
 GPU files against the same mutants instead (to see which of them the rest of the suite catches); the exit code then only
 reports that the run completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
 --json writes {target: {mutation: result}}.
@@ -161,6 +163,43 @@ MULTIPLANE = {
     'zero-padding band above slab D - 1 dropped': ('(fz < (float)g.D + 1.f)', '(fz < (float)(g.D - 1))'),
 }
 
+# render_v1.cu against tests/test_render_simt_paths_gpu.py: value mutations only - no index, bound, shared memory size or
+# launch shape changes, so every access stays in bounds and nothing can hang.  The fallback and NaN mutants act on
+# auto_axis's rays (NaN limits, fallback limits), the depth one on train_cull's rays with W = 0.
+RENDER_SIMT = {
+    'slab test near / far faces swapped': ('const float lo = __fmul_rn(__fsub_rn(neg ? h : -h, o), inv);',
+                                           'const float lo = __fmul_rn(__fsub_rn(neg ? -h : h, o), inv);'),
+    # the running near limit takes the smaller of the two (max_nan's fmaxf turned into fminf)
+    'near limit with fminf': ('? __int_as_float(0x7fffffff) : fmaxf(a, b); }', '? __int_as_float(0x7fffffff) : fminf(a, b); }'),
+    # fmaxf / fminf drop a 0 * inf NaN that torch.maximum / torch.minimum keep
+    'NaN limits dropped': ('tmin = max_nan(tmin, lo);\n            tmax = min_nan(tmax, hi);',
+                           'tmin = fmaxf(tmin, lo);\n            tmax = fminf(tmax, hi);'),
+    # the fallback end of a ray that misses is the largest valid end instead of the largest valid start (renderer.py:170)
+    'fallback end from the largest t1': ('atomicMax(&bounds[3], float_to_ordered(tmin));', 'atomicMax(&bounds[3], float_to_ordered(tmax));'),
+    'depth finalize without NaN -> inf': ('    if (isnan(d)) d = INFINITY;\n    depth[r] = fminf(fmaxf(d, lo), hi);',
+                                          '    depth[r] = fminf(fmaxf(d, lo), hi);'),
+    'white background not added to xyz': ('__fmul_rn(__fadd_rn(v, back), 2.f)', '__fmul_rn(v, 2.f)'),
+    # fine samples per view counted as M max(S, Sf): the view index of a fine sample can only shrink, so it stays in bounds;
+    # equal to the kernel when S <= Sf (s4_sf1 has S > Sf and two views)
+    'fine per-view count from max(S, Sf)': ('sa.per_view = (long long)g.M * g.Sf;', 'sa.per_view = (long long)g.M * max(g.S, g.Sf);'),
+}
+
+# render_device.cuh, the helpers only the SIMT renderer runs (importance_ray, composite_weights) and the 'auto' fallback of
+# coarse_sample_depth, against tests/test_render_simt_paths_gpu.py: value mutations only.  `below` stays within the cdf's
+# nb + 1 entries and the depths' S.  No mutant touches the bitonic sort: an unsorted fine list breaks merge_by_rank's rank
+# positions, leaving merged slots whose colour row index is never written.  The pdf threshold goes to 1e-2 because 1e-3 is
+# equivalent: every bin's pdf is at least 0.01 / (2 + 0.01 nb) > 1e-3.
+RENDER_SIMT_HELPERS = {
+    'pdf floor 0.01 dropped': ('v = __fadd_rn(__fadd_rn(pooled, 0.01f), 1e-5f);', 'v = __fadd_rn(pooled, 1e-5f);'),
+    'max-pool with fminf': ('__fadd_rn(fmaxf(wl, wc), fmaxf(wc, wr))', '__fadd_rn(fminf(wl, wc), fmaxf(wc, wr))'),
+    'cdf carry not added': ('const float incl = warp_scan_add(pdf, lane) + carry;', 'const float incl = warp_scan_add(pdf, lane);'),
+    'below = lo (clamped to nb)': ('const int below = max(lo - 1, 0), above = min(lo, nb);',
+                                   'const int below = min(lo, nb), above = min(lo, nb);'),
+    'pdf denominator threshold 1e-2': ('if (den < 1e-5f) den = 1.f;', 'if (den < 1e-2f) den = 1.f;'),
+    'omega = w_i': ('v = __fmul_rn(__fadd_rn(wl, wr), 0.5f);', 'v = wr;'),
+    'fallback end from the smallest valid start': ('t1 = ordered_to_float(bounds[3]);', 't1 = ordered_to_float(bounds[2]);'),
+}
+
 # target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
 TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
@@ -171,6 +210,8 @@ TARGETS = {
     'modconv_paths': ('modconv.cu', 'tests/test_modconv_paths_gpu.py', MODCONV_PATHS),
     'render_fused': ('render_fused_ws3.cu', 'tests/test_render_fused_paths_gpu.py', RENDER_FUSED),
     'multiplane': ('render_device.cuh', 'tests/test_multiplane_paths_gpu.py', MULTIPLANE),
+    'render_simt': ('render_v1.cu', 'tests/test_render_simt_paths_gpu.py', RENDER_SIMT),
+    'render_simt_helpers': ('render_device.cuh', 'tests/test_render_simt_paths_gpu.py', RENDER_SIMT_HELPERS),
 }
 
 

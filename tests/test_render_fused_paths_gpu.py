@@ -41,7 +41,8 @@ Bars.  The kernel's error is bounded per sample and propagated to first order th
     entry (fp32 weights, their sum, the division and the scans);
   * per interval alpha = 1 - ex2.approx(-log2(e) softplus(smid) dt): 2^-22 (1 - alpha) + v alpha + (1 - alpha) (dt (4
     2^-22 softplus + 2 2^-22 + sigmoid(smid) v (|s_a| + |s_b| + 2)) + 6 v softplus dt), in both marches.
-  The oracle's render is restated as a graph of these perturbations (zero-valued leaves: `_render_graph`): the coarse
+  The oracle's render is restated as a graph of these perturbations (zero-valued leaves: `render_abi.render_graph`, built by
+  `render_abi.ray_oracle` with this kernel's rounding model `render_abi.FUSED_MODE1` / `FUSED_MODE2`): the coarse
   sigma / colour / depth perturbations move the coarse weights, the importance depths (kept differentiable) and, through
   each fine sample's slope along its ray, the fine sigma and colour.  For each output component o_k of a ray (32 rgb,
   depth, wsum, 3 xyz), one vector-Jacobian product per component over a chunk of rays (rays are independent) gives
@@ -78,7 +79,7 @@ import torch
 from oracle import renderer_oracle as orc
 from tests import render_abi as ra
 from tests.render_abi import (BW, DEV, OUTPUTS, U32, Worst, cull_sigma, dec64, decode_points, make_decoder, n_sm,
-                              single_pass_bars, three_pass_bars)
+                              three_pass_bars)
 
 pytestmark = pytest.mark.gpu
 PROF_FUSED = 5                    # profile slot of k_render_ws3 (csrc/p3d_common.cuh)
@@ -91,7 +92,6 @@ EXCLUDE_SHARE = {1: 0.01, 2: 0.05}
 EXCLUDE_SHARE_MASKS = {'eval_flags96': 0.95, 'binarize48': 0.35}
 PIN = 2e-6                        # fp64 device oracle vs the CPU fp32 one: the fp32 run's rounding (measured 7.6e-7)
 FREE_BYTES = 12 << 30             # the 512^2 cases: measured peak 8.1 GB (bench8), with margin
-MUFU = 2.0 ** -22
 OUT_COLS = dict(rgb=slice(0, 32), depth=slice(32, 33), wsum=slice(33, 34), xyz=slice(34, 37))
 AUTO = dict(ray_start='auto', ray_end='auto')
 
@@ -240,93 +240,11 @@ def _limits(name):
     return full(opts['ray_start']), full(opts['ray_end'])
 
 
-def _decoded(name, v, xyz, rd_s, mode):
-    """sigma (1,K,1) and colour (1,K,32) in fp64 at points xyz (1,K,3); their slopes along the ray direction rd_s (central
-    differences); their bars: the decoder's plus the points' fp32 rounding times one-sided slopes."""
-    case = CASES[name]
-    planes, dec, opts, *_ = _inputs(name)
-    tri = not case.get('eg3d')
-    p64, d64 = planes[v:v + 1].to(DEV, torch.float64), dec64(dec)
-    run = lambda x: orc.run_model(p64, d64, x, opts, tri)
-    rgb, sig = run(xyz)
-    if mode == 1:
-        b_rgb, b_sig = three_pass_bars(p64, d64, xyz, force_sigmoid=dec['force_sigmoid'], use_triplane=tri)
-    else:
-        assert tri and not dec['force_sigmoid']
-        b_rgb, b_sig = single_pass_bars(p64, d64, xyz)
-    h = 1e-7
-    beta_x = 4 * U32 * (xyz.abs() + BW)
-    g_sig, g_rgb = torch.zeros_like(sig), torch.zeros_like(rgb)
-    for i in range(3):
-        e = torch.zeros_like(xyz)
-        e[..., i] = h
-        rp, sp = run(xyz + e)
-        rm, sm = run(xyz - e)
-        b_sig = b_sig + torch.maximum((sp - sig).abs(), (sig - sm).abs()) / h * beta_x[..., i:i + 1]
-        b_rgb = b_rgb + torch.maximum((rp - rgb).abs(), (rgb - rm).abs()) / h * beta_x[..., i:i + 1]
-        g_sig = g_sig + (sp - sm) / (2 * h) * rd_s[..., i:i + 1]
-        g_rgb = g_rgb + (rp - rm) / (2 * h) * rd_s[..., i:i + 1]
-    return sig, rgb, g_sig, g_rgb, b_sig, b_rgb
-
-
-def _masks(name, sig, xyz):
-    """(masked sigma, mask) as apply_masks makes them, and the host's cull threshold."""
-    fl = CASES[name].get('flags', {})
-    masked = orc.apply_masks(sig, xyz, BW, fl.get('triplane_crop'), fl.get('cull_clouds'), fl.get('binarize_clouds'))
-    return masked, masked != sig
-
-
-def _alpha_bar(sig, t):
-    """Bound of the kernel's alpha error per interval (module docstring), from the fp64 sigma and depths (..,L,1)."""
-    dt = t[..., 1:, :] - t[..., :-1, :]
-    smid = (sig[..., 1:, :] + sig[..., :-1, :]) / 2 - 1
-    sp = torch.nn.functional.softplus(smid)
-    alpha = 1 - torch.exp(-sp * dt)
-    spread = sig[..., 1:, :].abs() + sig[..., :-1, :].abs() + 2
-    return (MUFU * (1 - alpha) + U32 * alpha +
-            (1 - alpha) * (dt.abs() * (4 * MUFU * sp + 2 * MUFU + torch.sigmoid(smid) * U32 * spread) + 6 * U32 * sp * dt.abs()))
-
-
-def _render_graph(ro, rd, d_c, u_f, c0, f0, white, leaves, floor=0.01, left=False):
-    """The oracle's render of a chunk of rays as a function of zero-valued perturbation leaves.  c0 / f0: (sigma masked,
-    colour, slope of sigma, slope of colour, mask) of the coarse samples and of the fine samples at the unperturbed fine
-    depths f0['t'].  Returns the outputs (m, 37) and the intermediate values the bars need."""
-    e = leaves
-    t_c = d_c + e['t_c']
-    s_c = c0['sig'] + torch.where(c0['mask'], 0, c0['g_sig']) * e['t_c'] + e['s_c']
-    col_c = c0['rgb'] + c0['g_rgb'] * e['t_c'] + e['c_c']
-    x_c = ro[:, None] + t_c * rd[:, None]
-    _, _, w = orc.march(torch.cat([col_c, x_c], -1)[None], s_c[None], t_c[None], white, alpha_eps=e['a_c'][None])
-    t_f = orc.importance_depths(t_c[..., 0], w[0, ..., 0], u_f, floor=floor, cdf_eps=e['cdf'])[..., None] + e['t_f']
-    dtf = t_f - f0['t']
-    s_f = f0['sig'] + torch.where(f0['mask'], 0, f0['g_sig']) * dtf + e['s_f']
-    col_f = f0['rgb'] + f0['g_rgb'] * dtf + e['c_f']
-    x_f = ro[:, None] + t_f * rd[:, None]
-    t_all = torch.cat([t_c, t_f], -2)
-    order = torch.sort(t_all.detach(), dim=-2, stable=True)[1]
-    t_all = torch.gather(t_all, -2, order)
-    col = torch.gather(torch.cat([torch.cat([col_c, x_c], -1), torch.cat([col_f, x_f], -1)], -2), -2,
-                       order.expand(-1, -1, 35))
-    sig = torch.gather(torch.cat([s_c, s_f], -2), -2, order)
-    inf = torch.tensor(float('inf'), device=DEV, dtype=torch.float64)
-    out, depth, w = orc.march(col[None], sig[None], t_all[None], white, -inf, inf, alpha_eps=e['a'][None], left_colours=left)
-    o = torch.cat([out[0, :, :32], depth[0], w[0].sum(1), out[0, :, 32:]], -1)
-    return o, dict(t_all=t_all, sig=sig, col=col, w=w[0], t_f=t_f)
-
-
-def _zero_leaves(m, S, grad=False):
-    L = 2 * S
-    shapes = dict(t_c=(m, S, 1), s_c=(m, S, 1), c_c=(m, S, 32), a_c=(m, S - 1, 1), cdf=(m, S - 2), t_f=(m, S, 1), s_f=(m, S, 1),
-                  c_f=(m, S, 32), a=(m, L - 1, 1))
-    return {k: torch.zeros(s, device=DEV, dtype=torch.float64, requires_grad=grad) for k, s in shapes.items()}
-
-
 def _chunk(name, v, sl, mode, with_bars=True, controls=False):
     """The oracle's outputs (m, 37) for rays `sl` of view v, and (with_bars) their bars (m, 37), the rays to exclude (m,)
-    and the mutated oracles' outputs (controls)."""
+    and the mutated oracles' outputs (controls): ra.ray_oracle with the fused kernel's rounding model."""
     case = CASES[name]
     planes, dec, opts, ro_all, rd_all, u_c_all, u_f_all = _inputs(name)
-    S = case['S']
     M = ro_all.shape[1]
     ro, rd = ro_all[v, sl].double(), rd_all[v, sl].double()
     m = ro.shape[0]
@@ -337,108 +255,24 @@ def _chunk(name, v, sl, mode, with_bars=True, controls=False):
         d_c = orc.stratified_depths(u_c[None], t0[None], t1[None])[0]
     else:
         d_c = orc.stratified_depths(u_c[None], opts['ray_start'], opts['ray_end'], opts.get('disparity_space_sampling', False))[0]
-    white = bool(opts.get('white_back', False))
-
-    def samples(t):
-        xyz = (ro[:, None] + t * rd[:, None]).reshape(1, -1, 3)
-        rd_s = rd[:, None].expand(-1, t.shape[1], -1).reshape(1, -1, 3)
-        sig, rgb, g_sig, g_rgb, b_sig, b_rgb = _decoded(name, v, xyz, rd_s, mode)
-        sig_m, mask = _masks(name, sig, xyz)
-        r = lambda x: x.reshape(m, t.shape[1], -1)
-        return dict(sig=r(sig_m), raw=r(sig), rgb=r(rgb), g_sig=r(g_sig), g_rgb=r(g_rgb), b_sig=r(torch.where(mask, 0, b_sig)),
-                    b_sig_raw=r(b_sig), g_sig_raw=r(g_sig), b_rgb=r(b_rgb), mask=r(mask), xyz=r(xyz), t=t)
-
-    c0 = samples(d_c)
-    _, _, w = orc.march(torch.cat([c0['rgb'], c0['xyz']], -1)[None], c0['sig'][None], d_c[None], white)
-    t_f0 = orc.importance_depths(d_c[..., 0], w[0, ..., 0], u_f)[..., None]
-    # Descending coarse depths give negative weights; where the pdf they make is not positive, the cdf is not monotone and
-    # the reference's searchsorted (and so its fine depths) depends on the search's probe order: such rays are counted,
-    # not compared
-    wp = torch.nn.functional.avg_pool1d(torch.nn.functional.max_pool1d(w[0, ..., 0][:, None], 2, 1, padding=1), 2, 1)[:, 0] + 0.01
-    illdef = (wp[:, 1:-1] + 1e-5).min(1).values <= 1e-6
-    f0 = samples(t_f0)
-    zero = _zero_leaves(m, S)
-    o, mid = _render_graph(ro, rd, d_c, u_f, c0, f0, white, zero)
-    res = dict(o=o, t_max=mid['t_all'].max(), t_min=mid['t_all'].min(), illdef=illdef)
+    tri = not case.get('eg3d')
+    if mode == 2:
+        assert tri and not dec['force_sigmoid']
+    p64 = planes[v:v + 1].to(DEV, torch.float64)
+    res, ctx = ra.ray_oracle(ra.FUSED_MODE1 if mode == 1 else ra.FUSED_MODE2, p64, dec64(dec), opts, case.get('flags', {}), tri,
+                             ro, rd, d_c, t0, t1, u_f, case['S'], with_bars=with_bars)
     if controls:
+        c0, f0, w, zero, white, samples = (ctx[k] for k in ('c0', 'f0', 'w', 'zero', 'white', 'samples'))
         # the colour map without its gain: s - 0.001 instead of 1.002 s - 0.001
         dec_s = dec64(dict(dec, force_sigmoid=True))
-        p64 = planes[v:v + 1].to(DEV, torch.float64)
-        rgb_s = lambda smp: orc.run_model(p64, dec_s, smp['xyz'].reshape(1, -1, 3), opts, not case.get('eg3d'))[0].reshape(m, -1, 32) - 0.001
+        rgb_s = lambda smp: orc.run_model(p64, dec_s, smp['xyz'].reshape(1, -1, 3), opts, tri)[0].reshape(m, -1, 32) - 0.001
         c0s, f0s = dict(c0, rgb=rgb_s(c0)), dict(f0, rgb=rgb_s(f0))
-        res['ctl_colour_map'] = _render_graph(ro, rd, d_c, u_f, c0s, f0s, white, zero)[0]
+        res['ctl_colour_map'] = ra.render_graph(ro, rd, d_c, u_f, c0s, f0s, white, zero)[0]
         # the pdf floor moves the fine depths: decode at the moved depths
-        t_f5 = orc.importance_depths(d_c[..., 0], w[0, ..., 0], u_f, floor=0.005)[..., None]
-        f5 = samples(t_f5)
-        res['ctl_pdf_floor'] = _render_graph(ro, rd, d_c, u_f, c0, f5, white, zero, floor=0.005)[0]
-        res['ctl_omega'] = _render_graph(ro, rd, d_c, u_f, c0, f0, white, zero, left=True)[0]
-    if not with_bars:
-        return res
-    leaves = _zero_leaves(m, S, grad=True)
-    o, mid = _render_graph(ro, rd, d_c, u_f, c0, f0, white, leaves)
-    # beta of every leaf
-    L = 2 * S
-    span = (t1 - t0).abs()[:, None]
-    beta = dict(t_c=16 * U32 * (d_c.abs() + t0.abs()[:, None] + t1.abs()[:, None]), s_c=c0['b_sig'], c_c=c0['b_rgb'],
-                a_c=_alpha_bar(c0['sig'], d_c), cdf=torch.full((m, S - 2), (2 * S + 40) * U32, device=DEV, dtype=torch.float64),
-                t_f=8 * U32 * (t_f0.abs() + span), s_f=f0['b_sig'], c_f=f0['b_rgb'], a=_alpha_bar(mid['sig'], mid['t_all']))
-    names = list(leaves)
-    bar = torch.zeros(m, 37, device=DEV, dtype=torch.float64)
-    for k in range(37):
-        gs = torch.autograd.grad(o[:, k].sum(), [leaves[n] for n in names], retain_graph=True, allow_unused=True)
-        for n, gk in zip(names, gs):
-            if gk is not None:
-                bar[:, k] += (gk.abs() * beta[n]).reshape(m, -1).sum(1)
-    fine_move = None
-    fl = case.get('flags', {})
-    if fl:                                    # the fine depths' own bars, for the mask borders
-        fine_move = torch.zeros(m, S, device=DEV, dtype=torch.float64)
-        tf = mid['t_f'][..., 0]
-        for f in range(S):
-            gs = torch.autograd.grad(tf[:, f].sum(), [leaves[n] for n in ('t_c', 's_c', 'a_c', 'cdf', 't_f')], retain_graph=True,
-                                     allow_unused=True)
-            for n, gk in zip(('t_c', 's_c', 'a_c', 'cdf', 't_f'), gs):
-                if gk is not None:
-                    fine_move[:, f] += (gk.abs() * beta[n]).reshape(m, -1).sum(1)
-        fine_move = 2 * fine_move
-    # floors: the roundings of the sums that form each output
-    wts = mid['w'][..., 0].detach()
-    W = wts.sum(1)
-    tm = (mid['t_all'][:, 1:] + mid['t_all'][:, :-1])[..., 0] / 2
-    om = torch.cat([wts[:, :1] * 0, wts], 1) / 2 + torch.cat([wts, wts[:, :1] * 0], 1) / 2
-    rel = 2 * (L + 8) * U32
-    fW = rel * W
-    fD = rel * (wts * tm.abs()).sum(1)
-    floor = torch.zeros_like(bar)
-    floor[:, :32] = 2 * rel * (om[..., None] * (mid['col'][..., :32].detach().abs() + 0.002)).sum(1) + (2 * fW[:, None] if white else 0) + 8 * U32
-    dep = (wts * tm).sum(1) / W
-    floor[:, 32] = (fD + dep.abs() * fW) / W + U32 * dep.abs()
-    floor[:, 33] = fW
-    floor[:, 34:] = 2 * (ro.abs() * fW[:, None] + rd.abs() * fD[:, None] + 3 * U32 * (ro.abs() * W[:, None] + rd.abs() * (wts * tm).sum(1)[:, None])
-                         + (fW[:, None] if white else 0)) + 4 * U32
-    res['bar'] = 2 * bar + floor
-    # rays with a sample within its bar of a jump
-    near = torch.zeros(m, dtype=torch.bool, device=DEV)
-    if fl.get('cull_clouds') or fl.get('binarize_clouds'):
-        thr = cull_sigma(fl.get('cull_clouds') or fl.get('binarize_clouds'))
-        for smp, move in ((c0, beta['t_c'][..., 0]), (f0, fine_move)):
-            cropped = orc.crop_mask(smp['xyz'].reshape(1, -1, 3), fl['triplane_crop'], BW).reshape(m, -1) if fl.get('triplane_crop') \
-                else torch.zeros(m, S, dtype=torch.bool, device=DEV)
-            # the slope of the unmasked sigma along the ray, times how far the sample's depth may move
-            g_raw = smp['g_sig_raw'][..., 0].abs()
-            b = smp['b_sig_raw'][..., 0] + g_raw * move + 2 * U32 * abs(thr) + 1e-12
-            near |= (~cropped & ((smp['raw'][..., 0] - thr).abs() <= b)).any(1)
-    if fl.get('triplane_crop'):
-        lim = BW / 2 - fl['triplane_crop']
-        for smp, move in ((c0, beta['t_c'][..., 0]), (f0, fine_move)):
-            bx = 4 * U32 * (smp['xyz'].abs() + BW) + rd.abs()[:, None] * move[..., None] + 2 * U32 * lim
-            near |= ((smp['xyz'][..., [0, 2]].abs() - lim).abs() <= bx[..., [0, 2]]).any(-1).any(1)
-    res['near'] = near
-    res['cull_share'] = None
-    if fl.get('cull_clouds'):
-        unc = ~orc.crop_mask(c0['xyz'].reshape(1, -1, 3), fl['triplane_crop'], BW).reshape(m, -1) if fl.get('triplane_crop') else \
-            torch.ones(m, S, dtype=torch.bool, device=DEV)
-        res['cull_share'] = ((c0['mask'][..., 0] & unc).sum().item(), unc.sum().item())
+        floor5 = functools.partial(orc.importance_depths, floor=0.005)
+        f5 = samples(floor5(d_c[..., 0], w, u_f)[..., None])
+        res['ctl_pdf_floor'] = ra.render_graph(ro, rd, d_c, u_f, c0, f5, white, zero, importance=floor5)[0]
+        res['ctl_omega'] = ra.render_graph(ro, rd, d_c, u_f, c0, f0, white, zero, left=True)[0]
     return res
 
 
