@@ -11,7 +11,7 @@ tests/test_render_backward_oracle_cpu.py checks the signed run against torch aut
 Positions are taken as the kernel makes them: ``ro + t rd`` and the tap footprint in fp32 (``taps``).  They are constants of
 the reference graph, so this fixes which texels a sample reads without changing any derivative.
 
-``depth`` > 1 is multiplane tri-planes (dev::trilinear_footprint / slab_texels): planes (N, 3, C*depth, H, W) in the
+``depth`` > 1 is multiplane tri-planes (dev::slab_footprint / dev::plane_tap<true>): planes (N, 3, C*depth, H, W) in the
 reference's indexing (channel c*depth + d is feature c of slab d, as multiplane_oracle.sample_multiplane reads them), 8 taps
 per plane, and the plane gradient comes back in the same indexing.  At depth 1 every function computes what it did before
 the argument existed, bit for bit.
@@ -35,9 +35,9 @@ CHUNK = 1 << 16             # samples per step of the (K, taps, C) intermediates
 
 def taps(xyz: Tensor, H: int, W: int, box_warp: float, use_triplane: bool, depth: int = 1, *, normal_triplane=None,
          slab_align_corners: bool = False):
-    """Taps of points xyz (K,3), in the kernel's fp32.  depth 1: bilinear (dev::bilinear_footprint, tap_texels), texel
+    """Taps of points xyz (K,3), in the kernel's fp32.  depth 1: bilinear (dev::bilinear_footprint, dev::plane_tap<false>), texel
     index p*H*W + y*W + x (-1 outside the plane) and weight wx*wy, each (K,12) in plane-major, then row, then column order.
-    depth D > 1: trilinear (dev::trilinear_footprint, slab_texels), texel index ((p*D + z)*H + y)*W + x and weight
+    depth D > 1: trilinear (dev::slab_footprint, dev::plane_tap<true>), texel index ((p*D + z)*H + y)*W + x and weight
     (wx*wy)*wz, each (K,24): per plane, k & 1 the column, (k >> 1) & 1 the row, k >> 2 the slab (z0, then z0 + 1).
     normal_triplane (plane 2's normal from that plane order) and slab_align_corners exist for negative controls."""
     assert xyz.dtype == torch.float32
@@ -56,7 +56,7 @@ def taps(xyz: Tensor, H: int, W: int, box_warp: float, use_triplane: bool, depth
         fz = (gz + 1) * (D - 1) * 0.5 if slab_align_corners else ((gz + 1) * D - 1) * 0.5
         z0f = torch.floor(fz)
         wz1 = fz - z0f
-        z0 = torch.where((fz > -2) & (fz < D + 1), z0f, torch.full_like(z0f, -4)).long()   # trilinear_footprint's `sane`
+        z0 = torch.where((fz > -2) & (fz < D + 1), z0f, torch.full_like(z0f, -4)).long()   # slab_footprint's `sane`
         for p in range(3):
             for dz, wz in ((0, 1 - wz1[p]), (1, wz1[p])):
                 for dy, wy in ((0, 1 - wy1[p]), (1, wy1[p])):
@@ -206,7 +206,7 @@ def sigma_error_bound(planes_n: Tensor, dec: Dict, xyz: Tensor, box_warp: float,
     """Per point (K,), a bound on the fp32 SIMT decode's sigma error (render_v1.cu): the gather, the pre-activation's
     C + 1 fmas, softplus_t to 4 ulp and the logit's Hd + 1 fmas, each taken over the magnitudes of its operands.  The
     gather: one slab, 12 fmas, two adds and a division by 3 (16u of the features' magnitude); depth > 1, 24 fmas
-    (gather_features3: 8 per plane), the two roundings of the weight (wx wy) wz, two adds and the division (29u)."""
+    (gather_features<*, true>: 8 per plane), the two roundings of the weight (wx wy) wz, two adds and the division (29u)."""
     idx, wgt, flat, x, pre, hs, o = _decoder_forward(planes_n, dec, xyz, box_warp, use_triplane, depth)
     lr = dec.get('lr_mul', 1.0)
     C = dec['w1'].shape[1]

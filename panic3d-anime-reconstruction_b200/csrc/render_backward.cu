@@ -50,27 +50,8 @@ __global__ void __launch_bounds__(128) k_ray_backward(const RayBwdArgs a) {
     int* src = reinterpret_cast<int*>(q + L);
 
     merge_by_rank(a.depth_c + ray * S, a.sigma_c + ray * S, a.depth_f + ray * Sf, a.sigma_f + ray * Sf, S, Sf, t, sg, src, lane);
-    // forward quantities per interval
-    float carry = 1.f, acc_w = 0.f, acc_d = 0.f;
-    for (int base = 0; base < L - 1; base += 32) {
-        const int i = base + lane;
-        float alpha = 0.f, factor = 1.f, tmid = 0.f;
-        if (i < L - 1) {
-            const float delta = t[i + 1] - t[i];
-            const float dens = softplus_t(__fsub_rn(__fmul_rn(__fadd_rn(sg[i], sg[i + 1]), 0.5f), 1.f));
-            alpha = 1.f - expf(-__fmul_rn(dens, delta));
-            factor = __fadd_rn(__fsub_rn(1.f, alpha), 1e-10f);
-            tmid = __fmul_rn(__fadd_rn(t[i], t[i + 1]), 0.5f);
-        }
-        const float incl = warp_scan_mul(factor, lane);
-        float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-        if (lane == 0) excl = 1.f;
-        const float T = carry * excl;
-        const float wi = alpha * T;
-        if (i < L - 1) { w[i] = wi; al[i] = alpha; fc[i] = factor; Tr[i] = T; acc_w += wi; acc_d = fmaf(wi, tmid, acc_d); }
-        carry *= __shfl_sync(0xffffffffu, incl, 31);
-    }
-    const float W = warp_sum(acc_w), D = warp_sum(acc_d);
+    float W, D;                   // the forward's wsum and dnum, bit for bit
+    ray_weights<true>(t, sg, w, L, lane, W, D, al, fc, Tr);
     __syncwarp();
     // q_j = g_rgb . c_j   (lane = channel)
     const float grgb = a.g_rgb[ray * kRgb + lane];
@@ -156,21 +137,9 @@ struct SampleBwdArgs {
 
 constexpr int kXs = 33, kHs = 65, kDs = 36;
 // taps per sample: 4 per plane, 8 per plane for multiplane tri-planes (TRI)
-template <bool TRI> constexpr int kTaps = TRI ? 24 : 12;
+template <bool TRI> constexpr int kTaps = 3 * kPlaneTaps<TRI>;
 template <bool TRI> constexpr size_t kBwdSmemFloats = (size_t)kHidden * kC + kOut * kHidden + kHidden + 36 +
                                                       (size_t)kT * (kXs + kHs + kHs + kDs + kHs + kXs) + kT * kTaps<TRI> * 2 + kT * 2 + kT;
-
-// texel indices (p*H*W + y*W + x, or -1) and bilinear weights of one plane, from the forward's dev::bilinear_footprint
-__device__ __forceinline__ void tap_texels(const Geom& g, int plane, float2 c, int2* out) {
-    const Footprint f = bilinear_footprint(g, c.x, c.y);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int xi = f.x0 + (k & 1), yi = f.y0 + (k >> 1);
-        const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H);
-        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);
-        out[k] = make_int2(ok ? (plane * g.H + yi) * g.W + xi : -1, __float_as_int(ok ? wgt : 0.f));
-    }
-}
 
 // TRI: multiplane tri-planes (g.D > 1): trilinear re-gather, 8 taps per plane scattered to the (N,3,D,H,W,C) gradient
 template <bool BF16, bool TRI>
@@ -224,8 +193,7 @@ __global__ void __launch_bounds__(kT) k_sample_backward(const SampleBwdArgs a) {
             }
             if (qd < 3) {                                         // lanes 0..2 of a sample record plane qd's taps
                 if (ok) {
-                    if constexpr (TRI) slab_texels(g, qd, plane_coords(g, qd, px, py, pz), plane_normal(g, qd, px, py, pz), s_tap + local * NT + qd * PT);
-                    else tap_texels(g, qd, plane_coords(g, qd, px, py, pz), s_tap + local * NT + qd * PT);
+                    plane_texels<TRI>(g, qd, plane_coords(g, qd, px, py, pz), plane_normal(g, qd, px, py, pz), s_tap + local * NT + qd * PT);
                 } else {
 #pragma unroll
                     for (int k = 0; k < PT; ++k) s_tap[local * NT + qd * PT + k] = make_int2(-1, 0);

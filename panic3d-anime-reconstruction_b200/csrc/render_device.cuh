@@ -116,7 +116,7 @@ __device__ __forceinline__ float2 plane_coords(const Geom& g, int p, float x, fl
 
 // grid_sample's bilinear footprint of plane coordinates (ca, cb): the top-left texel (x0, y0) and the 1-D weights of columns
 // x0, x0 + 1 and rows y0, y0 + 1.  A point that is NaN or lies more than a texel outside the plane gets x0 = y0 = -4, so all
-// four taps fall outside.  The forward gathers (plane_taps, fused::write_tap_row) and the backward scatter (tap_texels)
+// four taps fall outside.  The forward gathers (plane_taps, fused::write_tap_row) and the backward scatter (plane_texels)
 // all take their taps from here, so the gradients land on exactly the texels and weights the forward used.
 struct Footprint {
     int x0, y0;
@@ -135,31 +135,11 @@ __device__ __forceinline__ Footprint bilinear_footprint(const Geom& g, float ca,
     return f;
 }
 
-struct Tap4 {
-    long long off[4];
-    float w[4];
-};
-
-__device__ __forceinline__ Tap4 plane_taps(const Geom& g, long long base, float2 c) {
-    const Footprint f = bilinear_footprint(g, c.x, c.y);
-    Tap4 t;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int xi = f.x0 + (k & 1), yi = f.y0 + (k >> 1);
-        const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H);
-        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);
-        t.w[k] = ok ? wgt : 0.f;
-        t.off[k] = base + (ok ? (long long)yi * g.stride_row + (long long)xi * g.stride_col : 0ll);
-    }
-    return t;
-}
-
 // -------------------------------------------------------------------------------------------
 // Multiplane tri-planes (triplane_depth D > 1).  renderer.py:84-94: each plane is a stack of D slabs sampled by a 5-D
 // grid_sample (trilinear, zero padding, align_corners=False).  project_onto_planes keeps all three components of
 // coordinates @ inv(plane_axes); the third indexes the slabs.  Slab d of plane p of a view starts at
-// p * stride_plane + d * H * stride_row.  The forward taps (plane_taps3) and the backward's texels (slab_texels) live side
-// by side here and come from one footprint, so the gradients land on exactly the texels and weights the forward read.
+// p * stride_plane + d * H * stride_row.
 // -------------------------------------------------------------------------------------------
 // The slab (normal-axis) coordinate of plane p: z, y, then x for P3D_PLANES_PANIC3D or y otherwise.
 __device__ __forceinline__ float plane_normal(const Geom& g, int p, float x, float y, float z) {
@@ -167,117 +147,115 @@ __device__ __forceinline__ float plane_normal(const Geom& g, int p, float x, flo
     return p == 0 ? z : (p == 1 ? y : (pm ? x : y));
 }
 
-// grid_sample's trilinear footprint: the bilinear one in the plane, and along the normal the first slab z0 with the weights
-// of slabs z0 and z0 + 1.  Slabs outside [0, D) contribute zero; a NaN or far-away normal coordinate gets z0 = -4.
-struct Footprint3 {
-    Footprint f;
+// grid_sample's footprint along the normal: the first slab z0 and the weights of slabs z0 and z0 + 1.  Slabs outside
+// [0, D) contribute zero; a NaN or far-away normal coordinate gets z0 = -4.
+struct SlabFootprint {
     int z0;
     float wz0, wz1;
 };
-__device__ __forceinline__ Footprint3 trilinear_footprint(const Geom& g, float ca, float cb, float cn) {
-    Footprint3 t;
-    t.f = bilinear_footprint(g, ca, cb);
+__device__ __forceinline__ SlabFootprint slab_footprint(const Geom& g, float cn) {
     const float gz = __fmul_rn(cn, g.coord_scale);
     const float fz = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)g.D), 1.f), 0.5f);
     const bool sane = (fz > -2.f) && (fz < (float)g.D + 1.f);
     const float z0f = floorf(fz);
-    t.wz1 = fz - z0f;
-    t.wz0 = 1.f - t.wz1;
-    t.z0 = sane ? (int)z0f : -4;
-    return t;
+    SlabFootprint s;
+    s.wz1 = fz - z0f;
+    s.wz0 = 1.f - s.wz1;
+    s.z0 = sane ? (int)z0f : -4;
+    return s;
 }
 
-// the 8 taps of one plane: k & 3 is the bilinear tap of plane_taps, k >> 2 the slab (z0, then z0 + 1)
-struct Tap8 {
-    long long off[8];
-    float w[8];
+// -------------------------------------------------------------------------------------------
+// The taps of one plane: 4 bilinear ones, or for multiplane planes (TRI) 8 = those 4 in slab z0, then in slab z0 + 1.
+// plane_tap gives tap k: texel (x0 + (k & 1), y0 + ((k >> 1) & 1), z0 + (k >> 2)) (z = 0 on one-slab planes), its weight
+// (wx wy) wz and whether it lies inside the plane.  The forward's element offsets (plane_taps) and the backward's scatter
+// list (plane_texels) both take their taps from it, so the gradients land on exactly the texels and weights the forward read.
+// -------------------------------------------------------------------------------------------
+template <bool TRI> constexpr int kPlaneTaps = TRI ? 8 : 4;
+
+template <bool TRI>
+__device__ __forceinline__ bool plane_tap(const Geom& g, const Footprint& f, const SlabFootprint& s, int k, int& x, int& y, int& z,
+                                          float& w) {
+    x = f.x0 + (k & 1); y = f.y0 + ((k >> 1) & 1); z = TRI ? s.z0 + (k >> 2) : 0;
+    w = ((k & 1) ? f.wx1 : f.wx0) * (((k >> 1) & 1) ? f.wy1 : f.wy0);
+    if constexpr (TRI) w = w * ((k >> 2) ? s.wz1 : s.wz0);
+    return (x >= 0) && (x < g.W) && (y >= 0) && (y < g.H) && (!TRI || ((z >= 0) && (z < g.D)));
+}
+
+// element offsets (base + slab + row + column) and weights of plane coordinates c; cn, the normal coordinate, is read for TRI
+template <bool TRI>
+struct Taps {
+    long long off[kPlaneTaps<TRI>];
+    float w[kPlaneTaps<TRI>];
 };
-__device__ __forceinline__ Tap8 plane_taps3(const Geom& g, long long base, float2 c, float cn) {
-    const Footprint3 t = trilinear_footprint(g, c.x, c.y, cn);
+template <bool TRI>
+__device__ __forceinline__ Taps<TRI> plane_taps(const Geom& g, long long base, float2 c, float cn) {
+    const Footprint f = bilinear_footprint(g, c.x, c.y);
+    const SlabFootprint s = TRI ? slab_footprint(g, cn) : SlabFootprint{};
     const long long slab = (long long)g.H * g.stride_row;
-    Tap8 r;
+    Taps<TRI> r;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const int xi = t.f.x0 + (k & 1), yi = t.f.y0 + ((k >> 1) & 1), zi = t.z0 + (k >> 2);
-        const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H) && (zi >= 0) && (zi < g.D);
-        const float wgt = ((k & 1) ? t.f.wx1 : t.f.wx0) * (((k >> 1) & 1) ? t.f.wy1 : t.f.wy0) * ((k >> 2) ? t.wz1 : t.wz0);
-        r.w[k] = ok ? wgt : 0.f;
-        r.off[k] = base + (ok ? (long long)zi * slab + (long long)yi * g.stride_row + (long long)xi * g.stride_col : 0ll);
+    for (int k = 0; k < kPlaneTaps<TRI>; ++k) {
+        int x, y, z;
+        float w;
+        const bool ok = plane_tap<TRI>(g, f, s, k, x, y, z, w);
+        long long o = (long long)y * g.stride_row + (long long)x * g.stride_col;
+        if constexpr (TRI) o += (long long)z * slab;
+        r.w[k] = ok ? w : 0.f;
+        r.off[k] = base + (ok ? o : 0ll);
     }
     return r;
 }
 
-// texel indices ((p * D + z) * H + y) * W + x in the backward's (N,3,D,H,W,C) gradient (or -1) and weights of plane p's taps,
-// in plane_taps3's order
-__device__ __forceinline__ void slab_texels(const Geom& g, int plane, float2 c, float cn, int2* out) {
-    const Footprint3 t = trilinear_footprint(g, c.x, c.y, cn);
+// texel indices ((p * D + z) * H + y) * W + x in the backward's (N,3,D,H,W,C) gradient (D = 1 on one-slab planes), or -1,
+// and the weight bits of plane p's taps; cn is read for TRI
+template <bool TRI>
+__device__ __forceinline__ void plane_texels(const Geom& g, int plane, float2 c, float cn, int2* out) {
+    const Footprint f = bilinear_footprint(g, c.x, c.y);
+    const SlabFootprint s = TRI ? slab_footprint(g, cn) : SlabFootprint{};
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const int xi = t.f.x0 + (k & 1), yi = t.f.y0 + ((k >> 1) & 1);
-        const int z = t.z0 + (k >> 2);
-        const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H) && (z >= 0) && (z < g.D);
-        const float wgt = ((k & 1) ? t.f.wx1 : t.f.wx0) * (((k >> 1) & 1) ? t.f.wy1 : t.f.wy0) * ((k >> 2) ? t.wz1 : t.wz0);
-        out[k] = make_int2(ok ? ((plane * g.D + z) * g.H + yi) * g.W + xi : -1, __float_as_int(ok ? wgt : 0.f));
+    for (int k = 0; k < kPlaneTaps<TRI>; ++k) {
+        int x, y, z;
+        float w;
+        const bool ok = plane_tap<TRI>(g, f, s, k, x, y, z, w);
+        const int pz = TRI ? plane * g.D + z : plane;
+        out[k] = make_int2(ok ? (pz * g.H + y) * g.W + x : -1, __float_as_int(ok ? w : 0.f));
     }
 }
 
-// channels [4q, 4q+4) of the plane mean at (x, y, z), trilinear per plane
-template <bool BF16>
-__device__ __forceinline__ float4 gather_features3(const void* planes, const Geom& g, int view, float x, float y, float z, int q) {
-    const long long vbase = (long long)view * g.stride_view + 4 * q;
-    float4 f[3];
-#pragma unroll
-    for (int p = 0; p < 3; ++p) {
-        const Tap8 t = plane_taps3(g, vbase + p * g.stride_plane, plane_coords(g, p, x, y, z), plane_normal(g, p, x, y, z));
-        float4 v[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[k] = load_quad<BF16>(planes, t.off[k]);
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            a.x = fmaf(v[k].x, t.w[k], a.x);
-            a.y = fmaf(v[k].y, t.w[k], a.y);
-            a.z = fmaf(v[k].z, t.w[k], a.z);
-            a.w = fmaf(v[k].w, t.w[k], a.w);
-        }
-        f[p] = a;
-    }
-    float4 r;
-    r.x = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].x, f[1].x), f[2].x), 3.f);
-    r.y = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].y, f[1].y), f[2].y), 3.f);
-    r.z = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].z, f[1].z), f[2].z), 3.f);
-    r.w = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].w, f[1].w), f[2].w), 3.f);
-    return r;
-}
-
-// TRI: multiplane planes (Geom::D > 1), gather_features3; otherwise one slab per plane
+// channels [4q, 4q+4) of the plane mean at (x, y, z); TRI: multiplane planes (Geom::D > 1), trilinear per plane.  The loads
+// of all three planes go out together on one-slab planes (12 taps), while multiplane planes (24 taps) are gathered one plane
+// at a time: with all 24 loads in flight, k_sample_backward<*, true> took 11 % longer (H100 80GB HBM3, 700 W power limit).
 template <bool BF16, bool TRI = false>
 __device__ __forceinline__ float4 gather_features(const void* planes, const Geom& g, int view, float x, float y, float z, int q) {
-    if constexpr (TRI) return gather_features3<BF16>(planes, g, view, x, y, z, q);
+    constexpr int NT = kPlaneTaps<TRI>, PB = TRI ? 1 : 3;
     const long long vbase = (long long)view * g.stride_view + 4 * q;
-    Tap4 t0 = plane_taps(g, vbase, plane_coords(g, 0, x, y, z));
-    Tap4 t1 = plane_taps(g, vbase + g.stride_plane, plane_coords(g, 1, x, y, z));
-    Tap4 t2 = plane_taps(g, vbase + 2 * g.stride_plane, plane_coords(g, 2, x, y, z));
-    float4 v[12];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        v[k] = load_quad<BF16>(planes, t0.off[k]);
-        v[4 + k] = load_quad<BF16>(planes, t1.off[k]);
-        v[8 + k] = load_quad<BF16>(planes, t2.off[k]);
-    }
     float4 f[3];
 #pragma unroll
-    for (int p = 0; p < 3; ++p) {
-        const Tap4& t = p == 0 ? t0 : (p == 1 ? t1 : t2);
-        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int p0 = 0; p0 < 3; p0 += PB) {
+        Taps<TRI> t[PB];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            a.x = fmaf(v[4 * p + k].x, t.w[k], a.x);
-            a.y = fmaf(v[4 * p + k].y, t.w[k], a.y);
-            a.z = fmaf(v[4 * p + k].z, t.w[k], a.z);
-            a.w = fmaf(v[4 * p + k].w, t.w[k], a.w);
+        for (int p = 0; p < PB; ++p) {
+            const int pl = p0 + p;
+            t[p] = plane_taps<TRI>(g, vbase + pl * g.stride_plane, plane_coords(g, pl, x, y, z), plane_normal(g, pl, x, y, z));
         }
-        f[p] = a;
+        float4 v[PB][NT];
+#pragma unroll
+        for (int k = 0; k < NT; ++k)
+#pragma unroll
+            for (int p = 0; p < PB; ++p) v[p][k] = load_quad<BF16>(planes, t[p].off[k]);
+#pragma unroll
+        for (int p = 0; p < PB; ++p) {
+            float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int k = 0; k < NT; ++k) {
+                a.x = fmaf(v[p][k].x, t[p].w[k], a.x);
+                a.y = fmaf(v[p][k].y, t[p].w[k], a.y);
+                a.z = fmaf(v[p][k].z, t[p].w[k], a.z);
+                a.w = fmaf(v[p][k].w, t[p].w[k], a.w);
+            }
+            f[p0 + p] = a;
+        }
     }
     float4 r;
     r.x = __fdiv_rn(__fadd_rn(__fadd_rn(f[0].x, f[1].x), f[2].x), 3.f);
@@ -304,9 +282,11 @@ __device__ __forceinline__ float apply_masks(const Geom& g, float sigma, float x
 //   alpha_i = 1 - exp(-softplus((s_i+s_{i+1})/2 - 1) * (t_{i+1}-t_i)),
 //   w_i = alpha_i * prod_{k<i} (1 - alpha_k + 1e-10)
 // t, sg: L sorted samples in shared memory; writes w[0..L-2]; returns (sum w, sum w*t_mid) on all lanes.
+// KEEP (the backward's k_ray_backward): also writes alpha_i, 1 - alpha_i + 1e-10 and T_i to al, fc and Tr.
 // -------------------------------------------------------------------------------------------
+template <bool KEEP = false>
 __device__ __forceinline__ void ray_weights(const float* t, const float* sg, float* w, int L, int lane,
-                                            float& wsum, float& dnum) {
+                                            float& wsum, float& dnum, float* al = nullptr, float* fc = nullptr, float* Tr = nullptr) {
     float carry = 1.f, acc_w = 0.f, acc_d = 0.f;
     for (int base = 0; base < L - 1; base += 32) {
         const int i = base + lane;
@@ -323,7 +303,11 @@ __device__ __forceinline__ void ray_weights(const float* t, const float* sg, flo
         if (lane == 0) excl = 1.f;
         const float T = carry * excl;
         const float wi = alpha * T;
-        if (i < L - 1) { w[i] = wi; acc_w += wi; acc_d = fmaf(wi, tmid, acc_d); }
+        if (i < L - 1) {
+            w[i] = wi;
+            if constexpr (KEEP) { al[i] = alpha; fc[i] = factor; Tr[i] = T; }
+            acc_w += wi; acc_d = fmaf(wi, tmid, acc_d);
+        }
         carry *= __shfl_sync(0xffffffffu, incl, 31);
     }
     wsum = warp_sum(acc_w);

@@ -300,11 +300,15 @@ __global__ void __launch_bounds__(128) k_ray_composite(const CompositeArgs a) {
     }
 }
 
-// nan_to_num(nan=inf) then clamp(min(depths), max(depths)) over the whole batch.  ray_marcher.py:49-50
-__global__ void k_depth_finalize(float* depth, long long R, const unsigned int* bounds) {
+// nan_to_num(nan=inf) then clamp(min(depths), max(depths)) over the whole batch.  ray_marcher.py:49-50.  The bounds are the
+// workspace's ordered uints (bounds[0..1]), or two floats from the caller when the clamp was deferred (defer_depth_clamp).
+__device__ __forceinline__ float depth_bound(unsigned int b) { return ordered_to_float(b); }
+__device__ __forceinline__ float depth_bound(float b) { return b; }
+template <typename B>
+__global__ void k_depth_finalize(float* depth, long long R, const B* bounds) {
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= R) return;
-    const float lo = ordered_to_float(bounds[0]), hi = ordered_to_float(bounds[1]);
+    const float lo = depth_bound(bounds[0]), hi = depth_bound(bounds[1]);
     float d = depth[r];
     if (isnan(d)) d = INFINITY;
     depth[r] = fminf(fmaxf(d, lo), hi);
@@ -312,13 +316,6 @@ __global__ void k_depth_finalize(float* depth, long long R, const unsigned int* 
 
 __global__ void k_bounds_to_float(const unsigned int* bounds, float* out2) {
     if (threadIdx.x < 2) out2[threadIdx.x] = ordered_to_float(bounds[threadIdx.x]);
-}
-__global__ void k_depth_finalize_f(float* depth, long long R, const float* bounds2) {
-    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
-    float d = depth[r];
-    if (isnan(d)) d = INFINITY;
-    depth[r] = fminf(fmaxf(d, bounds2[0]), bounds2[1]);
 }
 
 template <int MODE>
@@ -356,7 +353,7 @@ int launch_bounds_to_float(const unsigned int* bounds, float* out2, cudaStream_t
     return P3D_OK;
 }
 int launch_depth_finalize_f(float* depth, long long R, const float* bounds2, cudaStream_t stream) {
-    k_depth_finalize_f<<<(unsigned)((R + 255) / 256), 256, 0, stream>>>(depth, R, bounds2);
+    k_depth_finalize<<<(unsigned)((R + 255) / 256), 256, 0, stream>>>(depth, R, bounds2);
     P3D_LAUNCH_CHECK();
     return P3D_OK;
 }

@@ -5,12 +5,13 @@ fails it, as it must.  The tree is not modified.
     python tests/run_mutations.py TARGET [TARGET ...] [--files F ...] [--json out.json] [--build-only]
 
 TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane (the TRI lines of
-render_backward.cu), modconv, modconv_paths (more modconv.cu mutations, against tests/test_modconv_paths_gpu.py),
-render_fused, multiplane (the multiplane section of the header render_device.cuh), render_simt (render_v1.cu, against
-tests/test_render_simt_paths_gpu.py) and render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same
-file).  Each mutant recompiles every translation unit that includes its source, directly or through other headers.  --files runs other
-GPU files against the same mutants instead (to see which of them the rest of the suite catches); the exit code then only
-reports that the run completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
+render_backward.cu), render_taps (the tap enumeration of render_device.cuh, against tests/test_render_backward_paths_gpu.py),
+modconv, modconv_paths (more modconv.cu mutations, against tests/test_modconv_paths_gpu.py), render_fused, multiplane (the
+multiplane section of the header render_device.cuh), render_simt (render_v1.cu, against tests/test_render_simt_paths_gpu.py)
+and render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same file).  Each mutant recompiles every
+translation unit that includes its source, directly or through other headers.  --files runs other GPU files against the
+same mutants instead (to see which of them the rest of the suite catches); the exit code then only reports that the run
+completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
 --json writes {target: {mutation: result}}.
 """
 import argparse
@@ -65,8 +66,7 @@ PASTE_FRONT = {
     'nearest row rounded half up': ('floorf((float)oy * a.scale)', 'floorf(((float)oy + 0.5f) * a.scale)'),
 }
 
-# render_backward.cu: every mutation changes a value, never an index or a bound that guards a memory access (the tap
-# mutation narrows the bound, so it only drops taps).
+# render_backward.cu: every mutation changes a value, never an index or a bound that guards a memory access.
 # The depth gate `depth_raw >= lo_b` is not mutated: a ray's unclamped depth is a weighted mean of its interval midpoints,
 # which lie strictly inside [min depth, max depth] of the batch, so no case can put it on the bound and `>` equals `>=`.
 RENDER_BACKWARD = {
@@ -75,15 +75,13 @@ RENDER_BACKWARD = {
     'interval softplus derivative linear branch 1 -> 0': ('smid > 20.f ? 1.f : sigmoid_t(smid)', 'smid > 20.f ? 0.f : sigmoid_t(smid)'),
     'white background term without g_xyz': ('2.f * back * (grgb_sum + gx_sum)', '2.f * back * (grgb_sum)'),
     'suffix term not divided by 1 - alpha': ('Tr[i] * P - suffix / fc[i];', 'Tr[i] * P - suffix;'),
-    'tap bound xi < W - 1': ('const bool ok = (xi >= 0) && (xi < g.W) && (yi >= 0) && (yi < g.H);\n        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);\n        out[k]',
-                             'const bool ok = (xi >= 0) && (xi < g.W - 1) && (yi >= 0) && (yi < g.H);\n        const float wgt = ((k & 1) ? f.wx1 : f.wx0) * ((k >> 1) ? f.wy1 : f.wy0);\n        out[k]'),
     'd_w1 scaled by the bias gain': ('acc[i][j] * g.w1_gain);', 'acc[i][j] * g.b1_gain);'),
     'd_b2 scaled by the weight gain': ('atomicAdd(a.d_b2 + tid, acc * g.b2_gain);', 'atomicAdd(a.d_b2 + tid, acc * g.w2_gain);'),
     'omega without its 1/2': ('om = 0.5f * (wl + wr);', 'om = (wl + wr);'),
 }
 
 # render_backward.cu, the multiplane (TRI) lines of k_sample_backward: value mutations that keep every access in bounds (the
-# view offset without D only shrinks it, the scatter bound only drops taps, the normal stays bounds-checked in slab_texels).
+# view offset without D only shrinks it, the scatter bound only drops taps, the normal stays bounds-checked in plane_tap).
 RENDER_BACKWARD_MULTIPLANE = {
     'per-view gradient offset without D': ('(long long)3 * (TRI ? g.D : 1) * g.H', '(long long)3 * g.H'),
     'scatter stopped after the first 12 of 24 taps': ('for (int k = 0; k < NT; ++k) {', 'for (int k = 0; k < 12; ++k) {'),
@@ -150,14 +148,13 @@ MULTIPLANE = {
     'slab coordinate with align_corners=True': (
         'const float fz = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)g.D), 1.f), 0.5f);',
         'const float fz = __fmul_rn(__fmul_rn(__fadd_rn(gz, 1.f), (float)(g.D - 1)), 0.5f);'),
-    'slab index off by one': ('t.z0 = sane ? (int)z0f : -4;', 't.z0 = sane ? (int)z0f + 1 : -4;'),
+    'slab index off by one': ('s.z0 = sane ? (int)z0f : -4;', 's.z0 = sane ? (int)z0f + 1 : -4;'),
     'EG3D plane 2 normal taken as x': ('(pm ? x : y));', '(pm ? x : x));'),
-    'depth axis clamped instead of zero-padded': (', zi = t.z0 + (k >> 2);', ', zi = min(max(t.z0 + (k >> 2), 0), g.D - 1);'),
-    'backward scatters to one slab only': ('const int z = t.z0 + (k >> 2);', 'const int z = t.z0;'),
+    'depth axis clamped instead of zero-padded': ('z = TRI ? s.z0 + (k >> 2) : 0;', 'z = TRI ? min(max(s.z0 + (k >> 2), 0), g.D - 1) : 0;'),
+    'taps of slab z0 + 1 taken from slab z0': ('z = TRI ? s.z0 + (k >> 2) : 0;', 'z = TRI ? s.z0 : 0;'),
     'slab offset from plane_w instead of plane_h': ('const long long slab = (long long)g.H * g.stride_row;',
                                                     'const long long slab = (long long)g.W * g.stride_row;'),
-    # the backward's weight of slab z0 + 1 (slab_texels; the same line in plane_taps3 is followed by `r.w[k]`)
-    'backward weight of slab z0 + 1 taken as z0\'s': ('t.wz1 : t.wz0);\n        out[k]', 't.wz0 : t.wz0);\n        out[k]'),
+    'weight of slab z0 + 1 taken as z0\'s': ('((k >> 2) ? s.wz1 : s.wz0)', '((k >> 2) ? s.wz0 : s.wz0)'),
     # the normal's zero-padding bands dropped: a point within a slab below slab 0 (or above slab D - 1) reads nothing
     'zero-padding band below slab 0 dropped': ('(fz > -2.f) &&', '(fz >= 0.f) &&'),
     'zero-padding band above slab D - 1 dropped': ('(fz < (float)g.D + 1.f)', '(fz < (float)(g.D - 1))'),
@@ -165,7 +162,8 @@ MULTIPLANE = {
 
 # render_v1.cu against tests/test_render_simt_paths_gpu.py: value mutations only - no index, bound, shared memory size or
 # launch shape changes, so every access stays in bounds and nothing can hang.  The fallback and NaN mutants act on
-# auto_axis's rays (NaN limits, fallback limits), the depth one on train_cull's rays with W = 0.
+# auto_axis's rays (NaN limits, fallback limits), the depth one on train_cull's rays with W = 0 (k_depth_finalize is the
+# clamp of both the direct and the deferred path).
 RENDER_SIMT = {
     'slab test near / far faces swapped': ('const float lo = __fmul_rn(__fsub_rn(neg ? h : -h, o), inv);',
                                            'const float lo = __fmul_rn(__fsub_rn(neg ? -h : h, o), inv);'),
@@ -200,12 +198,19 @@ RENDER_SIMT_HELPERS = {
     'fallback end from the smallest valid start': ('t1 = ordered_to_float(bounds[3]);', 't1 = ordered_to_float(bounds[2]);'),
 }
 
+# render_device.cuh, the tap enumeration every SIMT gather and scatter shares (plane_tap), against
+# tests/test_render_backward_paths_gpu.py: the narrowed bound only drops taps.
+RENDER_TAPS = {
+    'tap bound xi < W - 1': ('(x < g.W)', '(x < g.W - 1)'),
+}
+
 # target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
 TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
     'paste_front': ('paste_front.cu', 'tests/test_paste_paths_gpu.py', PASTE_FRONT),
     'render_backward': ('render_backward.cu', 'tests/test_render_backward_paths_gpu.py', RENDER_BACKWARD),
     'render_backward_multiplane': ('render_backward.cu', 'tests/test_multiplane_paths_gpu.py', RENDER_BACKWARD_MULTIPLANE),
+    'render_taps': ('render_device.cuh', 'tests/test_render_backward_paths_gpu.py', RENDER_TAPS),
     'modconv': ('modconv.cu', 'tests/test_modconv_gpu.py', MODCONV),
     'modconv_paths': ('modconv.cu', 'tests/test_modconv_paths_gpu.py', MODCONV_PATHS),
     'render_fused': ('render_fused_ws3.cu', 'tests/test_render_fused_paths_gpu.py', RENDER_FUSED),

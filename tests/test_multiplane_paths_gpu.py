@@ -98,7 +98,7 @@ def _inputs(name):
 
 
 def _normal_fz(xyz, D, box_warp, use_triplane):
-    """(3,K) fp32 slab coordinate fz of every plane (dev::plane_normal, trilinear_footprint): slab d is centred on fz = d."""
+    """(3,K) fp32 slab coordinate fz of every plane (dev::plane_normal, dev::slab_footprint): slab d is centred on fz = d."""
     s = (2.0 / box_warp) * xyz
     gz = torch.stack([s[:, 2], s[:, 1], s[:, 0 if use_triplane else 1]])
     return ((gz + 1) * D - 1) * 0.5
