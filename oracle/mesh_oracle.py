@@ -1,7 +1,10 @@
 """TEST INFRASTRUCTURE ONLY - numpy restatement of the mesh extraction rules of DESIGN.md section 2 ("Marching cubes"),
-written from the rules, not from the kernel: vertices are generated vectorised, triangles by walking the six faces of
-every surface cell (asymptotic decider on ambiguous faces), chaining the face segments into loops and fanning each loop
-from its smallest vertex index.  A Python loop over surface cells: fine up to ~64^3.
+written from the rules, not from the kernel.  Vertices are generated vectorised.  Triangles follow the per-cell rule: the
+segments of the six faces (asymptotic decider on ambiguous faces) are chained into loops, each fanned from its smallest
+vertex index.  That rule depends only on a cell's 8 inside bits and the decider's result on each of its ambiguous faces
+(6 bits at most), so it is evaluated once per such configuration (`fan_table`, from `loops_for`) and gathered for every
+surface cell at once: a 256^3 volume meshes in seconds.  The per-cell walk (`_faces_by_walk`, a Python loop over surface
+cells, fine up to ~64^3) stays as the written-out definition the table is pinned against.
 
 Only ``tests/`` (and the benchmark's reference arm) may import this module; the product path is ``panic3d_b200.mesh``.
 """
@@ -59,20 +62,50 @@ def saddle(v00, v01, v10, v11):
         return (v00 * v11 - v01 * v10) / (((v00 + v11) - v01) - v10)
 
 
-def cell_loops(cv, level):
-    """Closed loops of local edge ids of one cell with corner values cv[8], each oriented so its right-hand normal points
-    from inside to outside, starting at its smallest edge; loops ordered by that first edge."""
+def inside_bits(cv, level):
+    """Case of cells with corner values cv (..., 8): bit k set when corner k is inside (v > level, fp32)."""
+    cv = np.asarray(cv, dtype=F32)
+    return ((cv > F32(level)).astype(np.int64) << np.arange(8)).sum(-1)
+
+
+def _ambiguous(case):
+    """6-bit mask of the faces of one case with exactly two diagonally opposite inside corners."""
+    m = 0
+    for f, (cyc, _) in enumerate(FACES):
+        ins = [(case >> q) & 1 for q in cyc]
+        m |= (sum(ins) == 2 and ins[0] == ins[2]) << f
+    return m
+
+
+AMBIGUOUS = np.array([_ambiguous(case) for case in range(256)], dtype=np.int64)
+
+
+def face_decisions(cv, level):
+    """Decision bits of cells with corner values cv (..., 8): bit f set when face f is ambiguous and its fp32 saddle value
+    (`saddle`, at the face's canonical corners) exceeds the level, i.e. the inside corners are connected."""
+    cv = np.asarray(cv, dtype=F32)
     level = F32(level)
-    inside = [bool(F32(c) > level) for c in cv]
+    amb = AMBIGUOUS[inside_bits(cv, level)]
+    d = np.zeros(cv.shape[:-1], dtype=np.int64)
+    for f, (_, (c00, c01, c10, c11)) in enumerate(FACES):
+        conn = saddle(cv[..., c00], cv[..., c01], cv[..., c10], cv[..., c11]) > level
+        d |= ((amb >> f) & 1 & conn.astype(np.int64)) << f
+    return d
+
+
+def loops_for(case, decisions):
+    """Closed loops of local edge ids of a cell with inside bits `case` whose ambiguous faces f are connected where bit f
+    of `decisions` is set; each loop oriented so its right-hand normal points from inside to outside, starting at its
+    smallest edge; loops ordered by that first edge."""
     nxt = {}
-    for cyc, (c00, c01, c10, c11) in FACES:
-        ins = [inside[q] for q in cyc]
+    for f, (cyc, _) in enumerate(FACES):
+        ins = [bool((case >> q) & 1) for q in cyc]
         n_in = sum(ins)
         if n_in in (0, 4):
             continue
         fe = [_edge_between(cyc[k], cyc[(k + 1) % 4]) for k in range(4)]     # fe[k] joins cyc[k] and cyc[k+1]
         if n_in == 2 and ins[0] == ins[2]:                                    # two diagonally opposite inside corners
-            connected = bool(saddle(cv[c00], cv[c01], cv[c10], cv[c11]) > level)
+            connected = bool((decisions >> f) & 1)
             for k in range(4):
                 if ins[k] and not connected:          # cut off the inside corner
                     nxt[fe[k - 1]] = fe[k]
@@ -91,11 +124,128 @@ def cell_loops(cv, level):
         seen.add(e)
         cur = nxt[e]
         while cur != e:
+            assert cur not in seen and len(loop) <= 12, (case, decisions)
             loop.append(cur)
             seen.add(cur)
             cur = nxt[cur]
         loops.append(loop)
     return loops
+
+
+def cell_loops(cv, level):
+    """`loops_for` of one cell with corner values cv[8]."""
+    return loops_for(int(inside_bits(cv, level)), int(face_decisions(cv, level)))
+
+
+def configurations():
+    """Every (case, decisions) key: decisions runs over the subsets of the case's ambiguous faces."""
+    out = []
+    for case in range(256):
+        amb = int(AMBIGUOUS[case])
+        sub = amb
+        keys = []
+        while True:                                   # the subsets of amb
+            keys.append(sub)
+            if sub == 0:
+                break
+            sub = (sub - 1) & amb
+        out += [(case, d) for d in sorted(keys)]
+    return out
+
+
+MAX_FAN = 10                                          # fan triangles of one cell: 12 sign-change edges at most, minus 2 per loop
+
+
+def _build_fan_table():
+    tri = np.zeros((256, 64, MAX_FAN, 3), dtype=np.int8)
+    cnt = np.zeros((256, 64), dtype=np.int64)
+    for case, d in configurations():
+        fan = [(lp[0], lp[i], lp[i + 1]) for lp in loops_for(case, d) for i in range(1, len(lp) - 1)]
+        tri[case, d, :len(fan)] = np.reshape(fan, (-1, 3))
+        cnt[case, d] = len(fan)
+    return tri, cnt
+
+
+_FAN = []
+
+
+def fan_table():
+    """(tri (256, 64, MAX_FAN, 3) int8, count (256, 64)): the fan triangles of every configuration as local-edge triples in
+    (loop, fan position) order, from `loops_for`; built on first use."""
+    if not _FAN:
+        _FAN.append(_build_fan_table())
+    return _FAN[0]
+
+
+EDGE_CORNER = np.array([k for k, _ in EDGES], dtype=np.int64)
+EDGE_AXIS = np.array([ax for _, ax in EDGES], dtype=np.int64)
+OFFSETS = np.array(CORNER_OFFSETS, dtype=np.int64)
+
+
+def _case_volume(v, level):
+    inside = v > level
+    D = v.shape
+    cell_in = np.zeros((D[0] - 1, D[1] - 1, D[2] - 1), dtype=np.int64)
+    for k, (dx, dy, dz) in enumerate(CORNER_OFFSETS):
+        cell_in += inside[dx:dx + D[0] - 1, dy:dy + D[1] - 1, dz:dz + D[2] - 1].astype(np.int64) << k
+    return cell_in
+
+
+def surface_cells(v, level=0.5):
+    """Surface cells in flat order: (lower-corner coordinates (n, 3), case (n,), decisions (n,))."""
+    v = np.ascontiguousarray(v, dtype=F32)
+    cell_in = _case_volume(v, F32(level))
+    idx = np.argwhere((cell_in != 0) & (cell_in != 255))
+    a, b, c = idx.T
+    cv = np.stack([v[a + dx, b + dy, c + dz] for dx, dy, dz in CORNER_OFFSETS], -1)
+    return idx, cell_in[a, b, c], face_decisions(cv, level)
+
+
+def fan_triangles(v, level=0.5):
+    """Fan triangles of the volume before degenerate removal (marching_cubes_index keeps those with 3 distinct positions)."""
+    _, case, dec = surface_cells(v, level)
+    return int(fan_table()[1][case, dec].sum())
+
+
+def _faces_by_table(v, level, keys, verts):
+    idx, case, dec = surface_cells(v, level)
+    tri, cnt = fan_table()
+    n = cnt[case, dec]
+    e = tri[case, dec][np.arange(MAX_FAN) < n[:, None]].astype(np.int64)   # (F0, 3) local edges, cells in flat order
+    cell = np.repeat(idx, n, axis=0)[:, None, :]                             # (F0, 1, 3)
+    node = cell + OFFSETS[EDGE_CORNER[e]]                                    # (F0, 3, 3) owner nodes
+    D = v.shape
+    key = ((node[..., 0] * D[1] + node[..., 1]) * D[2] + node[..., 2]) * 3 + EDGE_AXIS[e]
+    gid = np.searchsorted(keys, key)
+    assert np.array_equal(keys[np.minimum(gid, len(keys) - 1)], key)
+    p = verts[gid]
+    same = lambda i, j: (p[:, i] == p[:, j]).all(-1)
+    keep = ~(same(0, 1) | same(1, 2) | same(0, 2))                          # allow_degenerate=False
+    return gid[keep].astype(np.int32).reshape(-1, 3)
+
+
+def _faces_by_walk(v, level, keys, verts):
+    D = v.shape
+    cell_in = _case_volume(v, level)
+    faces = []
+    for a, b, c in np.argwhere((cell_in != 0) & (cell_in != 255)):
+        cv = [v[a + dx, b + dy, c + dz] for dx, dy, dz in CORNER_OFFSETS]
+        gid = []
+        for k, ax in EDGES:
+            dx, dy, dz = CORNER_OFFSETS[k]
+            key = ((int(a) + dx) * D[1] + int(b) + dy) * D[2] + int(c) + dz
+            i = np.searchsorted(keys, key * 3 + ax)
+            gid.append(int(i) if i < len(keys) and keys[i] == key * 3 + ax else -1)
+        for loop in cell_loops(cv, level):
+            g = [gid[e] for e in loop]
+            assert min(g) >= 0
+            for i in range(1, len(g) - 1):
+                tri = (g[0], g[i], g[i + 1])
+                p0, p1, p2 = verts[tri[0]], verts[tri[1]], verts[tri[2]]
+                if np.array_equal(p0, p1) or np.array_equal(p1, p2) or np.array_equal(p0, p2):
+                    continue                                          # allow_degenerate=False
+                faces.append(tri)
+    return np.asarray(faces, dtype=np.int32).reshape(-1, 3)
 
 
 def _gradient(v):
@@ -110,9 +260,10 @@ def _gradient(v):
     return g
 
 
-def marching_cubes_index(v, level=0.5):
+def marching_cubes_index(v, level=0.5, walk=False):
     """v (D0, D1, D2) fp32 -> dict of numpy arrays in index space:
-    verts (V,3) fp32, faces (F,3) int32, normals (V,3) fp32, values (V,) fp32, floor_node (V,) int64."""
+    verts (V,3) fp32, faces (F,3) int32, normals (V,3) fp32, values (V,) fp32, floor_node (V,) int64.
+    walk: triangles by the per-cell walk instead of the table (the same faces, bit for bit and in order; small volumes)."""
     v = np.ascontiguousarray(v, dtype=F32)
     assert v.ndim == 3 and min(v.shape) >= 2
     level = F32(level)
@@ -155,28 +306,7 @@ def marching_cubes_index(v, level=0.5):
     fl = np.floor(verts).astype(np.int64)
     floor_node = (fl[:, 0] * D[1] + fl[:, 1]) * D[2] + fl[:, 2]
     # ---- triangles: surface cells in flat order, loops, fans
-    cell_in = np.zeros((D[0] - 1, D[1] - 1, D[2] - 1), dtype=np.int32)
-    for k, (dx, dy, dz) in enumerate(CORNER_OFFSETS):
-        cell_in += inside[dx:dx + D[0] - 1, dy:dy + D[1] - 1, dz:dz + D[2] - 1].astype(np.int32) << k
-    faces = []
-    for a, b, c in np.argwhere((cell_in != 0) & (cell_in != 255)):
-        cv = [v[a + dx, b + dy, c + dz] for dx, dy, dz in CORNER_OFFSETS]
-        gid = []
-        for k, ax in EDGES:
-            dx, dy, dz = CORNER_OFFSETS[k]
-            key = ((int(a) + dx) * D[1] + int(b) + dy) * D[2] + int(c) + dz
-            i = np.searchsorted(keys, key * 3 + ax)
-            gid.append(int(i) if i < len(keys) and keys[i] == key * 3 + ax else -1)
-        for loop in cell_loops(cv, level):
-            g = [gid[e] for e in loop]
-            assert min(g) >= 0
-            for i in range(1, len(g) - 1):
-                tri = (g[0], g[i], g[i + 1])
-                p0, p1, p2 = verts[tri[0]], verts[tri[1]], verts[tri[2]]
-                if np.array_equal(p0, p1) or np.array_equal(p1, p2) or np.array_equal(p0, p2):
-                    continue                                          # allow_degenerate=False
-                faces.append(tri)
-    faces = np.asarray(faces, dtype=np.int32).reshape(-1, 3)
+    faces = (_faces_by_walk if walk else _faces_by_table)(v, level, keys, verts)
     return dict(verts=verts, faces=faces, normals=normals, values=values, floor_node=floor_node)
 
 

@@ -299,8 +299,9 @@ size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 int check_dims(int64_t d0, int64_t d1, int64_t d2) {
     P3D_REQUIRE(d0 >= 2 && d1 >= 2 && d2 >= 2, "marching cubes needs every volume side >= 2, got (%lld, %lld, %lld)",
                 (long long)d0, (long long)d1, (long long)d2);
-    P3D_REQUIRE(d0 * d1 <= kMaxNodes && d0 * d1 * d2 <= kMaxNodes, "marching cubes supports at most 2^30 nodes, got (%lld, %lld, %lld)",
-                (long long)d0, (long long)d1, (long long)d2);
+    // every factor is bounded before it is multiplied: products of unchecked int64 sides wrap (2 * 2 * (2^62 + 1) == 4)
+    P3D_REQUIRE(d0 <= kMaxNodes && d1 <= kMaxNodes && d2 <= kMaxNodes && d0 * d1 <= kMaxNodes && d0 * d1 * d2 <= kMaxNodes,
+                "marching cubes supports at most 2^30 nodes, got (%lld, %lld, %lld)", (long long)d0, (long long)d1, (long long)d2);
     return P3D_OK;
 }
 

@@ -165,16 +165,16 @@ def decode_points_call(p, planes_cl, wt, coords, rgb, sigma):
         sigma.data_ptr(), _lib.stream_ptr(planes_cl.device)))
 
 
-def twice(call, outs, slot=None, prefill=(), checks_later=False):
-    """call() twice, `outs` and `prefill` refilled before each run (floats with NaN, bytes with 0xFF), so an element the
-    call never writes is NaN.  With `slot`, each run is exactly one launch in that profile slot.  Returns both runs'
+def twice(call, outs, slot=None, prefill=(), checks_later=False, int_fill=0xFF):
+    """call() twice, `outs` and `prefill` refilled before each run (floats with NaN, integers with int_fill), so an
+    element the call never writes is NaN.  With `slot`, each run is exactly one launch in that profile slot.  Returns both runs'
     copies of `outs`; unless checks_later (the caller compares the values first: a kernel that reads memory it never
     wrote may still repeat itself), the second must equal the first bit for bit."""
     runs = []
     for _ in range(2):
         for t in (*outs, *prefill):
             if t is not None:
-                t.fill_(float('nan') if t.is_floating_point() else 0xFF)
+                t.fill_(float('nan') if t.is_floating_point() else int_fill)
         torch.cuda.synchronize()
         _, prof = profiled(call)
         if slot is not None:

@@ -7,8 +7,9 @@ fails it, as it must.  The tree is not modified.
 TARGET is one of decode_tc, paste_front, render_backward, render_backward_multiplane (the TRI lines of
 render_backward.cu), render_taps (the tap enumeration of render_device.cuh, against tests/test_render_backward_paths_gpu.py),
 modconv, modconv_paths (more modconv.cu mutations, against tests/test_modconv_paths_gpu.py), render_fused, multiplane (the
-multiplane section of the header render_device.cuh), render_simt (render_v1.cu, against tests/test_render_simt_paths_gpu.py)
-and render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same file).  Each mutant recompiles every
+multiplane section of the header render_device.cuh), render_simt (render_v1.cu, against tests/test_render_simt_paths_gpu.py),
+render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same file) and marching_cubes
+(marching_cubes.cu, against tests/test_mesh_paths_gpu.py).  Each mutant recompiles every
 translation unit that includes its source, directly or through other headers.  --files runs other GPU files against the
 same mutants instead (to see which of them the rest of the suite catches); the exit code then only reports that the run
 completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
@@ -204,6 +205,26 @@ RENDER_TAPS = {
     'tap bound xi < W - 1': ('(x < g.W)', '(x < g.W - 1)'),
 }
 
+# marching_cubes.cu against tests/test_mesh_paths_gpu.py: every mutant keeps all accesses in bounds (vertex ids only get
+# smaller, faces are written at the scanned slots), keeps the packed counts of the two passes consistent (both run the
+# same cell_build / cell_walk) and leaves every cell's loops closed (they are for any decider outcome:
+# tests/test_mesh_cpu.py checks all 656 configurations), so none can hang.
+MARCHING_CUBES = {
+    # the cell's inside bits count a node at the level as inside; node_edges and vertex_id still do not
+    'cell inside test v >= level': ('ins |= (c.cv[k] > level ? 1u : 0u) << k;', 'ins |= (c.cv[k] >= level ? 1u : 0u) << k;'),
+    'decider tie connects': ('const bool connected = s > level;', 'const bool connected = s >= level;'),
+    'degenerate triangles kept': ('if (!same_pos(c, r, prev, nd) && !same_pos(c, prev, cur, nd) && !same_pos(c, r, cur, nd)) tri(r, prev, cur);',
+                                  'tri(r, prev, cur);'),
+    'vertex id without the +b edge of a +c vertex': ('    if (ax >= 2 && ob + 1 < A.d1) id += (__ldg(A.vol + o + s1) > A.level) != in0;\n', ''),
+    # the two cells of a face read its corners in their own cyclic order, so they can decide differently
+    'decider reads the face cycle': ('const float v00 = c.cv[kFaceCanon[f][0]], v01 = c.cv[kFaceCanon[f][1]];\n'
+                                     '            const float v10 = c.cv[kFaceCanon[f][2]], v11 = c.cv[kFaceCanon[f][3]];',
+                                     'const float v00 = c.cv[kFaceCyc[f][0]], v01 = c.cv[kFaceCyc[f][1]];\n'
+                                     '            const float v10 = c.cv[kFaceCyc[f][2]], v11 = c.cv[kFaceCyc[f][3]];'),
+    'upper-border gradient halved': ('if (i == D - 1) return __fsub_rn(__ldg(vol + n), __ldg(vol + n - stride));',
+                                     'if (i == D - 1) return __fmul_rn(__fsub_rn(__ldg(vol + n), __ldg(vol + n - stride)), 0.5f);'),
+}
+
 # target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
 TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
@@ -217,6 +238,7 @@ TARGETS = {
     'multiplane': ('render_device.cuh', 'tests/test_multiplane_paths_gpu.py', MULTIPLANE),
     'render_simt': ('render_v1.cu', 'tests/test_render_simt_paths_gpu.py', RENDER_SIMT),
     'render_simt_helpers': ('render_device.cuh', 'tests/test_render_simt_paths_gpu.py', RENDER_SIMT_HELPERS),
+    'marching_cubes': ('marching_cubes.cu', 'tests/test_mesh_paths_gpu.py', MARCHING_CUBES),
 }
 
 
