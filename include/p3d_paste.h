@@ -67,6 +67,16 @@ int p3d_paste_front(const p3d_paste_params* p, const float* image, const float* 
 int p3d_paste_front_backward(const p3d_paste_params* p, const float* image_xyz, const float* front_rgb, const float* mask,
                              const float* g_image, const float* g_paste, float* d_image, float* d_xyz, void* stream);
 
+/* Deterministic p3d_paste_front_backward (torch.use_deterministic_algorithms): the same gradients, bit-identical from run to
+   run.  d_image as above.  d_xyz is WRITTEN, not accumulated: each texel gathers, in a fixed order, the contributions the
+   scatter above adds atomically (output pixels row-major, then the pixel's taps (i0,i0), (i0,i1), (i1,i0), (i1,i1); the z
+   channel is zero).  scratch: p3d_paste_front_backward_det_scratch_bytes(p) device bytes (0 and p3d_last_error for bad
+   params), needed when d_xyz is not NULL. */
+size_t p3d_paste_front_backward_det_scratch_bytes(const p3d_paste_params* p);
+int p3d_paste_front_backward_det(const p3d_paste_params* p, const float* image_xyz, const float* front_rgb, const float* mask,
+                                 const float* g_image, const float* g_paste, void* scratch, size_t scratch_bytes,
+                                 float* d_image, float* d_xyz, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

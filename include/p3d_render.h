@@ -160,6 +160,23 @@ int p3d_render_backward(const p3d_render_params* p, const void* planes,
                         void* scratch, size_t scratch_bytes,
                         float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2, void* stream);
 
+/* Deterministic p3d_render_backward (torch.use_deterministic_algorithms): the same gradients, bit-identical from run to run
+   whatever the GPU, grid or timing.  The outputs are WRITTEN, not accumulated (no zero-fill needed).  Instead of float atomics:
+     d_planes  every tap is recorded as (texel, entry = (sample, plane, tap)); the entries are stably radix-sorted by texel and
+               each texel sums its run in entry order, acc = fl(acc + fl(weight * feature gradient)); samples are numbered
+               coarse pass first, then fine, each ray-major
+     d_w1 .. d_b2  each 128-sample CTA writes its partial sums; they are added over CTA index by adjacent pairs, level by level
+   At most 2^31 - 1 entries (views x rays x samples x 3 planes x 4 taps, 8 for multiplane planes) and texels; past that the
+   scratch query returns 0 and the call P3D_EINVAL.  scratch: p3d_render_backward_det_scratch_bytes(p) device bytes. */
+size_t p3d_render_backward_det_scratch_bytes(const p3d_render_params* p);
+int p3d_render_backward_det(const p3d_render_params* p, const void* planes,
+                            const float* w1, const float* b1, const float* w2, const float* b2,
+                            const float* ray_origins, const float* ray_dirs,
+                            const void* fwd_workspace, size_t fwd_workspace_bytes, const float* out_depth,
+                            const float* g_rgb, const float* g_depth, const float* g_wsum, const float* g_xyz,
+                            void* scratch, size_t scratch_bytes,
+                            float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2, void* stream);
+
 /* After a p3d_render_forward with defer_depth_clamp: write this call's (min depth, max depth) as 2 floats to
    device memory `bounds2` (from the call's workspace). */
 int p3d_render_depth_bounds(const void* workspace, float* bounds2, void* stream);
@@ -193,6 +210,16 @@ int p3d_decode_points_backward(const p3d_render_params* p, const void* planes,
                                const float* coords, int64_t n_points_per_view,
                                const float* g_rgb, const float* g_sigma,
                                float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2, void* stream);
+
+/* Deterministic p3d_decode_points_backward: written outputs and fixed summation orders as p3d_render_backward_det, sample
+   index = view * n_points_per_view + point.  scratch: p3d_decode_points_backward_det_scratch_bytes(p, n) device bytes (0 and
+   p3d_last_error past the 2^31 - 1 entry envelope or for a negative count). */
+size_t p3d_decode_points_backward_det_scratch_bytes(const p3d_render_params* p, int64_t n_points_per_view);
+int p3d_decode_points_backward_det(const p3d_render_params* p, const void* planes,
+                                   const float* w1, const float* b1, const float* w2, const float* b2,
+                                   const float* coords, int64_t n_points_per_view,
+                                   const float* g_rgb, const float* g_sigma, void* scratch, size_t scratch_bytes,
+                                   float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2, void* stream);
 
 /* Dense sigma / colour grid for mesh extraction: the renderer-level part of get_eg3d_volume
    (_util/eg3d_metrics3d.py:94-183), which the reference evaluates as 168 host-side chunks of 100k points through

@@ -57,6 +57,11 @@ _PROTOS = {
     'p3d_render_forward_host': (C.c_int, [C.POINTER(RenderParams)] + [_VP] * 7 + [C.c_int32] + [_VP] * 6),
     'p3d_render_backward_scratch_bytes': (C.c_size_t, [C.POINTER(RenderParams)]),
     'p3d_render_backward': (C.c_int, [C.POINTER(RenderParams)] + [_VP] * 7 + [_VP, C.c_size_t] + [_VP] * 5 + [_VP, C.c_size_t] + [_VP] * 6),
+    'p3d_render_backward_det_scratch_bytes': (C.c_size_t, [C.POINTER(RenderParams)]),
+    'p3d_render_backward_det': (C.c_int, [C.POINTER(RenderParams)] + [_VP] * 7 + [_VP, C.c_size_t] + [_VP] * 5 + [_VP, C.c_size_t] + [_VP] * 6),
+    'p3d_decode_points_backward_det_scratch_bytes': (C.c_size_t, [C.POINTER(RenderParams), C.c_int64]),
+    'p3d_decode_points_backward_det': (C.c_int, [C.POINTER(RenderParams)] + [_VP] * 6 + [C.c_int64] + [_VP] * 2 + [_VP, C.c_size_t]
+                                       + [_VP] * 5 + [_VP]),
     'p3d_render_depth_bounds': (C.c_int, [_VP, _VP, _VP]),
     'p3d_depth_finalize': (C.c_int, [_VP, C.c_int64, _VP, _VP]),
     'p3d_host_arena_release': (None, []),

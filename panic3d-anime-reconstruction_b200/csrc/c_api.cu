@@ -455,6 +455,43 @@ int p3d_render_backward(const p3d_render_params* p, const void* planes, const fl
                               scratch, scratch_bytes, d_planes, d_w1, d_b1, d_w2, d_b2, (cudaStream_t)stream);
 }
 
+// an empty batch of the deterministic backward still writes every output: zeros
+static int det_zero(const DetPlan& d, float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2, cudaStream_t st) {
+    P3D_CUDA_TRY(cudaMemsetAsync(d_planes, 0, (size_t)d.texels * kC * sizeof(float), st));
+    P3D_CUDA_TRY(cudaMemsetAsync(d_w1, 0, (size_t)kHidden * kC * sizeof(float), st));
+    P3D_CUDA_TRY(cudaMemsetAsync(d_b1, 0, (size_t)kHidden * sizeof(float), st));
+    P3D_CUDA_TRY(cudaMemsetAsync(d_w2, 0, (size_t)kOut * kHidden * sizeof(float), st));
+    P3D_CUDA_TRY(cudaMemsetAsync(d_b2, 0, (size_t)kOut * sizeof(float), st));
+    return P3D_OK;
+}
+
+size_t p3d_render_backward_det_scratch_bytes(const p3d_render_params* p) {
+    Geom g;
+    DetPlan d;
+    if (make_geom(p, &g) || det_plan(g, -1, &d)) return 0;
+    return det_layout(d, p3d_render_backward_scratch_bytes(p), nullptr, nullptr);
+}
+
+int p3d_render_backward_det(const p3d_render_params* p, const void* planes, const float* w1, const float* b1, const float* w2,
+                            const float* b2, const float* ray_origins, const float* ray_dirs, const void* fwd_workspace,
+                            size_t fwd_workspace_bytes, const float* out_depth, const float* g_rgb, const float* g_depth,
+                            const float* g_wsum, const float* g_xyz, void* scratch, size_t scratch_bytes, float* d_planes,
+                            float* d_w1, float* d_b1, float* d_w2, float* d_b2, void* stream) {
+    Geom g;
+    DetPlan d;
+    int rc = make_geom(p, &g);
+    if (rc || (rc = det_plan(g, -1, &d))) return rc;
+    P3D_REQUIRE(planes && w1 && b1 && w2 && b2 && ray_origins && ray_dirs && fwd_workspace && out_depth, "null input pointer");
+    P3D_REQUIRE(g_rgb && g_depth && g_wsum && g_xyz, "null gradient pointer (pass zeros for unused outputs)");
+    P3D_REQUIRE(scratch && d_planes && d_w1 && d_b1 && d_w2 && d_b2, "null output pointer");
+    if (d.samples == 0) return det_zero(d, d_planes, d_w1, d_b1, d_w2, d_b2, (cudaStream_t)stream);
+    Workspace ws;
+    const size_t need = workspace_layout(p, const_cast<void*>(fwd_workspace), &ws);
+    if (fwd_workspace_bytes < need) { set_error("forward workspace too small: need %zu bytes", need); return P3D_EWORKSPACE; }
+    return render_backward_v1(g, p, planes, w1, b1, w2, b2, ray_origins, ray_dirs, ws, out_depth, g_rgb, g_depth, g_wsum, g_xyz,
+                              scratch, scratch_bytes, d_planes, d_w1, d_b1, d_w2, d_b2, (cudaStream_t)stream, &d);
+}
+
 int p3d_render_depth_bounds(const void* workspace, float* bounds2, void* stream) {
     P3D_REQUIRE(workspace && bounds2, "null pointer");
     return launch_bounds_to_float(reinterpret_cast<const unsigned int*>(workspace), bounds2, (cudaStream_t)stream);   // bounds live at offset 0
@@ -499,6 +536,32 @@ int p3d_decode_points_backward(const p3d_render_params* p, const void* planes, c
     P3D_REQUIRE(d_planes && d_w1 && d_b1 && d_w2 && d_b2, "null output pointer");
     return decode_points_backward_v1(g, p, planes, w1, b1, w2, b2, coords, n_points_per_view, g_rgb, g_sigma, d_planes, d_w1,
                                      d_b1, d_w2, d_b2, (cudaStream_t)stream);
+}
+
+size_t p3d_decode_points_backward_det_scratch_bytes(const p3d_render_params* p, int64_t n_points_per_view) {
+    Geom g;
+    DetPlan d;
+    if (make_geom(p, &g)) return 0;
+    if (n_points_per_view < 0) { set_error("negative point count"); return 0; }
+    if (det_plan(g, n_points_per_view, &d)) return 0;
+    return det_layout(d, 0, nullptr, nullptr);
+}
+
+int p3d_decode_points_backward_det(const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
+                                   const float* w2, const float* b2, const float* coords, int64_t n_points_per_view,
+                                   const float* g_rgb, const float* g_sigma, void* scratch, size_t scratch_bytes, float* d_planes,
+                                   float* d_w1, float* d_b1, float* d_w2, float* d_b2, void* stream) {
+    Geom g;
+    DetPlan d;
+    int rc = make_geom(p, &g);
+    if (rc) return rc;
+    P3D_REQUIRE(n_points_per_view >= 0, "negative point count");
+    if ((rc = det_plan(g, n_points_per_view, &d))) return rc;
+    P3D_REQUIRE(planes && w1 && b1 && w2 && b2 && coords && g_rgb && g_sigma, "null input pointer (pass zeros for an unused gradient)");
+    P3D_REQUIRE(scratch && d_planes && d_w1 && d_b1 && d_w2 && d_b2, "null output pointer");
+    if (d.samples == 0) return det_zero(d, d_planes, d_w1, d_b1, d_w2, d_b2, (cudaStream_t)stream);
+    return decode_points_backward_v1(g, p, planes, w1, b1, w2, b2, coords, n_points_per_view, g_rgb, g_sigma, d_planes, d_w1,
+                                     d_b1, d_w2, d_b2, (cudaStream_t)stream, &d, scratch, scratch_bytes);
 }
 
 int p3d_volume_query(const p3d_render_params* p, const void* planes, const float* w1, const float* b1, const float* w2,

@@ -187,8 +187,11 @@ struct PasteBwdArgs {
     float *d_image, *d_xyz;
     int N, R, S, normalize;
     float inv_bw, half_bw, scale;
+    float* g_v;        // DET: (N,2,S,S) gradients of the up-sampled x and y, gathered into d_xyz by k_paste_dxyz_gather
 };
 
+// DET (torch.use_deterministic_algorithms): record each pixel's gradients of the up-sampled (x, y) instead of scattering them
+template <bool DET>
 __global__ void __launch_bounds__(NT) k_paste_front_bwd(PasteBwdArgs a) {
     const int n = blockIdx.z, ox = blockIdx.x * TW + (threadIdx.x & (TW - 1)), oy = blockIdx.y * TH + threadIdx.x / TW;
     const int R = a.R, S = a.S;
@@ -220,6 +223,11 @@ __global__ void __launch_bounds__(NT) k_paste_front_bwd(PasteBwdArgs a) {
         g_c += gp[c] * ((f01 - f00) * (1.f - tr.f) + (f11 - f10) * tr.f);
     }
     const float g_vy = g_r * tr.gmul, g_vx = g_c * tc.gmul;          // rows follow world y, columns world x
+    if constexpr (DET) {
+        a.g_v[(size_t)n * 2 * plane + pix] = g_vx;
+        a.g_v[((size_t)n * 2 + 1) * plane + pix] = g_vy;
+        return;
+    }
     float* d = a.d_xyz + (size_t)n * 3 * R * R;
     const float w00 = by.l0 * bx.l0, w01 = by.l0 * bx.l1, w10 = by.l1 * bx.l0, w11 = by.l1 * bx.l1;
     if (g_vx != 0.f) {
@@ -231,6 +239,55 @@ __global__ void __launch_bounds__(NT) k_paste_front_bwd(PasteBwdArgs a) {
         atomicAdd(d + by.i0 * R + bx.i0, g_vy * w00); atomicAdd(d + by.i0 * R + bx.i1, g_vy * w01);
         atomicAdd(d + by.i1 * R + bx.i0, g_vy * w10); atomicAdd(d + by.i1 * R + bx.i1, g_vy * w11);
     }
+}
+
+// first output coordinate in [0, size) whose up-sampling source (i1 if HI, else i0) is >= src; both are monotone in it
+template <bool HI>
+__device__ __forceinline__ int first_dst(int src, float scale, int in, int size) {
+    int lo = 0, hi = size;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        const Lin l = lin_src(mid, scale, in);
+        if ((int)(HI ? l.i1 : l.i0) < src) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// Deterministic d_xyz: texel (row, col) of view n sums, in a fixed order, every contribution the scatter would add to it -
+// output pixels (oy, ox) ascending row-major over the static stencil whose bilinear footprint covers the texel, and per pixel
+// its taps (i0,i0), (i0,i1), (i1,i0), (i1,i1) that land here: acc = fl(acc + fl(g * fl(ly * lx))), zero gradients skipped
+// as the scatter skips them.  The z channel gets no gradient and is written as zero.
+__global__ void __launch_bounds__(256) k_paste_dxyz_gather(const float* __restrict__ g_v, float* __restrict__ d_xyz, int R, int S,
+                                                           float scale) {
+    const int n = blockIdx.y, t = blockIdx.x * 256 + threadIdx.x;
+    if (t >= R * R) return;
+    const int row = t / R, col = t - row * R;
+    const int y0 = first_dst<true>(row, scale, R, S), y1 = first_dst<false>(row + 1, scale, R, S);
+    const int x0 = first_dst<true>(col, scale, R, S), x1 = first_dst<false>(col + 1, scale, R, S);
+    const size_t plane = (size_t)S * S;
+    const float* gx = g_v + (size_t)n * 2 * plane;
+    const float* gy = gx + plane;
+    float ax = 0.f, ay = 0.f;
+    for (int oy = y0; oy < y1; ++oy) {
+        const Lin by = lin_src(oy, scale, R);
+        for (int ox = x0; ox < x1; ++ox) {
+            const Lin bx = lin_src(ox, scale, R);
+            const float vx = __ldg(gx + (size_t)oy * S + ox), vy = __ldg(gy + (size_t)oy * S + ox);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const unsigned ry = (k >> 1) ? by.i1 : by.i0, cx = (k & 1) ? bx.i1 : bx.i0;
+                if (ry != (unsigned)row || cx != (unsigned)col) continue;
+                const float w = __fmul_rn((k >> 1) ? by.l1 : by.l0, (k & 1) ? bx.l1 : bx.l0);
+                if (vx != 0.f) ax = __fadd_rn(ax, __fmul_rn(vx, w));
+                if (vy != 0.f) ay = __fadd_rn(ay, __fmul_rn(vy, w));
+            }
+        }
+    }
+    float* d = d_xyz + (size_t)n * 3 * R * R + t;
+    d[0] = ax;
+    d[(size_t)R * R] = ay;
+    d[(size_t)2 * R * R] = 0.f;
 }
 
 // ---------------------------------------------------------------- small kernels
@@ -335,7 +392,40 @@ extern "C" int p3d_paste_front_backward(const p3d_paste_params* p, const float* 
     a.inv_bw = 1.f / (float)p->box_warp; a.half_bw = (float)(p->box_warp / 2);
     a.scale = (float)p->res_render / (float)p->res_image;
     dim3 grd((a.S + TW - 1) / TW, (a.S + TH - 1) / TH, a.N);
-    k_paste_front_bwd<<<grd, NT, 0, (cudaStream_t)stream>>>(a);
+    k_paste_front_bwd<false><<<grd, NT, 0, (cudaStream_t)stream>>>(a);
     P3D_LAUNCH_CHECK();
+    return P3D_OK;
+}
+
+extern "C" size_t p3d_paste_front_backward_det_scratch_bytes(const p3d_paste_params* p) {
+    if (check_params(p)) return 0;
+    return (size_t)2 * p->n_views * p->res_image * p->res_image * sizeof(float);
+}
+
+extern "C" int p3d_paste_front_backward_det(const p3d_paste_params* p, const float* image_xyz, const float* front_rgb, const float* mask,
+                                            const float* g_image, const float* g_paste, void* scratch, size_t scratch_bytes,
+                                            float* d_image, float* d_xyz, void* stream) {
+    if (int rc = check_params(p)) return rc;
+    P3D_REQUIRE(image_xyz && front_rgb && mask && g_image && d_image, "p3d_paste_front_backward_det: NULL pointer");
+    const size_t need = p3d_paste_front_backward_det_scratch_bytes(p);
+    if (d_xyz && (!scratch || scratch_bytes < need)) {
+        set_error("p3d_paste_front_backward_det: scratch too small: need %zu bytes, got %zu", need, scratch_bytes);
+        return P3D_EWORKSPACE;
+    }
+    PasteBwdArgs a;
+    a.xyz = image_xyz; a.front = front_rgb; a.mask = mask; a.g_image = g_image; a.g_paste = g_paste;
+    a.d_image = d_image; a.d_xyz = d_xyz; a.g_v = reinterpret_cast<float*>(scratch);
+    a.N = p->n_views; a.R = p->res_render; a.S = p->res_image; a.normalize = p->normalize_images;
+    a.inv_bw = 1.f / (float)p->box_warp; a.half_bw = (float)(p->box_warp / 2);
+    a.scale = (float)p->res_render / (float)p->res_image;
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfileScope prof(PROF_OTHER, st);
+    dim3 grd((a.S + TW - 1) / TW, (a.S + TH - 1) / TH, a.N);
+    k_paste_front_bwd<true><<<grd, NT, 0, st>>>(a);
+    P3D_LAUNCH_CHECK();
+    if (d_xyz) {
+        k_paste_dxyz_gather<<<dim3((unsigned)((a.R * a.R + 255) / 256), (unsigned)a.N), 256, 0, st>>>(a.g_v, d_xyz, a.R, a.S, a.scale);
+        P3D_LAUNCH_CHECK();
+    }
     return P3D_OK;
 }

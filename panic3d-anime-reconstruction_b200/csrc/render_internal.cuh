@@ -53,6 +53,24 @@ struct VolumeSpec {
     int crop_on, cull_on;
 };
 
+// Sizes of a deterministic backward (render_backward.cu, DESIGN.md section 4.3): samples of the call, NT = 3 planes x taps
+// entries per sample, CTAs of the sample kernel, texels of the gradient, radix-sort key bits and CUB's temporary bytes.
+struct DetPlan {
+    long long samples, entries, ctas, texels, texels_view;
+    int nt, key_bits;
+    size_t sort_bytes;
+};
+// its scratch: sample feature gradients, entry weights, keys and ids (two buffers each for the sort), CTA partials, the
+// pairwise levels over them and the sort's temporaries
+struct DetBufs {
+    float *dx, *w, *part, *part2;
+    unsigned *key0, *key1, *id0, *id1;
+    void* sort_tmp;
+};
+// n_pts < 0: a render of g's rays, else a point query of n_pts points per view.  P3D_EINVAL past the 2^31 - 1 entry / texel envelope
+int det_plan(const Geom& g, long long n_pts, DetPlan* d);
+size_t det_layout(const DetPlan& d, size_t head, void* base, DetBufs* b);
+
 int make_geom(const p3d_render_params* p, Geom* g);
 size_t workspace_layout(const p3d_render_params* p, void* base, Workspace* ws);
 
@@ -65,7 +83,7 @@ int render_backward_v1(const Geom& g, const p3d_render_params* p, const void* pl
                        const float* w2, const float* b2, const float* ro, const float* rd, const Workspace& ws,
                        const float* out_depth, const float* g_rgb, const float* g_depth, const float* g_wsum,
                        const float* g_xyz, void* scratch, size_t scratch_bytes, float* d_planes, float* d_w1, float* d_b1,
-                       float* d_w2, float* d_b2, cudaStream_t stream);
+                       float* d_w2, float* d_b2, cudaStream_t stream, const DetPlan* det = nullptr);
 // small launches of render_v1.cu shared by both renderers
 int launch_bounds_init(unsigned int* bounds, cudaStream_t stream);
 int launch_ray_limits(const float* ro, const float* rd, long long R, float h, float* t0, float* t1, unsigned int* bounds,
@@ -93,7 +111,7 @@ int volume_query_tc(const Geom& g, const p3d_render_params* p, const void* plane
 int decode_points_backward_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
                               const float* w2, const float* b2, const float* coords, long long n_pts, const float* g_rgb,
                               const float* g_sigma, float* d_planes, float* d_w1, float* d_b1, float* d_w2, float* d_b2,
-                              cudaStream_t stream);
+                              cudaStream_t stream, const DetPlan* det = nullptr, void* scratch = nullptr, size_t scratch_bytes = 0);
 int volume_query_v1(const Geom& g, const p3d_render_params* p, const void* planes, const float* w1, const float* b1,
                     const float* w2, const float* b2, const VolumeSpec& vol, float* out_sigma, float* out_rgb,
                     float* out_density, float* out_coords, cudaStream_t stream);

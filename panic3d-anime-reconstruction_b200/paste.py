@@ -44,6 +44,8 @@ _lib.register_protos({
     'p3d_paste_erode': (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, _VP, _VP]),
     'p3d_paste_front': (C.c_int, [C.POINTER(PasteParams)] + [_VP] * 8 + [_VP] * 4 + [_VP]),
     'p3d_paste_front_backward': (C.c_int, [C.POINTER(PasteParams)] + [_VP] * 7 + [_VP]),
+    'p3d_paste_front_backward_det_scratch_bytes': (C.c_size_t, [C.POINTER(PasteParams)]),
+    'p3d_paste_front_backward_det': (C.c_int, [C.POINTER(PasteParams)] + [_VP] * 5 + [_VP, C.c_size_t] + [_VP] * 2 + [_VP]),
 })
 
 
@@ -138,7 +140,8 @@ def erode_front_weights(frontw, e, thresh=0.5):
 
 # ---------------------------------------------------------------- the fused op
 class _PasteFunction(torch.autograd.Function):
-    """(image, image_xyz) -> (image_out, paste, mask, parts): p3d_paste_front / p3d_paste_front_backward."""
+    """(image, image_xyz) -> (image_out, paste, mask, parts): p3d_paste_front / p3d_paste_front_backward, or
+    p3d_paste_front_backward_det under ``torch.use_deterministic_algorithms(True)``."""
 
     @staticmethod
     def forward(ctx, image, image_xyz, consts, p, grad_sample, want_parts):
@@ -172,9 +175,19 @@ class _PasteFunction(torch.autograd.Function):
         want_xyz = ctx.grad_sample and ctx.needs_input_grad[1]
         g_paste = None if (g_paste is None or not ctx.grad_sample) else g_paste.float().contiguous()
         d_img = torch.empty_like(g_img)
+        L = _lib.lib()
+        if torch.are_deterministic_algorithms_enabled():
+            d_xyz = torch.empty(ctx.xyz_shape, device=dev, dtype=torch.float32) if want_xyz else None
+            scratch = torch.empty(int(L.p3d_paste_front_backward_det_scratch_bytes(C.byref(ctx.p))) if want_xyz else 0,
+                                  dtype=torch.uint8, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(L.p3d_paste_front_backward_det(C.byref(ctx.p), xyz.data_ptr(), front.data_ptr(), mask.data_ptr(),
+                                                          g_img.data_ptr(), _lib.ptr(g_paste), _lib.ptr(scratch if want_xyz else None),
+                                                          scratch.numel(), d_img.data_ptr(), _lib.ptr(d_xyz), _lib.stream_ptr(dev)))
+            return d_img, d_xyz, None, None, None, None
         d_xyz = torch.zeros(ctx.xyz_shape, device=dev, dtype=torch.float32) if want_xyz else None
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().p3d_paste_front_backward(C.byref(ctx.p), xyz.data_ptr(), front.data_ptr(), mask.data_ptr(),
+            _lib.check(L.p3d_paste_front_backward(C.byref(ctx.p), xyz.data_ptr(), front.data_ptr(), mask.data_ptr(),
                                                           g_img.data_ptr(), _lib.ptr(g_paste), d_img.data_ptr(), _lib.ptr(d_xyz),
                                                           _lib.stream_ptr(dev)))
         return d_img, d_xyz, None, None, None, None

@@ -164,11 +164,17 @@ class _RenderFunction(torch.autograd.Function):
         N, M = p.n_views, p.n_rays
         z = lambda g_, sh: (torch.zeros(sh, device=dev, dtype=torch.float32) if g_ is None else g_.float().contiguous())
         g_rgb, g_depth, g_wsum, g_xyz = z(g_rgb, (N, M, p.out_dim - 1)), z(g_depth, (N, M, 1)), z(g_wsum, (N, M, 1)), z(g_xyz, (N, M, 3))
-        d_planes = torch.zeros_like(planes_cl)
-        d_w = [torch.zeros_like(t) for t in (w1, b1, w2, b2)]
-        scratch = torch.empty(int(L.p3d_render_backward_scratch_bytes(C.byref(p))), dtype=torch.uint8, device=dev)
+        # torch.use_deterministic_algorithms(True): fixed-order reductions that write every output, instead of float atomics
+        det = torch.are_deterministic_algorithms_enabled()
+        new = torch.empty_like if det else torch.zeros_like
+        d_planes = new(planes_cl)
+        d_w = [new(t) for t in (w1, b1, w2, b2)]
+        nbytes = L.p3d_render_backward_det_scratch_bytes(C.byref(p)) if det else L.p3d_render_backward_scratch_bytes(C.byref(p))
+        if not nbytes:
+            _lib.check(-1)
+        scratch = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(L.p3d_render_backward(C.byref(p), planes_cl.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(),
+            _lib.check((L.p3d_render_backward_det if det else L.p3d_render_backward)(C.byref(p), planes_cl.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(),
                                              ro.data_ptr(), rd.data_ptr(), ws.data_ptr(), ws.numel(), depth.data_ptr(),
                                              g_rgb.data_ptr(), g_depth.data_ptr(), g_wsum.data_ptr(), g_xyz.data_ptr(),
                                              scratch.data_ptr(), scratch.numel(), d_planes.data_ptr(), *[t.data_ptr() for t in d_w],
@@ -209,12 +215,25 @@ class _PointsFunction(torch.autograd.Function):
         N, K = coords.shape[0], coords.shape[1]
         g_rgb = torch.zeros((N, K, p.out_dim - 1), device=dev) if g_rgb is None else g_rgb.float().contiguous()
         g_sigma = torch.zeros((N, K, 1), device=dev) if g_sigma is None else g_sigma.float().contiguous()
-        d_planes = torch.zeros_like(planes_cl)
-        d_w = [torch.zeros_like(t) for t in (w1, b1, w2, b2)]
-        with torch.cuda.device(dev):
-            _lib.check(L.p3d_decode_points_backward(C.byref(p), planes_cl.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
-                                                    b2.data_ptr(), coords.data_ptr(), K, g_rgb.data_ptr(), g_sigma.data_ptr(),
-                                                    d_planes.data_ptr(), *[t.data_ptr() for t in d_w], _lib.stream_ptr(dev)))
+        if torch.are_deterministic_algorithms_enabled():
+            d_planes = torch.empty_like(planes_cl)
+            d_w = [torch.empty_like(t) for t in (w1, b1, w2, b2)]
+            nbytes = L.p3d_decode_points_backward_det_scratch_bytes(C.byref(p), K)
+            if not nbytes:
+                _lib.check(-1)
+            scratch = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(L.p3d_decode_points_backward_det(C.byref(p), planes_cl.data_ptr(), w1.data_ptr(), b1.data_ptr(),
+                                                            w2.data_ptr(), b2.data_ptr(), coords.data_ptr(), K, g_rgb.data_ptr(),
+                                                            g_sigma.data_ptr(), scratch.data_ptr(), scratch.numel(),
+                                                            d_planes.data_ptr(), *[t.data_ptr() for t in d_w], _lib.stream_ptr(dev)))
+        else:
+            d_planes = torch.zeros_like(planes_cl)
+            d_w = [torch.zeros_like(t) for t in (w1, b1, w2, b2)]
+            with torch.cuda.device(dev):
+                _lib.check(L.p3d_decode_points_backward(C.byref(p), planes_cl.data_ptr(), w1.data_ptr(), b1.data_ptr(), w2.data_ptr(),
+                                                        b2.data_ptr(), coords.data_ptr(), K, g_rgb.data_ptr(), g_sigma.data_ptr(),
+                                                        d_planes.data_ptr(), *[t.data_ptr() for t in d_w], _lib.stream_ptr(dev)))
         dts = ctx.in_dtypes
         return (_planes_grad(d_planes, dts[0]), d_w[0].to(dts[1]), d_w[1].to(dts[2]), d_w[2].to(dts[3]), d_w[3].to(dts[4]),
                 None, None)
