@@ -8,8 +8,9 @@ TARGET is one of decode_tc, paste_front, render_backward, render_backward_multip
 render_backward.cu), render_taps (the tap enumeration of render_device.cuh, against tests/test_render_backward_paths_gpu.py),
 modconv, modconv_paths (more modconv.cu mutations, against tests/test_modconv_paths_gpu.py), render_fused, multiplane (the
 multiplane section of the header render_device.cuh), render_simt (render_v1.cu, against tests/test_render_simt_paths_gpu.py),
-render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same file) and marching_cubes
-(marching_cubes.cu, against tests/test_mesh_paths_gpu.py).  Each mutant recompiles every
+render_simt_helpers (the SIMT-only helpers of render_device.cuh, against the same file), marching_cubes
+(marching_cubes.cu, against tests/test_mesh_paths_gpu.py), and bias_act, upfirdn2d and filtered_lrelu (ops_bias_act.cu,
+ops_upfirdn2d.cu and ops_filtered_lrelu.cu, against tests/test_ops_paths_gpu.py).  Each mutant recompiles every
 translation unit that includes its source, directly or through other headers.  --files runs other GPU files against the
 same mutants instead (to see which of them the rest of the suite catches); the exit code then only reports that the run
 completed.  --build-only builds every mutant and stops; nvcc cross-compiles, so it needs no GPU.
@@ -225,6 +226,89 @@ MARCHING_CUBES = {
                                      'if (i == D - 1) return __fmul_rn(__fsub_rn(__ldg(vol + n), __ldg(vol + n - stride)), 0.5f);'),
 }
 
+# ops_bias_act.cu against tests/test_ops_paths_gpu.py: value mutations only.  Every bias index these mutants produce is taken
+# modulo size_b (the shifted BIAS == 2 run stays a whole aligned vector because size_b and ge are multiples of VEC there), and
+# no launch shape, UNROLL or vector count changes, so every access stays in bounds.
+BIAS_ACT = {
+    # gradient modes gate by the sign of the incoming gradient instead of the stored output
+    'lrelu gradient gate reads x': (': ((yy > 0) ? x : x * alpha); }', ': ((x > 0) ? x : x * alpha); }'),
+    'gradient clamp gate tests y, not yref': ('else y = (yref > -clamp && yref < clamp) ? y : (S)0;',
+                                              'else y = (y > -clamp && y < clamp) ? y : (S)0;'),
+    # equal to the kernel when gain == 1 (tanh's default) and for lrelu's sign gate at any positive gain
+    'yy without the division by gain': ('S yy = (gain != (S)0) ? yref / gain : (S)0;', 'S yy = yref;'),
+    'row-mode bias from row r + 1': ('if (BIAS == 4) brow = Elem<T>::ld(bp[r % size_b]);',
+                                     'if (BIAS == 4) brow = Elem<T>::ld(bp[(r + 1) % size_b]);'),
+    'per-vector bias from the next row': ('if (BIAS == 1) bshared = Elem<T>::ld(bp[(ge / step_b) % size_b]);',
+                                          'if (BIAS == 1) bshared = Elem<T>::ld(bp[(ge / step_b + 1) % size_b]);'),
+    'bias run shifted by one vector': ('if (BIAS == 2) bv = *reinterpret_cast<const V*>(bp + ge % size_b);',
+                                       'if (BIAS == 2) bv = *reinterpret_cast<const V*>(bp + (ge + VEC) % size_b);'),
+    # a vector that straddles two rows (step_b % VEC != 0) takes the first row's bias for all its elements
+    'generic strided index without + k': ('((ge + k) / step_b) % size_b', '(ge / step_b) % size_b'),
+    # the channel of a channels-last element counted in vectors instead of elements; equal to the kernel when VEC % C == 1
+    # (fp32 on RGB)
+    'generic channel run from the vector index': ('if (BIAS == 3) bi0 = (step_b == 1) ? ge % size_b : 0;',
+                                                  'if (BIAS == 3) bi0 = (step_b == 1) ? vi % size_b : 0;'),
+    # the tail's elements take the biases of the tensor's first elements; equal to the kernel for an unaligned caller
+    # (main_n == 0) and when numel % VEC == 0 (no tail)
+    'scalar tail launched with base 0': ('q.base = main_n;', 'q.base = 0;'),
+}
+
+# ops_upfirdn2d.cu against tests/test_ops_paths_gpu.py: value mutations only.  The fast kernel's shared rows are PITCH >= IN_W
+# + VEC - 1 wide, so reading them without the shift a_r stays inside the row; the narrowed border test only zero-fills more
+# elements of a straddling vector; the edge-clamped tiled load and the wrapped channel group index inside the image and C (a
+# whole aligned group, C % VEC == 0).  No cp.async source, group count or wait, tile size, shared-memory size or launch shape
+# changes.
+UPF_TILED_W = 's_w[i] = p.f[sy * p.fsh + sx * p.fsw] * p.gain;\n    }\n    const int tile'
+UPF_TILED_FLIP = 'const int sy = p.flip ? ky : p.fH - 1 - ky, sx = p.flip ? kx : p.fW - 1 - kx;\n        ' + UPF_TILED_W
+UPFIRDN2D = {
+    'fast: row flip sense swapped': ('const int sy = p.flip ? ky : F - 1 - ky;', 'const int sy = p.flip ? F - 1 - ky : ky;'),
+    # equal to the kernel on rows whose base is 16-byte aligned
+    'fast: shared row read without its shift a_r': ('const T* rowp = sb + (by + sr) * PITCH + s_a[b * IN_H + by + sr];',
+                                                    'const T* rowp = sb + (by + sr) * PITCH;'),
+    # the last image column is zero-filled where it falls inside a border-straddling vector
+    'fast: straddling vector drops the last column': ('tmp[j] = (ix + j >= 0 && ix + j < p.inW) ? src[j]',
+                                                      'tmp[j] = (ix + j >= 0 && ix + j < p.inW - 1) ? src[j]'),
+    # equal to the kernel at gain 1
+    'fast: odd-column taps without the gain': ('p.f[sy * p.fsh + sxo * p.fsw] * p.gain);', 'p.f[sy * p.fsh + sxo * p.fsw]);'),
+    'tiled: gain folded in twice': (UPF_TILED_W, UPF_TILED_W.replace('* p.gain;', '* p.gain * p.gain;')),
+    # equal to the kernel when flip is 0 or the filter is point-symmetric
+    'tiled: flip ignored': (UPF_TILED_FLIP, UPF_TILED_FLIP.replace('p.flip ? ky : ', '').replace('p.flip ? kx : ', '')),
+    # pixels outside the image read the nearest edge sample instead of zero
+    'tiled: edge sample instead of zero fill': (
+        'if (iy >= 0 && iy < p.inH && ix >= 0 && ix < p.inW) v = Px<T>::ld(xi[iy * p.xs[2] + ix * p.xs[3]]);',
+        'v = Px<T>::ld(xi[min(max(iy, 0), p.inH - 1) * p.xs[2] + min(max(ix, 0), p.inW - 1) * p.xs[3]]);'),
+    # every output column starts at tap 0; the input column (ux0 + kx) / up is still checked against [0, inW); equal to the
+    # kernel at up 1
+    'strided: column phase kx0 = 0': ('const int kx0 = pos_mod(-ux0, p.upx), ky0 = pos_mod(-uy0, p.upy);\n        const T* xi = xp + n * p.xs[0] + c * p.xs[1];',
+                                      'const int kx0 = 0, ky0 = pos_mod(-uy0, p.upy);\n        const T* xi = xp + n * p.xs[0] + c * p.xs[1];'),
+    # each thread reads channel group g + 1 (mod C / VEC) and writes group g; equal to the kernel when C == VEC
+    'channels-last: reads the next channel group': ('const T* xi = xp + n * p.xs[0] + c;', 'const T* xi = xp + n * p.xs[0] + (c + VEC) % p.C;'),
+}
+
+# ops_filtered_lrelu.cu against tests/test_ops_paths_gpu.py: value mutations only.  The sign tensor is allocated with
+# torch.zeros, so a byte no CTA writes reads back as code 0 every run; the shifted code position stays inside its byte and the
+# offset-free sign coordinate inside the qx < sW / qy < sH check.  No tile size, shared-memory size or loop bound changes.
+FILTERED_LRELU = {
+    'negative code written as 0': ('if (acc < 0.f) { acc *= p.slope; sc = 1; }', 'if (acc < 0.f) { acc *= p.slope; sc = 0; }'),
+    # equal to the kernel where the backward's sx = px0 - (fuW - 1) is 0
+    'sign x offset ignored': ('const int qx = ux + p.sx, qy = uy + p.sy;', 'const int qx = ux, qy = uy + p.sy;'),
+    'code position from qx + 1': ('>> ((qx & 3) << 1)) & 3u;', '>> (((qx + 1) & 3) << 1)) & 3u;'),
+    'clamped pixels scaled by the slope in the gradient pass': ('if (sc & 2u) acc = 0.f;', 'if (sc & 2u) acc *= p.slope;'),
+    # the separable vertical up-pass multiplies by up^2 * gain a second time
+    'separable vertical up-pass with the gain taps': ('acc = fmaf(col[j * p.upTW], s_wu[p.fuW + ky], acc);',
+                                                      'acc = fmaf(col[j * p.upTW], s_wu[ky], acc);'),
+    # equal to the kernel at up 1
+    'ugain without up * up': ('const float ugain = (float)p.up * (float)p.up * p.gain;', 'const float ugain = p.gain;'),
+    # the bottom row of tiles stops writing sign bytes at its nominal height: the rows of the down-filter's halo below it
+    # keep code 0
+    'last tile row owns only its own rows': ('const int own_y1 = (tyi == p.tilesY - 1) ? p.sH : uy0 + kOutH * p.down;',
+                                             'const int own_y1 = uy0 + kOutH * p.down;'),
+    # a full (non-separable) filter read with its rows in the flipped order; equal to the kernel on row-symmetric filters
+    'full filter rows flip sense swapped': ('const int yy = flip ? ky : fh - 1 - ky,', 'const int yy = flip ? fh - 1 - ky : ky,'),
+    # the separable down filter is never flipped; equal to the kernel when flip is set or the taps are symmetric
+    'separable down taps never flipped': ('s_wd[i] = p.fd[p.flip ? i : p.fdW - 1 - i];', 's_wd[i] = p.fd[i];'),
+}
+
 # target -> (source under csrc/, the GPU test file that must kill every mutant, mutations {name: (old, new)})
 TARGETS = {
     'decode_tc': ('decode_tc.cu', 'tests/test_decode_tc_depth_gpu.py', DECODE_TC),
@@ -239,6 +323,9 @@ TARGETS = {
     'render_simt': ('render_v1.cu', 'tests/test_render_simt_paths_gpu.py', RENDER_SIMT),
     'render_simt_helpers': ('render_device.cuh', 'tests/test_render_simt_paths_gpu.py', RENDER_SIMT_HELPERS),
     'marching_cubes': ('marching_cubes.cu', 'tests/test_mesh_paths_gpu.py', MARCHING_CUBES),
+    'bias_act': ('ops_bias_act.cu', 'tests/test_ops_paths_gpu.py', BIAS_ACT),
+    'upfirdn2d': ('ops_upfirdn2d.cu', 'tests/test_ops_paths_gpu.py', UPFIRDN2D),
+    'filtered_lrelu': ('ops_filtered_lrelu.cu', 'tests/test_ops_paths_gpu.py', FILTERED_LRELU),
 }
 
 

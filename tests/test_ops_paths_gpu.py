@@ -2,7 +2,10 @@
 
 tests/test_ops_gpu.py runs every op at fixture sizes, which are too small to reach the kernels training actually runs:
 row-mode bias_act, the persistent cp.async upfirdn2d kernel walking several tiles per CTA, the channels-last kernel's
-grid-stride loop, the image laps past gridDim.y = 32768, and filtered_lrelu's sign bytes on tile seams.  Each test
+grid-stride loop, the image laps past gridDim.y = 32768, and filtered_lrelu's sign bytes on tile seams; nor, at the sizes
+generator layers run, bias_act's per-vector, generic and scalar-tail launches or upfirdn2d's tiled and strided kernels
+with flip, gain and up-sampled phases.  tests/run_mutations.py's bias_act, upfirdn2d and filtered_lrelu mutants must
+each fail this file.  Each test
 below restates the dispatch rule its shape relies on (with the source lines) and asserts the property that matters.
 
 Reference: ``oracle/ops_oracle.py`` in float64 on the inputs already rounded to the storage dtype, with the scalars
@@ -152,15 +155,14 @@ def ba_inputs(shape, dim, dtype, act, kw, seed, fmt=torch.contiguous_format):
 
 
 def ba_near_kink(x, b, dim, act, kw):
-    """Distance of each element from the nearest gate discontinuity minus the required margin (>= 0 is safe)."""
-    if act != 'lrelu':
-        return torch.ones_like(x, dtype=F64)
+    """Distance of each element from the nearest gate discontinuity (the lrelu kink, the clamp of any activation) minus
+    the required margin (>= 0 is safe)."""
     k = f32_scalars(kw, act)
     s = x.double() + b.double().reshape(_bshape(x.ndim, dim))
-    d = s.abs() - 1e-3
+    d = s.abs() - 1e-3 if act == 'lrelu' else torch.ones_like(s)
     if k.get('clamp') is not None:
         c = k['clamp']
-        y = torch.where(s > 0, s, s * k['alpha']) * k['gain']
+        y = oo.bias_act(s, act=act, alpha=k['alpha'], gain=k['gain'])
         d = torch.minimum(d, (y.abs() - c).abs() - max(1e-3, ulp(torch.tensor(c, dtype=F64), x.dtype).item()))
     return d
 
@@ -227,6 +229,37 @@ def test_bias_act_channels_last_at_size(dtype):
     ba_compare(f'bias_act channels_last {dtype}', y, x, b, 1, 'lrelu', kw)
 
 
+BA_MODES = {
+    # generator layers at 8x8: 16 (fp32) / 8 (16-bit) vectors per (n, c) row, too few for row mode (BIAS == 1)
+    'per_vector': ((64, 512, 8, 8), torch.contiguous_format, 'per_vector'),
+    # NCHW with an odd H*W: vectors straddle two rows, each element finds its own row ((ge + k) / step_b, BIAS == 3)
+    'generic_strided': ((4, 64, 97, 101), torch.contiguous_format, 'generic'),
+    # channels_last RGB (C = 3, not a multiple of VEC): each element's channel counted from its element index (BIAS == 3)
+    'generic_run': ((16, 3, 256, 256), torch.channels_last, 'generic'),
+    # an aligned tensor with numel % VEC != 0: its last numel % VEC elements go through the scalar tail launch, whose
+    # bias index starts at base = main_n (ops_bias_act.cu:198-210)
+    'tail': ((5, 37, 41, 43), torch.contiguous_format, 'tail'),
+}
+
+
+@pytest.mark.parametrize('dtype', DT_ALL, ids=DT_IDS)
+@pytest.mark.parametrize('mode', list(BA_MODES))
+def test_bias_act_other_modes_at_size(mode, dtype):
+    """The per-vector, generic and scalar-tail bias indexing at generator sizes, lrelu with the generator's clamp 256
+    (which never bites, so a wrong bias shows in every element it reaches, the tail's last one included)."""
+    shape, fmt, want = BA_MODES[mode]
+    kw = dict(clamp=256.0)
+    x, b = ba_inputs(shape, 1, dtype, 'lrelu', kw, seed=105, fmt=fmt)
+    if want == 'tail':
+        assert x.numel() % (16 // x.element_size()) != 0 and x.data_ptr() % 16 == 0
+    else:
+        d = ba_dispatch(x, 1, 0)
+        assert d['mode'] == want, d
+    y = _ba().bias_act(x, b, dim=1, act='lrelu', **kw)
+    assert y.stride() == x.stride()
+    ba_compare(f'bias_act {mode} {dtype}', y, x, b, 1, 'lrelu', kw)
+
+
 def ba_grad_ref(g, y, kw, act, order, dy=None):
     """The kernel's derivative formulas (ops_bias_act.cu:46-50, 82-85) in float64, gated on the op's own stored y.
     order 1: g * act'(s) * gain, zero where |y| >= clamp; order 2 (tanh): g * act''(s) * gain * dy."""
@@ -246,17 +279,23 @@ def ba_grad_ref(g, y, kw, act, order, dy=None):
 
 
 GRAD_N = {2: 6, 4: 3, 8: 2}
+BA_GRAD = {'lrelu': ('lrelu', dict(clamp=1.0)), 'tanh': ('tanh', {}),
+           # the derivative's yy = yref / gain (ops_bias_act.cu:42) at a gain != 1, and the gradient clamp gate on yref
+           # (:85) in both orders: 2 |tanh(s)| >= 1 on about 40 % of the elements
+           'tanh_gain2_clamp1': ('tanh', dict(gain=2.0, clamp=1.0))}
 
 
 @pytest.mark.parametrize('dtype', DT_ALL, ids=DT_IDS)
-@pytest.mark.parametrize('act', ['lrelu', 'tanh'])
-def test_bias_act_row_mode_gradients(act, dtype):
+@pytest.mark.parametrize('variant', list(BA_GRAD))
+def test_bias_act_row_mode_gradients(variant, dtype):
     """dx and db through row mode (grad = 1: UNROLL = 2, twice the items), then the R1 pattern: d/d(dy) of <dx, ddx>
     (grad = 1 again) and, for tanh, d/dx and d/db of it (grad = 2).  The gates must agree with the fp64 signs, which the
     input margin guarantees; the test checks that on the stored y too."""
-    kw = dict(clamp=1.0) if act == 'lrelu' else {}
+    act, kw = BA_GRAD[variant]
+    kw = dict(kw)
     shape = (GRAD_N[torch.empty(0, dtype=dtype).element_size()], 96, 160, 200)
     x, b = ba_inputs(shape, 1, dtype, act, kw, seed=110)
+    assert ba_near_kink(x, b, 1, act, kw).min().item() >= 0
     d = assert_row_mode(x, 1, 1)
     g = torch.Generator(device=DEV).manual_seed(111)
     dy = torch.randn(shape, generator=g, device=DEV).to(dtype).requires_grad_(True)
@@ -275,19 +314,21 @@ def test_bias_act_row_mode_gradients(act, dtype):
         got = (y > 0) & (y.double().abs() < k['clamp'])
         assert torch.equal(want, got)
         assert 0.05 < (~want).double().mean().item() < 0.95   # both gates are taken
+    elif kw.get('clamp') is not None:                       # the clamp gate is taken on both sides
+        assert 0.05 < (y.double().abs() >= kw['clamp']).double().mean().item() < 0.95
     n_ulp = 8 if act == 'tanh' else 4
-    m = Meter(f'bias_act row dx {act} {dtype} ({d["items"]} items)', dtype)
+    m = Meter(f'bias_act row dx {variant} {dtype} ({d["items"]} items)', dtype)
     m.add(dx, ba_grad_ref(dy.detach(), y, kw, act, 1), n_ulp=n_ulp)
     m.done()
-    m = Meter(f'bias_act row d(dy) R1 {act} {dtype}', dtype)
+    m = Meter(f'bias_act row d(dy) R1 {variant} {dtype}', dtype)
     m.add(second[0], ba_grad_ref(ddx, y, kw, act, 1), n_ulp=n_ulp)
     m.done()
-    _check_db(f'bias_act db {act} {dtype}', db, dx)
+    _check_db(f'bias_act db {variant} {dtype}', db, dx)
     if act == 'tanh':
-        m = Meter(f'bias_act row d(x) R1 {act} {dtype}', dtype)
+        m = Meter(f'bias_act row d(x) R1 {variant} {dtype}', dtype)
         m.add(second[1], ba_grad_ref(ddx, y, kw, act, 2, dy=dy.detach()), n_ulp=n_ulp)
         m.done()
-        _check_db(f'bias_act d(b) R1 {act} {dtype}', second[2], second[1])
+        _check_db(f'bias_act d(b) R1 {variant} {dtype}', second[2], second[1])
 
 
 def _check_db(name, db, dx):
@@ -502,6 +543,39 @@ def test_upfirdn2d_more_than_32768_images():
     assert d['path'] == 'tiled' and d['images'] > 32768, d
     y = _up().upfirdn2d(x, f, **kw)
     upf_compare('upfirdn2d tiled 34000 images fp32', y, x, f, kw, cdim=1, step=4096)
+
+
+GENERIC = {
+    # a 5x5 / 3x5 filter (not the fast kernel's 4x4) on NCHW: the tiled kernel with flip (ops_upfirdn2d.cu:58), gain and
+    # zero fill on every side of the up-sampled image, then decimation with a crop
+    'tiled_up2_flip': ((8, 32, 97, 101), 'nchw', (5, 5), dict(up=2, padding=[3, 2, 2, 3], flip_filter=True, gain=4.0)),
+    'tiled_down2_crop': ((8, 32, 97, 101), 'nchw', (3, 5), dict(down=2, padding=[-1, 3, 2, -2], gain=0.5)),
+    # channels_last RGB (C = 3 < VEC, so x.stride(3) = 3): the strided kernel, channel-fastest, up 2 (column phases)
+    'strided_up2_cl3': ((16, 3, 128, 129), 'cl', (4, 4), dict(up=2, padding=[2, 1, 2, 1], gain=4.0)),
+    # every other column of an NCHW buffer (x.stride(3) = 2): the strided kernel, column-fastest, up 2 and flipped
+    'strided_up2_flip_cols': ((8, 16, 64, 75), 'cols', (4, 4), dict(up=2, padding=[1, 2, 2, 1], flip_filter=True, gain=4.0)),
+}
+
+
+@pytest.mark.parametrize('dtype', DT3, ids=DT3_IDS)
+@pytest.mark.parametrize('case', list(GENERIC))
+def test_upfirdn2d_tiled_and_strided_kernels(case, dtype):
+    """The kernels every non-4x4 filter and every layout without a unit column stride takes, with the inputs that tell
+    their index maths apart: an asymmetric filter with flip, a gain, up-sampled column phases, padding and crops."""
+    shape, layout, fshape, kw = GENERIC[case]
+    g = torch.Generator(device=DEV).manual_seed(260)
+    if layout == 'cols':
+        x = torch.randn(shape[:3] + (2 * shape[3],), generator=g, device=DEV).to(dtype)[..., ::2]
+    else:
+        x = torch.randn(shape, generator=g, device=DEV).to(dtype)
+        if layout == 'cl':
+            x = x.contiguous(memory_format=torch.channels_last)
+    f = (torch.rand(fshape, generator=torch.Generator().manual_seed(261)) + 0.1).to(DEV)
+    d = upf_dispatch(x, f, kw.get('up', 1), kw.get('down', 1), kw['padding'])
+    assert d['path'] == ('tiled' if layout == 'nchw' else 'strided'), d
+    y = _up().upfirdn2d(x, f, **kw)
+    assert tuple(y.shape[2:]) == d['out']
+    upf_compare(f'upfirdn2d {case} {dtype}', y, x, f, kw, cdim=0)
 
 
 def test_upfirdn2d_fast_kernel_64bit_offsets():
