@@ -58,6 +58,28 @@ int p3d_png_writer_submit(void* writer, const uint8_t* dev_scanlines, int32_t h,
 /* Same with scan-lines already in HOST memory (copied before the call returns).  No CUDA involved. */
 int p3d_png_writer_submit_host(void* writer, const uint8_t* host_scanlines, int32_t h, int32_t w, int32_t channels,
                                const char* path);
+/* Device encoder: N filtered scan-line streams (device memory, what p3d_image_to_png_scanlines writes) -> N complete PNG
+   files in device memory (signature, IHDR, one IDAT with one zlib stream, IEND), deflated on the GPU: 16 KB segments of
+   each stream are LZ77-matched (32 KB window, reaching back across segments) and coded as the smallest of a dynamic,
+   fixed or stored block, then joined by sync flushes; every CRC-32, the Adler-32 and each file's length are computed on
+   the device.  The bytes written are a function of the input bytes alone (not of the grid, the SM count or timing).
+   Envelope: 1 <= n <= 65535, C in {1, 3, 4}, h, w >= 1 and h * (1 + w * C) <= 2^28; outside it the size queries return
+   0 and the encoder P3D_EINVAL.
+     bound       worst-case file bytes: 63 + h * (1 + w * C) + 10 * ceil(h * (1 + w * C) / 16384) (all-stored blocks).
+     workspace   device scratch of p3d_png_device_workspace_bytes(n, h, w, C) bytes; its contents on entry do not matter.
+     out         file i at out + i * out_stride (out_stride >= bound); bytes past its length are left untouched.
+     out_lens    device array of n lengths, written by the encoder.
+   Asynchronous on `stream`; P3D_EWORKSPACE when workspace_bytes is short, P3D_EINVAL on NULL pointers or bad shapes. */
+size_t p3d_png_device_bound(int32_t h, int32_t w, int32_t channels);
+size_t p3d_png_device_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t channels);
+int p3d_png_encode_device(const uint8_t* scanlines, int32_t n, int32_t h, int32_t w, int32_t channels, void* workspace,
+                          size_t workspace_bytes, uint8_t* out, size_t out_stride, uint64_t* out_lens, void* stream);
+/* Enqueue one file that p3d_png_encode_device left in DEVICE memory: the D2H copies of its length and of
+   p3d_png_device_bound(h, w, channels) bytes (into the writer's pinned staging) are enqueued on `stream` and the call
+   returns at once; a worker waits for them and writes the file's length in bytes to `path` (".tmp" + rename, as above).
+   The shape only sizes the copy: the worker writes what the device encoded. */
+int p3d_png_writer_submit_encoded(void* writer, const uint8_t* dev_file, const uint64_t* dev_len, int32_t h, int32_t w,
+                                  int32_t channels, const char* path, void* stream);
 /* Wait until every submitted image is on disk; *n_failed = number of images that could not be written since the
    last flush (p3d_last_error() has the first failure's message). */
 int p3d_png_writer_flush(void* writer, int32_t* n_failed);

@@ -157,6 +157,7 @@ struct Job {
     bool pinned;
     cudaEvent_t ev = nullptr;     // D2H copy done (nullptr for host submissions)
     int device;
+    bool encoded = false;         // host holds [u64 length | file bytes] from p3d_png_encode_device
 };
 
 struct Writer {
@@ -192,13 +193,21 @@ struct Writer {
                 if (e != cudaSuccess) { fail(std::string("copy of ") + j.path + " failed: " + cudaGetErrorString(e)); ok = false; }
             }
             if (ok) {
-                png.resize(encode_bound(j.h, j.w, j.c));
+                const unsigned char* file = png.data();
                 size_t len = 0;
-                if (encode(j.host, j.h, j.w, j.c, level, png.data(), png.size(), &len) != P3D_OK) { fail("encoding " + j.path + " failed"); ok = false; }
+                if (j.encoded) {
+                    memcpy(&len, j.host, sizeof(uint64_t));
+                    file = j.host + sizeof(uint64_t);
+                    if (len > j.bytes - sizeof(uint64_t)) { fail("encoded " + j.path + " is longer than its bound"); ok = false; }
+                } else {
+                    png.resize(encode_bound(j.h, j.w, j.c));
+                    if (encode(j.host, j.h, j.w, j.c, level, png.data(), png.size(), &len) != P3D_OK) { fail("encoding " + j.path + " failed"); ok = false; }
+                    file = png.data();
+                }
                 if (ok) {
                     const std::string tmp = j.path + ".tmp";
                     FILE* f = fopen(tmp.c_str(), "wb");
-                    if (!f || fwrite(png.data(), 1, len, f) != len || fclose(f) != 0 || rename(tmp.c_str(), j.path.c_str()) != 0) {
+                    if (!f || fwrite(file, 1, len, f) != len || fclose(f) != 0 || rename(tmp.c_str(), j.path.c_str()) != 0) {
                         if (f) remove(tmp.c_str());
                         fail("cannot write " + j.path);
                     }
@@ -284,12 +293,14 @@ extern "C" int p3d_png_writer_create(int32_t n_threads, int32_t compress_level, 
     return P3D_OK;
 }
 
-extern "C" int p3d_png_writer_submit(void* writer, const uint8_t* dev_scanlines, int32_t h, int32_t w, int32_t channels,
-                                     const char* path, void* stream) {
-    if (int rc = check_image(writer, dev_scanlines, h, w, channels, path)) return rc;
-    Writer* wr = (Writer*)writer;
-    Job j;
-    j.path = path; j.h = h; j.w = w; j.c = channels; j.bytes = p3d_png_scanline_bytes(h, w, channels); j.pinned = true; j.host = nullptr; j.cap = 0;
+namespace p3d {
+namespace {
+
+// D2H copies of `n` (pointer, bytes) pieces, back to back into the writer's pinned staging, then the job is queued
+int submit_device(Writer* wr, Job& j, const void* const* src, const size_t* bytes, int n, cudaStream_t stream) {
+    j.bytes = 0;
+    for (int i = 0; i < n; ++i) j.bytes += bytes[i];
+    j.pinned = true; j.host = nullptr; j.cap = 0;
     {
         std::lock_guard<std::mutex> lk(wr->m);
         for (size_t i = 0; i < wr->pinned_free.size(); ++i)
@@ -304,9 +315,10 @@ extern "C" int p3d_png_writer_submit(void* writer, const uint8_t* dev_scanlines,
         j.cap = j.bytes;
     }
     P3D_CUDA_TRY(cudaGetDevice(&j.device));
-    P3D_CUDA_TRY(cudaMemcpyAsync(j.host, dev_scanlines, j.bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    for (size_t i = 0, o = 0; i < (size_t)n; o += bytes[i++])
+        P3D_CUDA_TRY(cudaMemcpyAsync(j.host + o, src[i], bytes[i], cudaMemcpyDeviceToHost, stream));
     P3D_CUDA_TRY(cudaEventCreateWithFlags(&j.ev, cudaEventDisableTiming | cudaEventBlockingSync));
-    P3D_CUDA_TRY(cudaEventRecord(j.ev, (cudaStream_t)stream));
+    P3D_CUDA_TRY(cudaEventRecord(j.ev, stream));
     {
         std::lock_guard<std::mutex> lk(wr->m);
         wr->q.push_back(std::move(j));
@@ -314,6 +326,32 @@ extern "C" int p3d_png_writer_submit(void* writer, const uint8_t* dev_scanlines,
     }
     wr->cv_work.notify_one();
     return P3D_OK;
+}
+
+}  // namespace
+}  // namespace p3d
+
+extern "C" int p3d_png_writer_submit(void* writer, const uint8_t* dev_scanlines, int32_t h, int32_t w, int32_t channels,
+                                     const char* path, void* stream) {
+    if (int rc = check_image(writer, dev_scanlines, h, w, channels, path)) return rc;
+    Job j;
+    j.path = path; j.h = h; j.w = w; j.c = channels;
+    const void* src[1] = {dev_scanlines};
+    const size_t bytes[1] = {p3d_png_scanline_bytes(h, w, channels)};
+    return submit_device((Writer*)writer, j, src, bytes, 1, (cudaStream_t)stream);
+}
+
+extern "C" int p3d_png_writer_submit_encoded(void* writer, const uint8_t* dev_file, const uint64_t* dev_len, int32_t h, int32_t w,
+                                             int32_t channels, const char* path, void* stream) {
+    if (int rc = check_image(writer, dev_file, h, w, channels, path)) return rc;
+    P3D_REQUIRE(dev_len != nullptr, "p3d_png_writer_submit_encoded: NULL length pointer");
+    const size_t bound = p3d_png_device_bound(h, w, channels);
+    P3D_REQUIRE(bound != 0, "p3d_png_writer_submit_encoded: h=%d w=%d c=%d outside the device encoder's envelope", h, w, channels);
+    Job j;
+    j.path = path; j.h = h; j.w = w; j.c = channels; j.encoded = true;
+    const void* src[2] = {dev_len, dev_file};
+    const size_t bytes[2] = {sizeof(uint64_t), bound};
+    return submit_device((Writer*)writer, j, src, bytes, 2, (cudaStream_t)stream);
 }
 
 extern "C" int p3d_png_writer_submit_host(void* writer, const uint8_t* host_scanlines, int32_t h, int32_t w, int32_t channels,
