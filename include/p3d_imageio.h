@@ -1,5 +1,6 @@
 /*
- * p3d_imageio.h - C ABI of the image output path behind the renderer (SURVEY.md 8f-4).
+ * p3d_imageio.h - C ABI of the image output path behind the renderer (SURVEY.md 8f-4) and of the PNG input path of
+ * the training set (load_images, at the end of this header).
  *
  * The reference's eval sweep ends every view with `I(out['image']).save(fn)` and `I(xyza).save(fn)`
  * (/root/reference/_scripts/eval/generate.py:141-148): a blocking `.cpu()` of fp32 images, torchvision's
@@ -84,6 +85,72 @@ int p3d_png_writer_submit_encoded(void* writer, const uint8_t* dev_file, const u
    last flush (p3d_last_error() has the first failure's message). */
 int p3d_png_writer_flush(void* writer, int32_t* n_failed);
 int p3d_png_writer_destroy(void* writer);
+
+/* ---- Image input: PNG files decoded on the device (DESIGN.md 4.7) ----
+   The training set's chain `I(path).resize(size)[.convert('RGBA').bg('w').convert('RGB')].t()` (twodee_v1.py) for a
+   batch of files: the host inspects each file and packs its zlib stream, the device inflates, unfilters, resizes
+   (PIL's nearest), optionally composites onto white (PIL's integer `Image.alpha_composite`) and writes float32 / 255.
+   Supported: colour type 0 at 8 bits (PIL mode L), types 2 and 6 at 8 or 16 bits (RGB / RGBA; PIL keeps the high byte
+   of a 16-bit sample), compression 0, filter method 0, no interlace, and no tRNS chunk on type 0 or 2. */
+typedef struct {
+    int32_t h, w;
+    int32_t channels;       /* colour type 0 / 2 / 6 -> 1 / 3 / 4 */
+    int32_t depth;          /* bits per sample: 8, or 16 for 3 and 4 channels */
+    int32_t n_idat;         /* IDAT chunks, zero-length ones included */
+    int32_t reserved;
+    uint64_t stream_bytes;  /* the zlib stream: every IDAT payload, concatenated */
+} p3d_png_info;
+
+/* Inspect one PNG file in host memory (`len` bytes): the signature, every chunk's length and CRC, IHDR, consecutive
+   IDATs and IEND; ancillary chunks are skipped and unknown critical chunks refused.  Anything outside the supported set
+   is refused with P3D_EINVAL and a message naming the field.  When `stream` is not NULL the IDAT payloads are copied
+   there, info->stream_bytes of them.  No CUDA involved. */
+int p3d_png_inspect(const uint8_t* file, size_t len, p3d_png_info* info, uint8_t* stream);
+
+/* One image of a device decode.  The job array lives in device memory. */
+typedef struct {
+    uint64_t in_offset, in_bytes;  /* its zlib stream: in[in_offset, in_offset + in_bytes) */
+    uint64_t ws_offset;            /* its workspace span: 16-byte aligned, p3d_png_decode_workspace_bytes(...) bytes */
+    int32_t h, w, channels, depth; /* from p3d_png_inspect */
+    int32_t slot;                  /* output image: out + slot * out_channels * out_h * out_w; distinct per job */
+    int32_t reserved;
+} p3d_png_decode_job;
+
+/* Per-image status codes written by p3d_png_decode_device (and returned by p3d_png_inflate_host). */
+#define P3D_PNG_OK          0
+#define P3D_PNG_EJOB        1   /* the job's spans leave the buffers, or its fields leave the envelope */
+#define P3D_PNG_EHEADER     2   /* zlib header: method other than 8, CINFO above 7, bad FCHECK, or a preset dictionary */
+#define P3D_PNG_EBLOCK      3   /* block type 3, or a stored block whose LEN and NLEN disagree */
+#define P3D_PNG_ECODES      4   /* dynamic block header: too many symbols, bad repeat, over-subscribed or incomplete
+                                   code lengths, or no end-of-block code */
+#define P3D_PNG_ESYMBOL     5   /* bits that are no code of the block, literal/length 286-287 or distance 30-31 */
+#define P3D_PNG_EDISTANCE   6   /* a match reaching back past the start of the output */
+#define P3D_PNG_ELONG       7   /* more output than h * (1 + w * bytes per pixel) */
+#define P3D_PNG_ESHORT      8   /* less output than that */
+#define P3D_PNG_ETRUNCATED  9   /* the input ends before the stream (or its Adler-32) does */
+#define P3D_PNG_EADLER     10   /* the Adler-32 trailer does not match the output */
+#define P3D_PNG_EFILTER    11   /* a scan-line filter byte above 4 */
+
+/* Device workspace of one image decoded to out_h x out_w: its decompressed bytes h * (1 + w * channels * depth / 8),
+   16-byte aligned, then out_w + out_h int32 resize indices.  0 outside the envelope: h, w >= 1, a supported
+   (channels, depth), h * (1 + w * channels * depth / 8) <= 2^28 and 1 <= out_h, out_w <= 32768. */
+size_t p3d_png_decode_workspace_bytes(int32_t h, int32_t w, int32_t channels, int32_t depth, int32_t out_h, int32_t out_w);
+
+/* Decode n images (1 <= n <= 65535): `in` (device, in_bytes) holds the packed zlib streams, `jobs` (device, n) say
+   where each is and where it goes.  out (device, float32) is (n, out_channels, out_h, out_w); out_channels is 3 when
+   white_background is set, else every job's channel count.  status (device, n int32) gets one P3D_PNG_* code per job;
+   a job with a non-zero code has its output image zeroed (when its slot is valid) and touches nothing outside its own
+   spans, and the other jobs decode exactly as they would alone.  Every job is checked against in_bytes and
+   workspace_bytes on the device.  Asynchronous on `stream` (three kernels); P3D_EINVAL on NULL pointers or a batch
+   outside the envelope.  The output is a function of the input bytes alone. */
+int p3d_png_decode_device(const uint8_t* in, size_t in_bytes, const p3d_png_decode_job* jobs, int32_t n, int32_t out_h,
+                          int32_t out_w, int32_t out_channels, int32_t white_background, void* workspace,
+                          size_t workspace_bytes, float* out, int32_t* status, void* stream);
+
+/* The device decoder's inflate (bit reader, Huffman tables, copies, Adler-32) run on the CPU, for tests and debugging
+   of malformed streams; not an image path.  Returns the P3D_PNG_* status of inflating the zlib stream into exactly
+   raw_len bytes (1 <= raw_len <= 2^28), or P3D_EINVAL on NULL pointers. */
+int p3d_png_inflate_host(const uint8_t* stream, size_t len, uint8_t* raw, size_t raw_len);
 
 #ifdef __cplusplus
 }

@@ -13,10 +13,12 @@ not: filter choice and deflate level are not part of the image).
                                             ``.save_xyza(xyz, w, bw, fn)`` for ``I(cat([(xyz+bw/2)/bw, w])).save(fn)``
                                             (generate.py:141-147) without materialising the 4-channel image
                                             ``.flush()``                all files on disk (raises if one failed)
+    ``load_images(sources, size, white_background)``  PNG files -> (N,C,H,W) float32 on the GPU: the training set's
+                                            ``I(path).resize(size)[.convert('RGBA').bg('w').convert('RGB')].t()``
     ``AsyncPickleWriter``                   ``uutil.pdump(obj, fn)`` (generate.py:104-105, the marching-cubes dict) off-thread
 
-No CPU path for the device kernels: images must be CUDA tensors (the numpy restatement is ``oracle/imageio_oracle.py``,
-tests only).  ``encode_png`` / ``submit_host`` are pure host code (zlib) and work anywhere.
+No CPU path for the device kernels: images must be CUDA tensors and ``load_images`` decodes on a CUDA device (the numpy
+restatements are ``oracle/imageio_oracle.py`` and ``tests/png_oracle.py``, tests only).  ``encode_png`` / ``submit_host`` are pure host code (zlib) and work anywhere.
 """
 from __future__ import annotations
 
@@ -46,6 +48,35 @@ _lib.register_protos({
     'p3d_png_writer_submit_encoded': (C.c_int, [_VP, _VP, _VP, C.c_int32, C.c_int32, C.c_int32, C.c_char_p, _VP]),
     'p3d_png_writer_destroy': (C.c_int, [_VP]),
 })
+
+
+class PngInfo(C.Structure):
+    """Mirror of ``p3d_png_info`` (include/p3d_imageio.h)."""
+    _fields_ = [('h', C.c_int32), ('w', C.c_int32), ('channels', C.c_int32), ('depth', C.c_int32), ('n_idat', C.c_int32),
+                ('reserved', C.c_int32), ('stream_bytes', C.c_uint64)]
+
+
+class PngDecodeJob(C.Structure):
+    """Mirror of ``p3d_png_decode_job`` (include/p3d_imageio.h)."""
+    _fields_ = [('in_offset', C.c_uint64), ('in_bytes', C.c_uint64), ('ws_offset', C.c_uint64), ('h', C.c_int32),
+                ('w', C.c_int32), ('channels', C.c_int32), ('depth', C.c_int32), ('slot', C.c_int32), ('reserved', C.c_int32)]
+
+
+_lib.register_protos({
+    'p3d_png_inspect': (C.c_int, [_VP, C.c_size_t, C.POINTER(PngInfo), _VP]),
+    'p3d_png_decode_workspace_bytes': (C.c_size_t, [C.c_int32] * 6),
+    'p3d_png_decode_device': (C.c_int, [_VP, C.c_size_t, _VP, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _VP, C.c_size_t,
+                                        _VP, _VP, _VP]),
+    'p3d_png_inflate_host': (C.c_int, [_VP, C.c_size_t, _VP, C.c_size_t]),
+})
+
+# P3D_PNG_* status codes of p3d_png_decode_device
+PNG_STATUS = {
+    1: 'job outside the buffers or the envelope', 2: 'bad zlib header', 3: 'bad deflate block (type 3, or stored LEN/NLEN)',
+    4: 'bad Huffman code lengths', 5: 'invalid Huffman code or symbol', 6: 'match distance past the start of the output',
+    7: 'decompresses to more than h*(1+w*bytes per pixel) bytes', 8: 'decompresses to fewer than h*(1+w*bytes per pixel) bytes',
+    9: 'zlib stream truncated', 10: 'Adler-32 mismatch', 11: 'scan-line filter byte above 4',
+}
 
 
 def _canon(img, name='image'):
@@ -127,6 +158,120 @@ def png_encode_device(scan, shape):
         _lib.check(L.p3d_png_encode_device(scan.contiguous().data_ptr(), N, H, W, c, ws.data_ptr(), ws_bytes, files.data_ptr(), bound,
                                            lens.data_ptr(), _lib.stream_ptr(scan.device)))
     return files, lens
+
+
+def png_inspect(data):
+    """PNG file bytes -> ``PngInfo`` (``p3d_png_inspect``); RuntimeError naming the field for anything unsupported."""
+    import numpy as np
+    buf = np.frombuffer(data, dtype=np.uint8)
+    info = PngInfo()
+    _lib.check(_lib.lib().p3d_png_inspect(buf.ctypes.data, buf.size, C.byref(info), None))
+    return info
+
+
+def load_images(sources, size=None, white_background=False, device=None):
+    """PNG files (paths or ``bytes``) -> float32 (N, C, H, W) on the device, decoded on the GPU (``p3d_png_decode_device``).
+
+    Equal, element for element, to ``torch.stack([I(src).resize(size).t() ...])`` - with ``white_background``, to
+    ``I(src).resize(size).convert('RGBA').bg('w').convert('RGB').t()`` (C = 3) - where ``I`` is the reference's
+    ``_util/twodee_v1.py`` image class: PIL's nearest resize, PIL's integer alpha composite and ``to_tensor``'s / 255.
+    ``size``: an int (square) or (H, W); None keeps the files' size, which must then be the same for all of them.
+    Without ``white_background`` every file must have the same channel count (L: 1, RGB: 3, RGBA: 4).
+
+    The files are read and inspected on the host, their IDAT payloads packed into one pinned buffer behind the job
+    table, and one host-to-device copy and one decode launch sequence run on the current stream.  RuntimeError names
+    every file that is refused or fails to decode.  There is no host fallback."""
+    out, codes, names = decode_batch(sources, size, white_background, device)
+    bad = [f'{names[i]}: {PNG_STATUS.get(s, f"status {s}")}' for i, s in enumerate(codes) if s]
+    if bad:
+        raise RuntimeError('panic3d_b200.imageio.load_images: ' + '; '.join(bad))
+    return out
+
+
+def decode_batch(sources, size=None, white_background=False, device=None):
+    """``load_images`` without the raise on a failed decode: ``(out, status, names)``, with one ``P3D_PNG_*`` code per
+    source (``PNG_STATUS`` names them) and the failed images' outputs zeroed.  Refused files still raise."""
+    st, names = _stage(sources, size, white_background, device)
+    out, status = _decode_staged(st)
+    return out, status.cpu().tolist(), names
+
+
+def _stage(sources, size, white_background, device):
+    """Read and inspect the files and pack the job table and their zlib streams into one pinned buffer."""
+    import numpy as np
+    dev = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
+    if dev.type != 'cuda':
+        raise RuntimeError('panic3d_b200.imageio.load_images: the decoder runs on a CUDA device (there is no CPU path)')
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    names, datas = [], []
+    for i, src in enumerate(sources):
+        if isinstance(src, (bytes, bytearray, memoryview)):
+            names.append(f'<bytes #{i}>')
+            datas.append(np.frombuffer(src, dtype=np.uint8))
+        else:
+            names.append(os.fspath(src))
+            with open(names[-1], 'rb') as f:
+                datas.append(np.frombuffer(f.read(), dtype=np.uint8))
+    n = len(datas)
+    if n < 1:
+        raise RuntimeError('panic3d_b200.imageio.load_images: no sources')
+    L = _lib.lib()
+    infos, bad = [], []
+    for name, buf in zip(names, datas):
+        info = PngInfo()
+        if L.p3d_png_inspect(buf.ctypes.data, buf.size, C.byref(info), None) != 0:
+            bad.append(f'{name}: {L.p3d_last_error().decode("utf-8", "replace")}')
+        infos.append(info)
+    if bad:
+        raise RuntimeError('panic3d_b200.imageio.load_images: ' + '; '.join(bad))
+    if size is None:
+        shapes = {(f.h, f.w) for f in infos}
+        if len(shapes) != 1:
+            raise RuntimeError(f'panic3d_b200.imageio.load_images: files of sizes {sorted(shapes)} need a size to resize to')
+        out_h, out_w = shapes.pop()
+    else:
+        out_h, out_w = (size, size) if isinstance(size, int) else (int(size[0]), int(size[1]))
+    if white_background:
+        c = 3
+    else:
+        chans = {f.channels for f in infos}
+        if len(chans) != 1:
+            raise RuntimeError(f'panic3d_b200.imageio.load_images: files with {sorted(chans)} channels cannot be stacked '
+                               '(white_background=True gives 3 channels for all of them)')
+        c = chans.pop()
+    jobs = (PngDecodeJob * n)()
+    head = C.sizeof(jobs)
+    off, ws_total = 0, 0
+    for i, f in enumerate(infos):
+        ws = L.p3d_png_decode_workspace_bytes(f.h, f.w, f.channels, f.depth, out_h, out_w)
+        if not ws:
+            raise RuntimeError(f'panic3d_b200.imageio.load_images: {names[i]}: output {out_h}x{out_w} outside the envelope')
+        jobs[i] = PngDecodeJob(off, f.stream_bytes, ws_total, f.h, f.w, f.channels, f.depth, i, 0)
+        off += f.stream_bytes
+        ws_total += ws
+    pinned = torch.empty(head + off, dtype=torch.uint8, pin_memory=True)
+    base = pinned.data_ptr()
+    C.memmove(base, C.addressof(jobs), head)
+    for i, (buf, job) in enumerate(zip(datas, jobs)):
+        _lib.check(L.p3d_png_inspect(buf.ctypes.data, buf.size, C.byref(infos[i]), base + head + job.in_offset))
+    st = dict(dev=dev, pinned=pinned, head=head, in_bytes=off, n=n, out_h=out_h, out_w=out_w, c=c, white=int(bool(white_background)),
+              ws_bytes=ws_total)
+    return st, names
+
+
+def _decode_staged(st):
+    """One H2D copy of the packed jobs and streams, then the decode launch sequence, on the current stream of st['dev']."""
+    dev = st['dev']
+    with torch.cuda.device(dev):
+        staged = st['pinned'].to(dev, non_blocking=True)
+        ws = torch.empty(st['ws_bytes'], dtype=torch.uint8, device=dev)
+        out = torch.empty((st['n'], st['c'], st['out_h'], st['out_w']), dtype=torch.float32, device=dev)
+        status = torch.empty(st['n'], dtype=torch.int32, device=dev)
+        _lib.check(_lib.lib().p3d_png_decode_device(staged.data_ptr() + st['head'], st['in_bytes'], staged.data_ptr(), st['n'], st['out_h'],
+                                                    st['out_w'], st['c'], st['white'], ws.data_ptr(), st['ws_bytes'], out.data_ptr(),
+                                                    status.data_ptr(), _lib.stream_ptr(dev)))
+    return out, status
 
 
 def encode_png(scanlines, h, w, c, level=3):
