@@ -119,10 +119,12 @@ def run_gpu(args):
 
 
 # ------------------------------------------------------------------------------------------------------ CPU model
-def tap_lines(S, P=512, seed=0x5EED):
+def tap_lines(S, P=512, seed=0x5EED, fine=False):
     """Per view: the 128 B line of every coarse tap, (N, M, S, 3 planes, 4 taps) int64, -1 where the kernel predicates the
     plane's loads off (its footprint lies more than one texel outside the plane).  The footprint is clamped into the plane
-    the way fused::plane_taps_rec clamps it."""
+    the way fused::plane_taps_rec clamps it.  fine: the taps of the fine pass instead, at the depths of the oracle's
+    importance sampler fed flat coarse weights (the bench's random planes and decoder put no surface anywhere, and the
+    sampler's 0.01 floor spreads the rest)."""
     import numpy as np
     import torch
     from oracle import philox, renderer_oracle as orc
@@ -132,6 +134,10 @@ def tap_lines(S, P=512, seed=0x5EED):
     N, M = ro.shape[:2]
     u = philox.uniforms(seed, np.arange(N * M * S, dtype=np.uint64), philox.STREAM_COARSE).reshape(N, M, S, 1)
     t = orc.stratified_depths(torch.from_numpy(u), OPTS['ray_start'], OPTS['ray_end'])
+    if fine:
+        uf = torch.from_numpy(philox.uniforms(seed, np.arange(N * M * S, dtype=np.uint64), philox.STREAM_FINE).reshape(N * M, S))
+        z = t.reshape(N * M, S).to(uf.dtype)
+        t = orc.importance_depths(z, torch.ones(N * M, S - 1, dtype=z.dtype), uf).reshape(N, M, S, 1).to(t.dtype)
     xyz = (ro[:, :, None] + t * rd[:, :, None]).reshape(N, M * S, 3)
     co = (orc.plane_coords(xyz, True) * (2.0 / OPTS['box_warp'])).numpy().astype(np.float32)        # (N, 3, M*S, 2)
     f = ((co + 1.0) * P - 1.0) * 0.5
@@ -199,13 +205,66 @@ def run_model(args):
     return res
 
 
+def l2_model(S=96, P=512, sms=132):
+    """What shares L2 while k_render_ws3 runs bench.py's workload (--model).  Groups of GR rays run in waves of `sms`
+    groups (CTA b takes groups b, b + sms, ...), so wave w is rays [w sms GR, (w + 1) sms GR) of the call.  Per plane and
+    pass: the distinct 128 B texel lines a wave asks for, and how many waves back each of them was last asked for (its
+    reuse distance; 'first' = never before in the call).  Then the colour areas: their footprint, how many passes lie
+    between a tile's store and its load, and how many of their bytes are live (stored, not yet loaded) at once."""
+    import numpy as np
+    GR = 384 // S
+    res = {'wave_rays': sms * GR}
+    for name, fine in (('coarse', False), ('fine', True)):
+        lines = tap_lines(S, P, fine=fine)                                                 # (N, M, S, 3, 4)
+        N, M = lines.shape[:2]
+        wave = (np.arange(N * M) // GR) // sms                                             # wave of each ray of the call
+        for p in range(3):
+            x = lines[:, :, :, p, :].reshape(N, M, S * 4)
+            x = np.where(x >= 0, x + (np.arange(N) * 3 * P * P)[:, None, None], -1).reshape(N * M, S * 4)   # one id per view's line
+            keys = x * 4096 + wave[:, None]
+            keys = np.unique(keys[x >= 0])
+            line, w = keys // 4096, keys % 4096
+            per_wave = np.bincount(w)
+            same = np.concatenate([[False], line[1:] == line[:-1]])
+            dist = np.where(same, w - np.concatenate([[0], w[:-1]]), 0)
+            n = len(keys)
+            res[f'{name} plane {p}'] = dict(
+                distinct_lines_per_wave=int(np.median(per_wave)), mb_per_wave=round(float(np.median(per_wave)) * 128 / 1e6, 2),
+                reuse_1_wave=round(float((dist == 1).sum()) / n, 3), reuse_2_7_waves=round(float(((dist >= 2) & (dist < 8)).sum()) / n, 3),
+                reuse_8plus_waves=round(float((dist >= 8).sum()) / n, 3), first=round(float((~same).sum()) / n, 3),
+                distinct_lines_call_mb=round(len(np.unique(line)) * 128 / 1e6, 1))
+    # colour areas of one CTA with n_my groups: tile q of the tile sequence is stored at time q; colours(n) loads group n's
+    # six tiles during the pass after F(n) (the decoder signals F(n)'s stores in the next pass's first tile)
+    n_my = (N * M // GR + sms - 1) // sms
+    passes = [None] * (2 * n_my)
+    j_of = {}
+    for j in range(2 * n_my):
+        k = j - 2
+        if j == 0: pd = (0, 0)
+        elif n_my == 1: pd = (0, 1)
+        elif j == 1: pd = (1, 0)
+        elif k < 2 * (n_my - 2): pd = ((k >> 1) + 2, 0) if (k & 1) else (k >> 1, 1)
+        else: pd = (n_my - 2 + (k - 2 * (n_my - 2)), 1)
+        j_of[pd] = j
+    dist_c = [j_of[(n, 1)] + 1 - j_of[(n, 0)] for n in range(n_my)]
+    live = []
+    for j in range(2 * n_my):                                    # tiles stored and not yet loaded at the end of pass j
+        live.append(sum(3 * ((j_of[(n, 0)] <= j < j_of[(n, 1)] + 1) + (j_of[(n, 1)] <= j < j_of[(n, 1)] + 1)) for n in range(n_my)))
+    tile_b = 128 * 128
+    res['colour areas'] = dict(
+        footprint_mb=round(5 * 3 * tile_b * sms / 1e6, 1), bytes_per_call_gb=round(2 * N * M * S * 128 / 1e9, 2),
+        store_to_load_passes_coarse=sorted(set(dist_c[2:-2])), store_to_load_passes_fine=[1],
+        live_mb_steady=round(float(np.median(live[4:-4])) * tile_b * sms / 1e6, 1), live_mb_max=round(max(live) * tile_b * sms / 1e6, 1))
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
     ap.add_argument('--model', action='store_true', help='CPU: count the coarse pass\'s L2 line requests per ray order')
     ap.add_argument('--rounds', type=int, default=5)
     ap.add_argument('--launches', type=int, default=50)
     args = ap.parse_args()
-    print(json.dumps(run_model(args) if args.model else run_gpu(args)), flush=True)
+    print(json.dumps(dict(run_model(args), l2=l2_model()) if args.model else run_gpu(args)), flush=True)
 
 
 if __name__ == '__main__':

@@ -58,6 +58,21 @@ __device__ __forceinline__ void bulk_load(uint32_t sdst, const void* gsrc, uint3
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(sdst), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+// ---- L2 residency: per-instruction cache policies (createpolicy -> .L2::cache_hint operands) and line discards.  They
+// change which lines L2 keeps, never a value that is read.
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+// bulk_load under the L2 policy `pol`
+__device__ __forceinline__ void bulk_load_hint(uint32_t sdst, const void* gsrc, uint32_t bytes, unsigned long long* bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(sdst), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
+}
+// Invalidates the 128 B line at `p` (128-byte aligned) in L2 without writing it back: its contents become undefined.  A
+// generic-proxy write; an async-proxy write of the same bytes that must follow it needs fence.proxy.async.global between.
+__device__ __forceinline__ void l2_discard_line(const void* p) { asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory"); }
 // ---- warpgroup MMA (sm_90a).  Operands in shared memory use the K-major, no-swizzle canonical layout of tile_off():
 // 8-row x 16-byte core matrices, kSBO bytes between 8-row groups, `lbo` bytes between 8-column (16-byte) groups along K.
 // A warpgroup's accumulator fragment of m64nN: element i of thread (warp w, lane l) is row 16 w + l / 4 + 8 ((i / 2) & 1),

@@ -4,9 +4,9 @@
 //
 // A tile's colour sigmoids wait for the group's compositing weights (omega), which exist only after its fine pass.  They are
 // staged in global memory, in this CTA's own slices of the workspace colour buffers (see colour_area: coarse areas
-// CA[n % 3] and fine areas FA[n & 1], 5 x 48 KB per CTA, ~32 MB on 132 SMs).  The areas are rewritten every few groups, so
-// their footprint fits the 50 MB L2, but they share it with the streamed tri-plane gather; how much of the round trip is
-// served by L2 rather than HBM has not been measured.  The decoder's epilogue stages each 8 KB tile half in shared memory
+// CA[n % 3] and fine areas FA[n & 1], 5 x 48 KB per CTA, ~32 MB on 132 SMs).  They share the 50 MB L2 with the tri-plane
+// gather, so the ray warps load them evict-first and discard each line from L2 once its load has landed: a dead line
+// leaves without a write-back and without pushing out texels (DESIGN §5).  The decoder's epilogue stages each 8 KB tile half in shared memory
 // for one cp.async.bulk store; once a group's fine pass is stored, the ray warps bulk-load their own rays' rows back into
 // shared memory (mbarrier complete_tx) and reduce them there (colours(n)), off the decoder's critical path.  With F(n)
 // followed by C(n+2):
@@ -338,9 +338,20 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
             wgbar();
             if (elect) {
                 // The area was last read by the ray warps' loads for group n - 3 (CA[n % 3]) or n - 2 (FA[n & 1]).  Their
-                // colours() have waited for every load to land before arriving on that group's state_free.
+                // colours() have waited for every load to land, and discarded the lines from L2, before arriving on that
+                // group's state_free.  The chain from those discards to this thread's bulk stores into the same lines:
+                //   discard.global.L2             generic-proxy writes of each ray-warp lane, then __syncwarp (the warp's
+                //                                 lanes' writes are ordered before lane 0's later operations);
+                //   mbarrier.arrive               lane 0, release.cta (cumulative: includes its warp's discards);
+                //   mbarrier.try_wait             here, acquire.cta: observes the completed state_free phase;
+                //   fence.proxy.async.global      orders what was acquired before this thread's later async-proxy operations;
+                //   cp.async.bulk (store)         cannot be overtaken by a discard, which would leave undefined colours.
+                // One fence at tile 0 covers the area: tiles 1 and 2 are stored later by the same thread.
                 const int prev = td.n - (td.pass == 0 ? 3 : 2);
-                if (td.k == 0 && prev >= 0) RC_WAIT(1, RC_STATE_FREE, &sm.state_free[prev & 3], (prev >> 2) & 1);
+                if (td.k == 0 && prev >= 0) {
+                    RC_WAIT(1, RC_STATE_FREE, &sm.state_free[prev & 3], (prev >> 2) & 1);
+                    fence_proxy_async_global();
+                }
                 bulk_store(colour_area(td.n, td.pass) + (td.k * 128 + 64 * chunk) * kRgb, smem_u32(stage_tile), kHalfBytes);
                 bulk_commit();
             }
@@ -575,6 +586,12 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
         // colour area - are bulk-loaded into the same rows of col_buf[t % kColBufs], which the warp reloads with tile
         // t + kColBufs as soon as all its lanes have read it.
         constexpr int RW = GR / kRW;              // rays of this warp: rw + kRW i, i < RW (1 at S = 96, 2 at S = 48)
+        static_assert(RW * RPT == 32, "a ray warp's rows of a tile: one 128 B line per lane");
+        // The colour areas are a round trip through L2: each line is read once, by the warp that owns its row, one to three
+        // passes after its store.  The loads evict first, and the warp discards its lines once its load has landed, so a
+        // dead line leaves L2 without a write-back to HBM and without taking the place of the tri-plane's texels.
+        const uint64_t pol_colour = l2_evict_first();
+        const int my_row = (rw + kRW * (lane / RPT)) * RPT + lane % RPT;      // this lane's row (line) of a tile
         auto load_tile = [&](int n, int t) {      // lane 0 only
             const int pass = t / 3, k = t - 3 * pass, b = t % kColBufs;
             const float* area = colour_area(n, pass) + k * 128 * kRgb;
@@ -582,7 +599,7 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
 #pragma unroll
             for (int i = 0; i < RW; ++i) {
                 const int row = (rw + kRW * i) * RPT;
-                bulk_load(smem_u32(sm.col_buf[b] + row * kRgb), area + row * kRgb, RPT * kRowBytes, &sm.col_full[rw][b]);
+                bulk_load_hint(smem_u32(sm.col_buf[b] + row * kRgb), area + row * kRgb, RPT * kRowBytes, &sm.col_full[rw][b], pol_colour);
             }
         };
         auto colours = [&](int n, const float (&back)[RW]) {
@@ -616,6 +633,12 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
                     for (int j = 0; j < 16; ++j) omj[h][j] = live ? sl.om[rl * L + pos[r0 + j]] : 0.f;
                 }
                 RC_WAIT(2, RC_COL_FULL, &sm.col_full[rw][b], ((6 * n + t) / kColBufs) & 1);
+                {
+                    // the load of the warp's rows has landed (its reads of global memory are done): drop them from L2.  A
+                    // workspace that is not 128-byte aligned keeps its lines (the bulk copies need only 16 bytes).
+                    const float* line = colour_area(n, pass) + (k * 128 + my_row) * kRgb;
+                    if ((reinterpret_cast<uintptr_t>(line) & 127) == 0) l2_discard_line(line);
+                }
                 const float* buf = sm.col_buf[b];
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -659,7 +682,8 @@ __global__ void __launch_bounds__(kThreadsWS, 1) k_render_ws3(const WsArgs a) {
 #pragma unroll
                 for (int i = 0; i < RW; ++i) back[i] = composite_ray(n, rw + kRW * i);
                 colours(n, back);
-                if (lane == 0) mbar_arrive(&sm.state_free[si]);       // group state, and the colour areas' loads have landed
+                __syncwarp();                                          // every lane's discards, before lane 0's release
+                if (lane == 0) mbar_arrive(&sm.state_free[si]);       // group state; the colour areas' loads landed, lines discarded
             }
         }
         RC_END(2, RC_TOTAL, rc_role);
