@@ -7,7 +7,9 @@
 * ``over_white``: PIL's integer ``Image.alpha_composite`` of a pixel over opaque white;
 * ``chain``: all of it, then ``to_tensor``'s float32 / 255;
 * ``png_file``, ``filter_rows`` and ``Deflate``: PNG files with chosen filters, zlib settings and IDAT splits, and
-  hand-built deflate streams (fixed / dynamic / stored blocks, any match) for what zlib never emits.
+  hand-built deflate streams (fixed / dynamic / stored blocks, any match) for what zlib never emits;
+* ``malformed_streams``, ``refusal_streams`` and ``path_streams``: streams for each refusal of the decoder and for the
+  valid paths zlib never takes.
 """
 from __future__ import annotations
 
@@ -241,27 +243,41 @@ class Deflate:
         self.bits(1, 2)
         self._tokens(list(tokens) + ([256] if eob else []), canonical(FIXED_LIT), FIXED_LIT, canonical([5] * 32), [5] * 32)
 
-    def dynamic(self, tokens, llens, dlens, final=False, cllens=None):
+    def dynamic(self, tokens, llens, dlens, final=False, cllens=None, clsyms=None, hclen=19):
         """A dynamic block with the given code lengths (hlit = len(llens), hdist = len(dlens)), each length written as
-        its own code-length symbol under a 4-bit code for 0..15 unless `cllens` (19 lengths) says otherwise."""
+        its own code-length symbol under a 4-bit code for 0..15 unless `cllens` (19 lengths) says otherwise.
+        `clsyms` replaces that sequence: ints are symbols (16-18 without their repeat bits), (symbol, repeat) pairs
+        are repeat codes.  Only the first `hclen` code-length lengths are written.  `tokens=None` ends the block after
+        the code lengths (for malformed and truncated headers)."""
         self.bits(int(final), 1)
         self.bits(2, 2)
         cl = cllens if cllens is not None else [4] * 16 + [0] * 3
         self.bits(len(llens) - 257, 5)
         self.bits(len(dlens) - 1, 5)
         self.bits(19 - 4, 4)
-        for i in CLORDER:
+        for i in CLORDER[:hclen]:
             self.bits(cl[i], 3)
+        if hclen < 19:
+            return
         clc = canonical(cl)
-        for l in list(llens) + list(dlens):
-            self.huff(clc[l], cl[l])
-        self._tokens(list(tokens) + [256], canonical(llens), llens, canonical(dlens), dlens)
+        for s in (list(llens) + list(dlens) if clsyms is None else clsyms):
+            sym, rep = (s, None) if isinstance(s, int) else s
+            self.huff(clc[sym], cl[sym])
+            if rep is not None:
+                self.bits(rep - (11 if sym == 18 else 3), {16: 2, 17: 3, 18: 7}[sym])
+        if tokens is not None:
+            self._tokens(list(tokens) + [256], canonical(llens), llens, canonical(dlens), dlens)
 
     def zlib(self, cmf=0x78, flg=None, adler=None):
         self.align()
         if flg is None:
             flg = (31 - (cmf * 256) % 31) % 31
         return bytes([cmf, flg]) + bytes(self.out) + struct.pack('>I', zlib.adler32(bytes(self.raw)) if adler is None else adler)
+
+    def cut(self):
+        """The zlib header and the bits written so far, no trailer: a stream that ends here (the last byte's unwritten
+        bits are zeros)."""
+        return bytes([0x78, 0x9c]) + bytes(self.out) + (bytes([self.acc]) if self.n else b'')
 
 
 def lit_lengths_286():
@@ -354,4 +370,159 @@ def malformed_streams():
     res['truncated_adler'] = (good[:-2], n, 9)
     res['empty_stream'] = (b'', n, 9)
     res['bad_adler'] = (good[:-1] + bytes([good[-1] ^ 0x40]), n, 10)
+    return res
+
+
+CL_ALL = [4] * 13 + [5] * 6                      # a complete code-length code over all 19 symbols, 16-18 included
+DIST_30 = [4, 4] + [5] * 28                      # a complete distance code over all 30 symbols
+
+
+def _fixed_aligned(tokens_after):
+    """A fixed block of k 9-bit literals (200) and then `tokens_after`, with k in 0..7 chosen so the block's bits end on
+    a byte boundary: the stream can be cut right there.  Returns the Deflate."""
+    for k in range(8):
+        d = Deflate()
+        d.bits(0, 1)
+        d.bits(1, 2)
+        lc = canonical(FIXED_LIT)
+        for _ in range(k):
+            d.huff(lc[200], 9)
+        tokens_after(d, lc)
+        if d.n == 0:
+            return d
+    raise AssertionError('no alignment')
+
+
+def refusal_streams():
+    """Malformed streams that reach the decoder's refusal sites malformed_streams() leaves out: name -> (zlib stream,
+    bytes the image should inflate to, the P3D_PNG_* status).  tests/test_png_decode_paths_cpu.py maps each to the
+    source line that refuses it."""
+    n = 64
+    raw = bytes([0]) + bytes(range(1, n))
+    good = zlib.compress(raw)
+    res = {}
+    d = Deflate()
+    d.dynamic(list(raw), [8] * 287, [1], final=True)                   # HLIT = 287
+    res['hlit_287'] = (d.zlib(), n, 4)
+    d = Deflate()
+    d.dynamic(list(raw), lit_lengths_286(), [5] * 31, final=True)      # HDIST = 31
+    res['hdist_31'] = (d.zlib(), n, 4)
+    d = Deflate()
+    d.dynamic(None, lit_lengths_286(), [1], final=True, hclen=5)       # 17 + 15 bits: the cut is on a byte
+    res['truncated_in_code_length_lengths'] = (d.cut(), n, 9)
+    d = Deflate()
+    d.dynamic(None, lit_lengths_286(), [1], final=True, clsyms=[8])    # 74 + 4 bits: 2 bits left for a 4-bit code
+    res['truncated_in_code_lengths'] = (d.cut(), n, 9)
+    d = Deflate()
+    d.dynamic(None, lit_lengths_286(), [1], final=True, cllens=[0] * 8 + [1] + [0] * 10, clsyms=[8])
+    d.bits(1, 1)                                                       # no code of the one-code code-length code
+    res['code_length_symbol_outside_the_code'] = (d.zlib(), n, 4)
+    d = Deflate()
+    d.dynamic(list(raw), lit_lengths_286(), [1], final=True, cllens=CL_ALL, clsyms=[(16, 3)] + [8] * 283 + [1])
+    res['repeat_16_first'] = (d.zlib(), n, 4)
+    d = Deflate()
+    d.dynamic(None, lit_lengths_286(), [1], final=True, cllens=CL_ALL, clsyms=[18])   # 74 + 5 bits: 1 of 7 repeat bits
+    res['truncated_in_repeat_bits'] = (d.cut(), n, 9)
+    d = Deflate()
+    d.dynamic(list(raw), [8] * 256 + [1], [1], final=True, cllens=CL_ALL, clsyms=[(18, 138), (18, 138)])
+    res['repeat_past_hlit_hdist'] = (d.zlib(), n, 4)
+    d = Deflate()
+    d.fixed([0, 1], final=True, eob=False)
+    d.huff(canonical(FIXED_LIT)[257], 7)                              # a match of 3 ...
+    d.huff(canonical([5] * 32)[30], 5)                                 # ... at distance symbol 30
+    res['fixed_distance_symbol_30'] = (d.zlib(), n, 5)
+    d = Deflate()
+    d.fixed([0, 1], final=True, eob=False)
+    d.huff(canonical(FIXED_LIT)[257], 7)
+    d.huff(canonical([5] * 32)[31], 5)
+    res['fixed_distance_symbol_31'] = (d.zlib(), n, 5)
+    d = Deflate()
+    d.dynamic(None, [0] * 256 + [1], [0], final=True)                  # one literal/length code: end-of-block, '0'
+    d.bits(1, 1)
+    res['literal_bits_outside_a_one_code_code'] = (d.zlib(), n, 5)
+    d = Deflate()
+    d.fixed(list(raw[:-1]) + [(3, 2)], final=True)                     # 63 bytes, then a match of 3
+    res['too_long_by_a_match'] = (d.zlib(), n, 7)
+    d = Deflate()
+    d.stored(raw + b'x', final=True)
+    res['too_long_by_a_stored_block'] = (d.zlib(), n, 7)
+    d = Deflate()
+    d.stored(raw, final=True)
+    res['stored_len_past_the_input'] = (d.cut()[:-10], n, 9)
+    d = Deflate()
+    d.bits(1, 1)
+    d.bits(0, 2)
+    d.align()
+    d.bits(n, 16)                                                      # LEN, and the stream ends before NLEN
+    res['truncated_in_stored_len_nlen'] = (d.cut(), n, 9)
+    res['truncated_after_the_zlib_header'] = (good[:2], n, 9)
+
+    def match_len3(d, lc):
+        d.huff(lc[0], 8)
+        d.huff(lc[257], 7)
+    res['truncated_before_a_distance_code'] = (_fixed_aligned(match_len3).cut(), n, 9)
+
+    def match_dist29(d, lc):
+        match_len3(d, lc)
+        d.huff(29, 5)
+    res['truncated_in_distance_extra_bits'] = (_fixed_aligned(match_dist29).cut(), n, 9)
+    return res
+
+
+def _with_swaps(lens, pairs):
+    lens = list(lens)
+    for a, b in pairs:
+        lens[a], lens[b] = lens[b], lens[a]
+    return lens
+
+
+def path_streams():
+    """Valid streams along the decoder's rarer paths, each a one-row grey image: name -> (h, w, c, depth, zlib stream,
+    raw).  Block sequences zlib never writes with matches across every seam, 15-bit literal and distance codes at
+    HLIT = 286 / HDIST = 30, a repeat 16 that crosses from the literal into the distance lengths, and a repeat 18 of 138."""
+    g = np.random.default_rng(21)
+    res = {}
+
+    def lits(k, pool=None):
+        return [int(v) for v in (g.integers(0, 256, k) if pool is None else g.choice(pool, k))]
+
+    d = Deflate()                      # dynamic -> fixed -> fixed -> dynamic -> stored -> fixed, every block opens with a
+    d.dynamic([0] + lits(120) + [(10, 7), (258, 100)], lit_lengths_286(), DIST_30)         # match across the seam
+    d.fixed([(258, 300)] + lits(50) + [(40, 3)])
+    d.fixed([(100, 90), (258, 700)] + lits(30) + [(258, 1)])
+    d.dynamic([(77, 333), (200, 1000)] + lits(40) + [(258, 2)], lit_lengths_286()[::-1], DIST_30[::-1])
+    d.stored(bytes(lits(300)))
+    d.fixed([(258, 320), (258, 1500)] + lits(17) + [(5, 2000)], final=True)
+    raw = bytes(d.raw)
+    res['dynamic_fixed_fixed_dynamic_stored_fixed'] = (1, len(raw) - 1, 1, 8, d.zlib(), raw)
+
+    # 232 x 8 + 47 x 9 bits and a chain 10 .. 15, 15: complete; literal 7 and length symbol 270 get the 15-bit codes
+    llens = _with_swaps([8] * 232 + [9] * 47 + list(range(10, 16)) + [15], [(7, 284), (270, 285)])
+    # 12 x 4 + 7 x 5 bits and a chain 6 .. 15, 15: complete; distance symbols 2 and 29 get the 15-bit codes
+    dlens = _with_swaps([4] * 12 + [5] * 7 + list(range(6, 16)) + [15], [(2, 28)])
+    assert len(llens) == 286 and len(dlens) == 30 and max(llens) == max(dlens) == 15
+    toks = [0] + lits(3000, [7, 7, 7, 8, 9, 200, 255]) + lits(23000) + [(24, 3), (25, 4), (30, 24600), (258, 24577),
+                                                                        (23, 3), 7, (26, 26000), 7, (258, 1)]
+    d = Deflate()
+    d.dynamic(toks, llens, dlens, final=True)
+    raw = bytes(d.raw)
+    res['hlit_286_hdist_30_15_bit_codes'] = (1, len(raw) - 1, 1, 8, d.zlib(), raw)
+
+    # literal/length symbols 283-285 and distance symbols 0-3 all of 5 bits: one repeat 16 of 6 spans the two lists
+    llens = [8] * 181 + [9] * 102 + [5] * 3
+    dlens = [5] * 28 + [4] * 2
+    d = Deflate()
+    d.dynamic([0] + lits(300) + [(200, 3), (230, 1), (258, 4)] + lits(20) + [(258, 2), (3, 1)], llens, dlens, final=True,
+              cllens=CL_ALL, clsyms=llens[:284] + [(16, 6)] + dlens[4:])
+    raw = bytes(d.raw)
+    res['repeat_16_across_the_two_lists'] = (1, len(raw) - 1, 1, 8, d.zlib(), raw)
+
+    # literals 100-237 unused: one repeat 18 of 138 zeros
+    llens = [7] * 100 + [0] * 138 + [7] * 8 + [8] * 40
+    pool = list(range(100)) + list(range(238, 256))
+    d = Deflate()
+    d.dynamic([0] + lits(400, pool) + [(258, 33), (4, 1)] + lits(9, pool), llens, DIST_30, final=True, cllens=CL_ALL,
+              clsyms=llens[:100] + [(18, 138)] + llens[238:] + DIST_30)
+    raw = bytes(d.raw)
+    res['repeat_18_of_138'] = (1, len(raw) - 1, 1, 8, d.zlib(), raw)
     return res

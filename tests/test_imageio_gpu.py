@@ -28,6 +28,30 @@ def test_scanlines_equal_the_oracle_byte_for_byte(n, c, h, w):
         assert np.array_equal(got, want)
 
 
+def test_special_values_and_filter_ties():
+    """NaN -> 0, +-inf clamped, -0 -> 0, 1 -> 255 and 0.99999994 -> 254 (truncation, not rounding), in both kernels; and
+    rows where filters tie (an all-zero first row: every sum 0; constant rows: Up and Paeth both 0), which go to the
+    first minimum in the order none, sub, up, average, paeth."""
+    import panic3d_b200.imageio as pio
+    special = torch.tensor([float('nan'), float('inf'), float('-inf'), -0.0, 1.0, 0.99999994, 0.5, -1e-30, 2.0, 0.2])
+    want = np.array([0, 255, 0, 0, 255, 254, 127, 0, 255, 51], np.uint8)
+    w = 40
+    img = torch.zeros(1, 3, 5, w)
+    img[0, :, 1] = special.repeat(4)[None].roll(1, 1) * torch.ones(3, 1)
+    img[0, 0, 1] = special.repeat(4)
+    img[0, :, 2] = 0.5
+    img[0, :, 3] = 0.5
+    img[0, :, 4] = torch.linspace(0, 1, w)
+    pix = io_orc.quantize(torch.nan_to_num(img, nan=0.0))
+    assert np.array_equal(pix[0, 1, :, 0], np.tile(want, 4))
+    assert np.array_equal(pio.to_uint8(img.to(DEV)).cpu().numpy(), pix)
+    scan, _ = pio.png_scanlines(img.to(DEV))
+    got = scan[0].cpu().numpy().reshape(5, 1 + w * 3)
+    ref = io_orc.png_filter_rows(pix[0])
+    assert list(ref[:, 0][[0, 3]]) == [0, 2]
+    assert np.array_equal(got, ref)
+
+
 def test_rows_beyond_the_shared_memory_staging_use_filter_none():
     import panic3d_b200.imageio as pio
     img = torch.rand(1, 4, 2, 30000)
