@@ -16,6 +16,9 @@ discriminator, conv2d_gradfix - is the reference's code.  Two arms, one process 
 
     --arm reference   the unmodified modules: eager PyTorch renderer + the reference's JIT plugins (bias_act, upfirdn2d)
     --arm ours        panic3d_b200.dropin.install(): our renderer (forward + backward, run_model backward) and the three ops
+    --conv2d          (with --arm ours) also dropin.install_conv2d(): conv2d_gradfix's fp32 calls on the 3xTF32 kernels
+                      where conv.measured_faster admits them
+    --profile         one more iteration under torch.profiler: the convolutions' share of the step's kernel time
 
 Prints one JSON line with ms per phase (CUDA events, median of --iters) and, with --check, gradient statistics so the two
 arms can be compared (same seeds -> same weights and the same latents; the renderer's jitter differs, so losses agree
@@ -25,12 +28,42 @@ from __future__ import annotations
 import argparse
 import json
 import os
+import re
 import statistics
 import sys
 import types
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 REF_TREE = os.path.join(ROOT, 'baseline', '_ref')
+
+
+# Kernel names of convolutions: cuDNN's forward / data-gradient / weight-gradient kernels (implicit GEMM, Winograd, FFT) and
+# panic3d_b200.conv's.  Anything else (GEMMs of the mapping and FC layers, elementwise ops, the renderer) is not a conv.
+CONV_KERNEL = re.compile(r'conv|fprop|dgrad|wgrad|winograd|fft|k_weight_kmajor|k_split_sum', re.I)
+
+
+def conv_share(phases, modules):
+    """One iteration of the phases under torch.profiler (CUDA activity): device time of every kernel, the part in
+    convolution kernels (CONV_KERNEL), and the ten largest convolution kernels by time."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    for m in modules:
+        for p_ in m.parameters():
+            p_.grad = None
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _, fn in phases:
+            fn()
+        torch.cuda.synchronize()
+    per_kernel = {}
+    for e in prof.events():
+        if e.device_type == torch.autograd.DeviceType.CUDA:
+            per_kernel[e.name] = per_kernel.get(e.name, 0.0) + e.time_range.elapsed_us() / 1e3
+    total = sum(per_kernel.values())
+    conv = {k: v for k, v in per_kernel.items() if CONV_KERNEL.search(k)}
+    conv_ms = sum(conv.values())
+    top = sorted(conv.items(), key=lambda kv: -kv[1])[:10]
+    return {'kernel_ms': total, 'conv_ms': conv_ms, 'conv_share': conv_ms / total if total else None,
+            'top_conv_kernels': [[k[:120], v] for k, v in top]}
 
 
 def main():
@@ -44,7 +77,13 @@ def main():
                     help="training mode 'Agrad' (loss_orthocondA.py:146-150): G.f pastes the front image with grad_sample=True, so Gmain "
                          'back-propagates through paste_front into image_xyz; thresholds are permissive so that a random-weight generator '
                          'yields a non-empty mask')
+    ap.add_argument('--conv2d', action='store_true', help='with --arm ours: also install_conv2d() (panic3d_b200.conv)')
+    ap.add_argument('--profile', action='store_true',
+                    help='after the timed iterations, run the four phases once more under torch.profiler and report the '
+                         "convolutions' share of the step's kernel time")
     args = ap.parse_args()
+    if args.conv2d and args.arm != 'ours':
+        ap.error('--conv2d needs --arm ours')
     sys.path.insert(0, ROOT)
     from baseline import ref_env
     ref_env.setup()
@@ -64,6 +103,8 @@ def main():
     from training.dual_discriminator import DualDiscriminator
     from torch_utils.ops import conv2d_gradfix
     conv2d_gradfix.enabled = True                               # training_loop_v0.py:143
+    if args.conv2d:
+        dropin.install_conv2d(conv2d_gradfix)
     torch.backends.cuda.matmul.allow_tf32 = False               # :141-142
     torch.backends.cudnn.allow_tf32 = False
     mod_file = sys.modules[tp.ImportanceRenderer.__module__].__file__
@@ -173,6 +214,9 @@ def main():
                 torch.cuda.synchronize()
                 if it > 0:
                     times[name].append(e0.elapsed_time(e1))
+    prof_line = None
+    if args.profile and cuda:
+        prof_line = conv_share(phases, (G, D))
     # gradient statistics after a final Gmain + Greg (both arms should agree up to the renderer's jitter)
     for p_ in G.parameters():
         p_.grad = None
@@ -183,11 +227,14 @@ def main():
         gs = [p_.grad.float().norm().item() for p_ in mod.parameters() if p_.grad is not None]
         gstat[key] = {'n_tensors_with_grad': len(gs), 'grad_norm': float(np.sqrt(sum(x * x for x in gs)))}
     line = {'config': 'BASELINE configs[4]: training phases on synthetic 512^2 data (batch %d, R=%d, 48+48)' % (B, R), 'arm': args.arm,
+            'conv2d': args.conv2d,
             'ms': {n: (statistics.median(v) if v else None) for n, v in times.items()},
             'ms_total': (sum(statistics.median(v) for v in times.values()) if cuda else None),
             'renderer_module': mod_file.replace(ROOT, '.'), 'grads': gstat}
     if args.paste:
         line['paste'] = {'params': paste_params, 'mask_mean': last.get('mask_mean')}
+    if prof_line is not None:
+        line['profile'] = prof_line
     if args.arm == 'ours':
         from panic3d_b200 import _lib
         line['gpu_launches'] = _lib.launch_count()

@@ -97,6 +97,25 @@ def install_modconv(module=None):
     return names
 
 
+def install_conv2d(module=None):
+    """Rebind ``conv2d`` and ``conv_transpose2d`` of the reference's ``torch_utils.ops.conv2d_gradfix`` to
+    ``panic3d_b200.conv`` (the fp32 training convolutions in 3xTF32 on the tensor cores).  ``conv2d_resample`` looks both
+    up on that module at call time, so no caller changes.  Calls the kernels do not cover, or where they did not measure
+    faster than cuDNN (``conv.measured_faster``), run the originals, which stay reachable as ``_p3d_reference_conv2d`` /
+    ``_p3d_reference_conv_transpose2d``.  ``module``: the already-imported module (default: import it by that name).
+    Returns the names that were rebound."""
+    from . import conv
+    if module is None:
+        module = importlib.import_module('torch_utils.ops.conv2d_gradfix')
+    names = ['conv2d', 'conv_transpose2d']
+    for name in names:
+        if not hasattr(module, '_p3d_reference_' + name):
+            setattr(module, '_p3d_reference_' + name, getattr(module, name))     # keep the original reachable for A/B runs
+        setattr(module, name, getattr(conv, name))
+    conv._gradfix = module
+    return names
+
+
 def patch_generator(G):
     """For a TriPlaneGenerator that was built BEFORE install() (e.g. unpickled): swap its two hot-path
     sub-modules in place.  Both are parameter-free, so no weights move."""
